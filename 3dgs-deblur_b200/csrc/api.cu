@@ -33,6 +33,10 @@ bool blend_packed() {
     static const bool on = [] { const char *e = getenv("B200_BLEND_PACKED"); return !(e && e[0] == '0'); }();
     return on;
 }
+bool blend_tile_order() {
+    static const bool on = [] { const char *e = getenv("B200_BLEND_TILE_ORDER"); return !(e && e[0] == '0'); }();
+    return on;
+}
 }  // namespace b200
 #ifdef B200_BLEND_COUNTERS
 namespace b200 { __device__ unsigned long long g_blend_counters[16]; }

@@ -13,7 +13,8 @@
 //     transposing butterfly (generic kernel) instead of 13 x 5 shuffles; either way each sum ends on
 //     its own lane, so the 13 atomics issue as ONE predicated RED instruction instead of 13 serial
 //     ones from lane 0;
-//   * the same per-warp rectangle cull and TMA-bulk staged 64-byte records as the forward.
+//   * the same per-warp rectangle cull and TMA-bulk staged 64-byte records as the forward, and the same
+//     longest-list-first CTA order (blend_fwd.cu: tile_order_kernel).
 // Bound: FP32 issue, MUFU, LSU and L2 atomic throughput -- not HBM; see DESIGN.md section 4.
 #include "blend_common.cuh"
 
@@ -23,6 +24,7 @@ struct BlendBwdParams {
     BlendGeom g;
     const int32_t *ids_sorted;
     const int2 *tile_bins;
+    const int32_t *tile_order;  // CTA -> tile (b200_blend_tile_order), or null for raster order
     const PackedGaussian *packed;
     const float *background;
     const float *final_Ts;
@@ -70,7 +72,7 @@ __global__ void __launch_bounds__(BLEND_THREADS / PPL, PPL == 2 ? 5 : (PPL == 4 
     __shared__ int s_max[NT / 32];
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int tile = blockIdx.x;
+    const int tile = p.tile_order ? __ldg(p.tile_order + blockIdx.x) : (int)blockIdx.x;
     const int tile_x = tile % p.g.tbx, tile_y = tile / p.g.tbx;
     const int2 range = p.tile_bins[tile];
     const float inv_s = 1.0f / (float)S;
@@ -307,7 +309,7 @@ __global__ void __launch_bounds__(128, B200_BWD_MIN_CTAS) blend_backward_kernel2
 #endif
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int tile = blockIdx.x;
+    const int tile = p.tile_order ? __ldg(p.tile_order + blockIdx.x) : (int)blockIdx.x;
     const int tile_x = tile % p.g.tbx, tile_y = tile / p.g.tbx;
     const int2 range = p.tile_bins[tile];
     const float inv_s = 1.0f / (float)S;
@@ -587,7 +589,7 @@ static int run_blend_backward(int num_points, unsigned img_height, unsigned img_
                               const float *background, const float *final_Ts, const int32_t *final_idx,
                               const float *v_output, const float *v_output_alpha, float *v_xy, float *v_xy_abs,
                               float *v_pix_vels, float *v_conic, float *v_colors, float *v_opacity, bool outputs_are_zero,
-                              cudaStream_t st) {
+                              cudaStream_t st, const int32_t *tile_order = nullptr) {
     B200_REQUIRE(n_blur_samples > 0 && n_blur_samples <= B200_MAX_BLUR_SAMPLES, "unsupported blur size");
     B200_REQUIRE(num_points >= 1, "num_points must be >= 1");
     B200_REQUIRE(block_width > 1 && block_width <= 16, "block_width must be between 2 and 16");
@@ -610,6 +612,7 @@ static int run_blend_backward(int num_points, unsigned img_height, unsigned img_
                     (int)((img_height + block_width - 1) / block_width), rolling_shutter_time, exposure_time};
     p.ids_sorted = gaussian_ids_sorted;
     p.tile_bins = reinterpret_cast<const int2 *>(tile_bins);
+    p.tile_order = blend_tile_order() ? tile_order : nullptr;
     p.packed = reinterpret_cast<const PackedGaussian *>(packed);
     p.background = background;
     p.final_Ts = final_Ts; p.final_idx = final_idx; p.v_out = v_output; p.v_out_alpha = v_output_alpha;
@@ -640,6 +643,24 @@ extern "C" int b200_blend_backward_packed(int num_points, unsigned img_height, u
                               tile_bins, packed, rolling_shutter_time, exposure_time, background, final_Ts, final_idx,
                               v_output, v_output_alpha, v_xy, v_xy_abs, v_pix_vels, v_conic, v_colors, v_opacity,
                               outputs_are_zero != 0, as_stream(stream));
+}
+
+// b200_blend_backward_packed with the CTAs launched in `tile_order` (b200_blend_tile_order of the same tile_bins).  Only
+// the order in which CTAs add into the gradient arrays changes.
+extern "C" int b200_blend_backward_packed_ordered(int num_points, unsigned img_height, unsigned img_width,
+                                                  unsigned block_width, unsigned n_blur_samples,
+                                                  const int32_t *gaussian_ids_sorted, const int32_t *tile_bins,
+                                                  const void *packed, float rolling_shutter_time, float exposure_time,
+                                                  const float *background, const float *final_Ts, const int32_t *final_idx,
+                                                  const float *v_output, const float *v_output_alpha,
+                                                  const int32_t *tile_order, float *v_xy, float *v_xy_abs,
+                                                  float *v_pix_vels, float *v_conic, float *v_colors, float *v_opacity,
+                                                  int outputs_are_zero, void *stream) {
+    B200_REQUIRE(tile_order, "null tile_order pointer");
+    return run_blend_backward(num_points, img_height, img_width, block_width, n_blur_samples, gaussian_ids_sorted,
+                              tile_bins, packed, rolling_shutter_time, exposure_time, background, final_Ts, final_idx,
+                              v_output, v_output_alpha, v_xy, v_xy_abs, v_pix_vels, v_conic, v_colors, v_opacity,
+                              outputs_are_zero != 0, as_stream(stream), tile_order);
 }
 
 extern "C" int b200_rasterize_backward(int num_points, unsigned img_height, unsigned img_width, unsigned block_width,

@@ -13,6 +13,8 @@ constexpr int BLEND_STAGES = 2;
 int blend_pixels_per_lane(bool backward);
 // two-pixel kernels: float-pair form (default) or the scalar form (B200_BLEND_PACKED=0)
 bool blend_packed();
+// launch order of the blend CTAs: longest tile list first (default) or raster order (B200_BLEND_TILE_ORDER=0)
+bool blend_tile_order();
 
 // -DB200_BLEND_COUNTERS (A/B build only, see tools/blend_counters.py): the blend kernels count what they execute --
 //   [0] tile-list entries tested by a warp cull   [1] warp visits (entries that survive it)

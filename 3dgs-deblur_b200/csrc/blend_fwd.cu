@@ -9,7 +9,9 @@
 //   * each warp owns a compact 8x4 pixel block and first culls the staged batch against that
 //     rectangle (one Gaussian per lane + ballot), so only Gaussians that can reach alpha >= 1/255
 //     somewhere in the warp's pixels / sample times are evaluated.  The cull is conservative and the
-//     exact per-pixel tests of the reference are kept, so results do not change.
+//     exact per-pixel tests of the reference are kept, so results do not change;
+//   * CTA b blends tile tile_order[b], longest tile list first (tile_order_kernel below), so the costliest tiles start
+//     in the first wave instead of running alone at the end of the launch (DESIGN.md section 4).
 // Bound: FP32 issue + MUFU.EX2 (hundreds of flop per staged byte), not HBM -- see DESIGN.md.
 #include "blend_common.cuh"
 
@@ -19,6 +21,7 @@ struct BlendFwdParams {
     BlendGeom g;
     const int32_t *ids_sorted;
     const int2 *tile_bins;
+    const int32_t *tile_order;  // CTA -> tile (b200_blend_tile_order), or null for raster order
     const PackedGaussian *packed;
     const float *background;  // device float[3]
     float *out_img;           // (H,W,3)
@@ -49,7 +52,7 @@ __global__ void __launch_bounds__(BLEND_THREADS / PPL, PPL == 2 ? 6 : 1) blend_f
     __shared__ __align__(8) uint64_t s_bar[BLEND_STAGES];
 
     const int tid = threadIdx.x, lane = tid & 31;
-    const int tile = blockIdx.x;
+    const int tile = p.tile_order ? __ldg(p.tile_order + blockIdx.x) : (int)blockIdx.x;
     const int tile_x = tile % p.g.tbx, tile_y = tile / p.g.tbx;
     bool inside[PPL];
     float px[PPL], py[PPL], roll[PPL];
@@ -233,7 +236,7 @@ __global__ void __launch_bounds__(128, B200_FWD_MIN_CTAS) blend_forward_kernel2(
     __shared__ __align__(8) uint64_t s_bar[BLEND_STAGES];
 
     const int tid = threadIdx.x, lane = tid & 31;
-    const int tile = blockIdx.x;
+    const int tile = p.tile_order ? __ldg(p.tile_order + blockIdx.x) : (int)blockIdx.x;
     const int tile_x = tile % p.g.tbx, tile_y = tile / p.g.tbx;
     bool inside[2];
     float px[2], py[2], roll[2];
@@ -446,9 +449,68 @@ static int launch_fwd(const BlendFwdParams &p, cudaStream_t st) {
     return B200_OK;
 }
 
+// Launch order of the blend CTAs, longest tile list first.  Tile costs are uneven (the longest list is several times
+// the mean) and only ~6 CTAs fit on an SM, so in raster order the last waves leave SMs idle behind a few long tiles.
+// One CTA counting-sorts the tiles by list length into ORDER_BUCKETS buckets spanning [0, longest]: exact for lists
+// shorter than ORDER_BUCKETS entries, and within a bucket the order is whatever the atomics give.  The result is a
+// permutation of [0, num_tiles) whatever tile_bins holds, so the blend covers every tile exactly once.
+constexpr int ORDER_THREADS = 1024, ORDER_BUCKETS = 2048;
+static __global__ void __launch_bounds__(ORDER_THREADS) tile_order_kernel(int n, const int2 *__restrict__ bins,
+                                                                        int32_t *__restrict__ order) {
+    __shared__ int s_off[ORDER_BUCKETS];
+    __shared__ int s_warp[ORDER_THREADS / 32];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    auto len = [&](int t) {
+        const int2 r = bins[t];
+        return (int)min(max((long long)r.y - (long long)r.x, 0ll), 0x7fffffffll);
+    };
+    int mx = 0;
+    for (int t = tid; t < n; t += ORDER_THREADS) mx = max(mx, len(t));
+    mx = __reduce_max_sync(0xffffffffu, mx);
+    if (lane == 0) s_warp[warp] = mx;
+    for (int i = tid; i < ORDER_BUCKETS; i += ORDER_THREADS) s_off[i] = 0;
+    __syncthreads();
+    mx = 0;
+#pragma unroll
+    for (int w = 0; w < ORDER_THREADS / 32; ++w) mx = max(mx, s_warp[w]);
+    const long long span = max(mx, 1);
+    auto bucket = [&](int l) { return (int)((long long)(mx - l) * (ORDER_BUCKETS - 1) / span); };  // 0 = longest
+    for (int t = tid; t < n; t += ORDER_THREADS) atomicAdd(&s_off[bucket(len(t))], 1);
+    __syncthreads();
+    // exclusive scan of the bucket counts: thread i owns buckets 2i and 2i + 1
+    static_assert(ORDER_BUCKETS == 2 * ORDER_THREADS, "two buckets per thread");
+    const int c0 = s_off[2 * tid], c1 = s_off[2 * tid + 1];
+    int incl = c0 + c1;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const int v = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += v;
+    }
+    __syncthreads();  // s_warp is reused for the warp totals
+    if (lane == 31) s_warp[warp] = incl;
+    __syncthreads();
+    int base = 0;
+    for (int w = 0; w < warp; ++w) base += s_warp[w];
+    const int excl = base + incl - c0 - c1;
+    s_off[2 * tid] = excl;
+    s_off[2 * tid + 1] = excl + c0;
+    __syncthreads();
+    for (int t = tid; t < n; t += ORDER_THREADS) order[atomicAdd(&s_off[bucket(len(t))], 1)] = t;
+}
+
 }  // namespace b200
 
 using namespace b200;
+
+extern "C" int b200_blend_tile_order(int num_tiles, const int32_t *tile_bins, int32_t *tile_order, void *stream) {
+    B200_REQUIRE(num_tiles >= 1, "num_tiles must be >= 1");
+    B200_REQUIRE(tile_bins && tile_order, "null pointer");
+    if (!blend_tile_order()) return B200_OK;  // raster order: the blend entry points ignore tile_order
+    tile_order_kernel<<<1, ORDER_THREADS, 0, as_stream(stream)>>>(num_tiles, reinterpret_cast<const int2 *>(tile_bins),
+                                                                   tile_order);
+    B200_LAUNCH_CHECK();
+    return B200_OK;
+}
 
 extern "C" size_t b200_packed_record_bytes(void) { return sizeof(PackedGaussian); }
 
@@ -456,7 +518,7 @@ static int run_blend_forward(unsigned img_height, unsigned img_width, unsigned b
                              const int32_t *gaussian_ids_sorted, const int32_t *tile_bins, const void *packed,
                              float rolling_shutter_time, float exposure_time, const float *background, float *out_img,
                              float *final_Ts, int32_t *final_idx, float *out_alpha, cudaStream_t st,
-                             const int32_t *ref_isect = nullptr) {
+                             const int32_t *ref_isect = nullptr, const int32_t *tile_order = nullptr) {
     B200_REQUIRE(n_blur_samples > 0 && n_blur_samples <= B200_MAX_BLUR_SAMPLES, "unsupported blur size");  // bindings.cu:450-452
     B200_REQUIRE(block_width > 1 && block_width <= 16, "block_width must be between 2 and 16");
     B200_REQUIRE(img_height > 0 && img_width > 0, "image size must be positive");
@@ -469,6 +531,7 @@ static int run_blend_forward(unsigned img_height, unsigned img_width, unsigned b
                     (int)((img_height + block_width - 1) / block_width), rolling_shutter_time, exposure_time};
     p.ids_sorted = gaussian_ids_sorted;
     p.tile_bins = reinterpret_cast<const int2 *>(tile_bins);
+    p.tile_order = blend_tile_order() ? tile_order : nullptr;
     p.packed = reinterpret_cast<const PackedGaussian *>(packed);
     p.background = background;
     p.out_img = out_img; p.final_Ts = final_Ts; p.final_idx = final_idx; p.out_alpha = out_alpha;
@@ -538,6 +601,20 @@ extern "C" int b200_blend_forward_packed_status(unsigned img_height, unsigned im
     return run_blend_forward(img_height, img_width, block_width, n_blur_samples, gaussian_ids_sorted, tile_bins, packed,
                              rolling_shutter_time, exposure_time, background, out_img, final_Ts, final_idx, out_alpha,
                              as_stream(stream), status + 3);
+}
+
+// b200_blend_forward_packed / _status with the CTAs launched in `tile_order` (b200_blend_tile_order of the same
+// tile_bins); `status` may be null.  The order changes no output bit: every tile is blended on its own.
+extern "C" int b200_blend_forward_packed_ordered(unsigned img_height, unsigned img_width, unsigned block_width,
+                                                 unsigned n_blur_samples, const int32_t *gaussian_ids_sorted,
+                                                 const int32_t *tile_bins, const void *packed, float rolling_shutter_time,
+                                                 float exposure_time, const float *background, const int32_t *status,
+                                                 const int32_t *tile_order, float *out_img, float *final_Ts,
+                                                 int32_t *final_idx, float *out_alpha, void *stream) {
+    B200_REQUIRE(tile_order, "null tile_order pointer");
+    return run_blend_forward(img_height, img_width, block_width, n_blur_samples, gaussian_ids_sorted, tile_bins, packed,
+                             rolling_shutter_time, exposure_time, background, out_img, final_Ts, final_idx, out_alpha,
+                             as_stream(stream), status ? status + 3 : nullptr, tile_order);
 }
 
 namespace b200 {

@@ -43,6 +43,10 @@ SIGNATURES = {
     "b200_blend_forward_packed": (_i, [_u, _u, _u, _u, _p, _p, _p, _f, _f, _p, _p, _p, _p, _p, _p]),
     "b200_blend_backward_packed": (_i, [_i, _u, _u, _u, _u, _p, _p, _p, _f, _f, _p, _p, _p, _p, _p,
                                         _p, _p, _p, _p, _p, _p, _i, _p]),
+    "b200_blend_tile_order": (_i, [_i, _p, _p, _p]),
+    "b200_blend_forward_packed_ordered": (_i, [_u, _u, _u, _u, _p, _p, _p, _f, _f, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "b200_blend_backward_packed_ordered": (_i, [_i, _u, _u, _u, _u, _p, _p, _p, _f, _f, _p, _p, _p, _p, _p, _p,
+                                                _p, _p, _p, _p, _p, _p, _i, _p]),
     "b200_fused_preprocess_forward": (_i, [_i, _p, _p, _p, _p, _p, _p, _i, _i, _p, _p, _p, _p, _f, _f, _f, _f, _f, _f, _u, _u, _u,
                                            _f, _p, _p, _p, _p, _p]),
     "b200_fused_geometry_forward": (_i, [_i, _p, _p, _p, _p, _p, _p, _p, _f, _f, _f, _f, _f, _f, _u, _u, _u, _f, _p, _p, _p, _p, _p]),

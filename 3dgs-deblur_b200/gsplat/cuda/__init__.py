@@ -329,16 +329,12 @@ def blend_forward_packed(img_height, img_width, block_width, n_blur_samples, gau
         final_Ts = torch.empty((H, W, S), dtype=torch.float32, device=dev)
         final_idx = torch.empty((H, W, S), dtype=torch.int32, device=dev)
         alpha = torch.empty((H, W), dtype=torch.float32, device=dev) if want_alpha else None
-        if status is not None:  # capacity-mode lists: the reference's empty-render branch is taken on the device
-            check(_lib.load().b200_blend_forward_packed_status(
-                H, W, int(block_width), S, ptr(gaussian_ids_sorted), ptr(tile_bins), ptr(packed), float(rolling_shutter_time),
-                float(exposure_time), ptr(_f32(background)), ptr(status), ptr(out_img), ptr(final_Ts), ptr(final_idx), ptr(alpha),
-                stream()))
-        else:
-            check(_lib.load().b200_blend_forward_packed(H, W, int(block_width), S, ptr(gaussian_ids_sorted), ptr(tile_bins),
-                                                        ptr(packed), float(rolling_shutter_time), float(exposure_time),
-                                                        ptr(_f32(background)), ptr(out_img), ptr(final_Ts), ptr(final_idx),
-                                                        ptr(alpha), stream()))
+        # with `status` (capacity-mode lists) the reference's empty-render branch is taken on the device
+        order = _tile_order(tile_bins, H, W, int(block_width))
+        check(_lib.load().b200_blend_forward_packed_ordered(
+            H, W, int(block_width), S, ptr(gaussian_ids_sorted), ptr(tile_bins), ptr(packed), float(rolling_shutter_time),
+            float(exposure_time), ptr(_f32(background)), ptr(status), ptr(order), ptr(out_img), ptr(final_Ts), ptr(final_idx),
+            ptr(alpha), stream()))
     if want_alpha:
         return out_img, final_Ts, final_idx, alpha
     return out_img, final_Ts, final_idx
@@ -362,12 +358,21 @@ def blend_backward_packed(num_points, img_height, img_width, block_width, n_blur
         v_xy, v_xy_abs, v_pix = (acc[k * 2 * pitch:k * 2 * pitch + 2 * n].view(n, 2) for k in range(3))
         v_conic, v_colors = (acc[6 * pitch + k * 3 * pitch:6 * pitch + k * 3 * pitch + 3 * n].view(n, 3) for k in range(2))
         v_opacity = acc[12 * pitch:12 * pitch + n].view(n, 1)
-        check(_lib.load().b200_blend_backward_packed(
+        order = _tile_order(tile_bins, int(img_height), int(img_width), int(block_width))
+        check(_lib.load().b200_blend_backward_packed_ordered(
             n, int(img_height), int(img_width), int(block_width), int(n_blur_samples), ptr(gaussian_ids_sorted),
             ptr(tile_bins), ptr(packed), float(rolling_shutter_time), float(exposure_time), ptr(_f32(background)),
-            ptr(_f32(final_Ts)), ptr(final_idx), ptr(v_output), ptr(v_output_alpha), ptr(v_xy), ptr(v_xy_abs), ptr(v_pix),
-            ptr(v_conic), ptr(v_colors), ptr(v_opacity), 1, stream()))
+            ptr(_f32(final_Ts)), ptr(final_idx), ptr(v_output), ptr(v_output_alpha), ptr(order), ptr(v_xy), ptr(v_xy_abs),
+            ptr(v_pix), ptr(v_conic), ptr(v_colors), ptr(v_opacity), 1, stream()))
     return v_xy, v_xy_abs, v_pix, v_conic, v_colors, v_opacity
+
+
+def _tile_order(tile_bins, H, W, bw):
+    """Scratch int32[num_tiles] holding the blend's CTA -> tile order (longest list first), computed on the device."""
+    tiles = ((W + bw - 1) // bw) * ((H + bw - 1) // bw)
+    order = torch.empty((tiles,), dtype=torch.int32, device=tile_bins.device)
+    check(_lib.load().b200_blend_tile_order(tiles, ptr(tile_bins), ptr(order), stream()))
+    return order
 
 
 def _geom(tile_bounds, block, img_size):

@@ -191,6 +191,30 @@ B200_API int b200_blend_backward_packed(int num_points, unsigned img_height, uns
                                         float *v_xy, float *v_xy_abs, float *v_pix_vels, float *v_conic,
                                         float *v_colors, float *v_opacity, int outputs_are_zero, void *stream);
 
+/* Launch order of the blend CTAs.  b200_blend_tile_order writes tile_order (int32[num_tiles], num_tiles = tiles_x *
+ * tiles_y): a permutation of the tiles, longest tile_bins range first, so the costliest tiles start in the first wave
+ * instead of trailing the launch.  The _ordered blend entry points run one CTA per tile in that order and otherwise
+ * equal b200_blend_forward_packed_status (status may be null: no empty-render branch) and b200_blend_backward_packed:
+ * the forward's outputs are bit-identical, the backward's differ only by the order of float atomics.
+ * B200_BLEND_TILE_ORDER=0 in the environment restores raster order: b200_blend_tile_order then writes nothing and the
+ * _ordered entry points ignore tile_order. */
+B200_API int b200_blend_tile_order(int num_tiles, const int32_t *tile_bins, int32_t *tile_order, void *stream);
+B200_API int b200_blend_forward_packed_ordered(unsigned img_height, unsigned img_width, unsigned block_width,
+                                               unsigned n_blur_samples, const int32_t *gaussian_ids_sorted,
+                                               const int32_t *tile_bins, const void *packed, float rolling_shutter_time,
+                                               float exposure_time, const float *background, const int32_t *status,
+                                               const int32_t *tile_order, float *out_img, float *final_Ts,
+                                               int32_t *final_idx, float *out_alpha, void *stream);
+B200_API int b200_blend_backward_packed_ordered(int num_points, unsigned img_height, unsigned img_width,
+                                                unsigned block_width, unsigned n_blur_samples,
+                                                const int32_t *gaussian_ids_sorted, const int32_t *tile_bins,
+                                                const void *packed, float rolling_shutter_time, float exposure_time,
+                                                const float *background, const float *final_Ts, const int32_t *final_idx,
+                                                const float *v_output, const float *v_output_alpha,
+                                                const int32_t *tile_order, float *v_xy, float *v_xy_abs,
+                                                float *v_pix_vels, float *v_conic, float *v_colors, float *v_opacity,
+                                                int outputs_are_zero, void *stream);
+
 /* ---- blend (blur + rolling shutter), 3 channels ------------------------------------------
  * replaces rasterize_forward_tensor (bindings.h:110-127, bindings.cu:424-503; kernel forward.cu:306-456).
  * packed_ws: scratch of num_points * b200_packed_record_bytes() bytes, 16-byte aligned (filled here).
