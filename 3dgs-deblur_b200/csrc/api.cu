@@ -21,21 +21,12 @@ static std::atomic<long long> g_launches{0};
 void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 }  // namespace b200
 namespace b200 {
-// Two pixels per lane (default) halve the per-(warp, Gaussian) visit costs: pixels evaluated side by side with masked
-// updates, 96 registers, 5 CTAs per SM (tools/blend_probe.py times the variants).
-// B200_BLEND_PPL_FWD / B200_BLEND_PPL_BWD = 1 select the one-pixel kernels, 4 the experimental four-pixel ones.
-int blend_pixels_per_lane(bool backward) {
-    static const int fwd = [] { const char *e = getenv("B200_BLEND_PPL_FWD"); return (e && e[0] == '1') ? 1 : (e && e[0] == '4') ? 4 : 2; }();
-    static const int bwd = [] { const char *e = getenv("B200_BLEND_PPL_BWD"); return (e && e[0] == '1') ? 1 : (e && e[0] == '4') ? 4 : 2; }();
+// Test switch, read once per process: B200_BLEND_PPL_FWD=1 / B200_BLEND_PPL_BWD=1 run the one-pixel blend kernels on
+// 16x16 tiles, where the paired kernels run otherwise, so the tests can check them on 16-wide scenes.
+bool blend_force_one_pixel(bool backward) {
+    static const bool fwd = [] { const char *e = getenv("B200_BLEND_PPL_FWD"); return e && e[0] == '1'; }();
+    static const bool bwd = [] { const char *e = getenv("B200_BLEND_PPL_BWD"); return e && e[0] == '1'; }();
     return backward ? bwd : fwd;
-}
-bool blend_packed() {
-    static const bool on = [] { const char *e = getenv("B200_BLEND_PACKED"); return !(e && e[0] == '0'); }();
-    return on;
-}
-bool blend_tile_order() {
-    static const bool on = [] { const char *e = getenv("B200_BLEND_TILE_ORDER"); return !(e && e[0] == '0'); }();
-    return on;
 }
 }  // namespace b200
 #ifdef B200_BLEND_COUNTERS

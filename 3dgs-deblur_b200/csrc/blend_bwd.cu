@@ -10,7 +10,7 @@
 //     reduction: S x fewer shuffles and atomics than backward.cu:334-365;
 //   * the 13 per-Gaussian sums of a visit are reduced over the warp through a shared-memory
 //     transposition (paired kernel: 13 STS + 4 LDS.128 + 7 paired adds + 1 shuffle) or a 16-shuffle
-//     transposing butterfly (generic kernel) instead of 13 x 5 shuffles; either way each sum ends on
+//     transposing butterfly (one-pixel kernel) instead of 13 x 5 shuffles; either way each sum ends on
 //     its own lane, so the 13 atomics issue as ONE predicated RED instruction instead of 13 serial
 //     ones from lane 0;
 //   * the same per-warp rectangle cull and TMA-bulk staged 64-byte records as the forward, and the same
@@ -33,6 +33,24 @@ struct BlendBwdParams {
     const float *v_out_alpha;  // (H,W), or null for a zero cotangent
     float *v_xy, *v_xy_abs, *v_pix_vel, *v_conic, *v_rgb, *v_opac;
 };
+
+// The warp reduction leaves per-Gaussian sum k (rgb 3, conic 3, xy 2, |xy| 2, pixel velocity 2, opacity 1) on lane 2k,
+// which adds it at dst[id * stride] of the array returned here; the other lanes get null.
+__device__ __forceinline__ float *grad_lane_dst(int lane, float *v_rgb, float *v_conic, float *v_xy, float *v_xy_abs,
+                                                float *v_pix_vel, float *v_opac, int &stride) {
+    float *dst = nullptr;
+    stride = 0;
+    const int k = lane >> 1;
+    if ((lane & 1) == 0) {
+        if (k < 3) { dst = v_rgb + k; stride = 3; }
+        else if (k < 6) { dst = v_conic + (k - 3); stride = 3; }
+        else if (k < 8) { dst = v_xy + (k - 6); stride = 2; }
+        else if (k < 10) { dst = v_xy_abs + (k - 8); stride = 2; }
+        else if (k < 12) { dst = v_pix_vel + (k - 10); stride = 2; }
+        else if (k == 12) { dst = v_opac; stride = 1; }
+    }
+    return dst;
+}
 
 // Sum 16 per-lane values across the warp; lane L returns the total of value (L >> 1) & 15.
 __device__ __forceinline__ float butterfly16(const float (&v)[16], int lane) {
@@ -64,12 +82,12 @@ __device__ __forceinline__ float butterfly16(const float (&v)[16], int lane) {
     return w1;
 }
 
-template <int S, int PPL>
-__global__ void __launch_bounds__(BLEND_THREADS / PPL, PPL == 2 ? 5 : (PPL == 4 ? 6 : 3)) blend_backward_kernel(const BlendBwdParams p) {
-    constexpr int NT = BLEND_THREADS / PPL;
+// ---- one pixel per lane: tiles other than 16x16 ---------------------------------------------------------------------
+template <int S>
+__global__ void __launch_bounds__(BLEND_THREADS, 3) blend_backward_kernel(const BlendBwdParams p) {
     __shared__ __align__(128) PackedGaussian s_rec[BLEND_STAGES][BLEND_BATCH];
     __shared__ __align__(8) uint64_t s_bar[BLEND_STAGES];
-    __shared__ int s_max[NT / 32];
+    __shared__ int s_max[BLEND_THREADS / 32];
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int tile = p.tile_order ? __ldg(p.tile_order + blockIdx.x) : (int)blockIdx.x;
@@ -78,40 +96,33 @@ __global__ void __launch_bounds__(BLEND_THREADS / PPL, PPL == 2 ? 5 : (PPL == 4 
     const float inv_s = 1.0f / (float)S;
     const float bg0 = __ldg(p.background), bg1 = __ldg(p.background + 1), bg2 = __ldg(p.background + 2);
 
-    bool inside[PPL];
-    float px[PPL], py[PPL], roll[PPL];
+    int lx, ly;
+    bool has_pixel;
+    tile_pixel(p.g.bw, tid, lx, ly, has_pixel);
+    const int j = tile_x * p.g.bw + lx, i = tile_y * p.g.bw + ly;
+    const bool inside = has_pixel && i < p.g.H && j < p.g.W;
+    const float px = (float)j + 0.5f, py = (float)i + 0.5f;
+    const float roll = (float)((double)p.g.rs_time * ((double)(py / (float)p.g.H) - 0.5));
     // per-pixel cotangents and per-sample state (backward.cu:198-217)
-    float vo[PPL][3];
-    float Tm[PPL][S], D[PPL][S];  // Tm = T / S;  D = Tfinal/S * (v_alpha_out - bg.v_out) - sum_behind(fac * rgb.v_out)
-    int bin_final[PPL][S];
+    const size_t pix = inside ? (size_t)i * p.g.W + j : 0;
+    float vo0 = 0.f, vo1 = 0.f, vo2 = 0.f, voa = 0.f;
+    if (inside) {
+        vo0 = p.v_out[3 * pix]; vo1 = p.v_out[3 * pix + 1]; vo2 = p.v_out[3 * pix + 2];
+        voa = p.v_out_alpha ? p.v_out_alpha[pix] : 0.f;
+    }
+    const float bgdot = bg0 * vo0 + bg1 * vo1 + bg2 * vo2;
+    float Tm[S], D[S];  // Tm = T / S;  D = Tfinal/S * (v_alpha_out - bg.v_out) - sum_behind(fac * rgb.v_out)
+    int bin_final[S];
     int my_max = -1;
 #pragma unroll
-    for (int q = 0; q < PPL; ++q) {
-        int lx, ly;
-        bool has_pixel;
-        tile_pixel_ppl<PPL>(p.g.bw, tid, q, lx, ly, has_pixel);
-        const int j = tile_x * p.g.bw + lx, i = tile_y * p.g.bw + ly;
-        inside[q] = has_pixel && i < p.g.H && j < p.g.W;
-        px[q] = (float)j + 0.5f; py[q] = (float)i + 0.5f;
-        roll[q] = (float)((double)p.g.rs_time * ((double)(py[q] / (float)p.g.H) - 0.5));
-        const size_t pix = inside[q] ? (size_t)i * p.g.W + j : 0;
-        float voa = 0.f;
-        vo[q][0] = vo[q][1] = vo[q][2] = 0.f;
-        if (inside[q]) {
-            vo[q][0] = p.v_out[3 * pix]; vo[q][1] = p.v_out[3 * pix + 1]; vo[q][2] = p.v_out[3 * pix + 2];
-            voa = p.v_out_alpha ? p.v_out_alpha[pix] : 0.f;
-        }
-        const float bgdot = bg0 * vo[q][0] + bg1 * vo[q][1] + bg2 * vo[q][2];
-#pragma unroll
-        for (int s = 0; s < S; ++s) {
-            Tm[q][s] = inv_s; D[q][s] = 0.f; bin_final[q][s] = -1;
-            if (inside[q]) {
-                const float Tf = p.final_Ts[pix * S + s];
-                Tm[q][s] = Tf * inv_s;
-                D[q][s] = Tf * inv_s * (voa - bgdot);
-                bin_final[q][s] = min(p.final_idx[pix * S + s], range.y - 1);  // batches only cover [range.x, range.y)
-                my_max = max(my_max, bin_final[q][s]);
-            }
+    for (int s = 0; s < S; ++s) {
+        Tm[s] = inv_s; D[s] = 0.f; bin_final[s] = -1;
+        if (inside) {
+            const float Tf = p.final_Ts[pix * S + s];
+            Tm[s] = Tf * inv_s;
+            D[s] = Tf * inv_s * (voa - bgdot);
+            bin_final[s] = min(p.final_idx[pix * S + s], range.y - 1);  // batches only cover [range.x, range.y)
+            my_max = max(my_max, bin_final[s]);
         }
     }
     float blur[S];
@@ -120,49 +131,22 @@ __global__ void __launch_bounds__(BLEND_THREADS / PPL, PPL == 2 ? 5 : (PPL == 4 
 
     const int wmax = __reduce_max_sync(0xffffffffu, my_max);  // last contributor over the warp's pixel-samples
     if (lane == 0) s_max[warp] = wmax;
-    const WarpWindow win = warp_window<PPL>(inside, px, py, roll);
+    const WarpWindow win = warp_window<1>({inside}, {px}, {py}, {roll});
 
-    if (tid == 0) {
-#pragma unroll
-        for (int st = 0; st < BLEND_STAGES; ++st) mbar_init(&s_bar[st], 1);
-        fence_mbar_init();
-    }
-    __syncthreads();
+    init_stages(s_bar, tid);
     int hi = -1;
 #pragma unroll
-    for (int w = 0; w < NT / 32; ++w) hi = max(hi, s_max[w]);
+    for (int w = 0; w < BLEND_THREADS / 32; ++w) hi = max(hi, s_max[w]);
     const int total = hi - range.x + 1;  // entries hi, hi-1, ..., range.x
     const int nb = total > 0 ? (total + BLEND_BATCH - 1) / BLEND_BATCH : 0;
 
-    // which output array / component this lane's butterfly result goes to
-    float *my_dst = nullptr;
-    int my_stride = 0;
-    {
-        const int k = lane >> 1;
-        if ((lane & 1) == 0) {
-            if (k < 3) { my_dst = p.v_rgb + k; my_stride = 3; }
-            else if (k < 6) { my_dst = p.v_conic + (k - 3); my_stride = 3; }
-            else if (k < 8) { my_dst = p.v_xy + (k - 6); my_stride = 2; }
-            else if (k < 10) { my_dst = p.v_xy_abs + (k - 8); my_stride = 2; }
-            else if (k < 12) { my_dst = p.v_pix_vel + (k - 10); my_stride = 2; }
-            else if (k == 12) { my_dst = p.v_opac; my_stride = 1; }
-        }
-    }
+    int my_stride;
+    float *const my_dst = grad_lane_dst(lane, p.v_rgb, p.v_conic, p.v_xy, p.v_xy_abs, p.v_pix_vel, p.v_opac, my_stride);
 
     // stage entry t of batch b  <->  list index hi - b*BATCH - t  (t ascending = back to front)
     auto issue = [&](int b) {
-        const int st = b & 1;
         const int top = hi - b * BLEND_BATCH;
-        const int cnt = min(BLEND_BATCH, top - range.x + 1);
-        if (tid == 0) mbar_arrive_expect_tx(&s_bar[st], (uint32_t)cnt * (uint32_t)sizeof(PackedGaussian));
-#pragma unroll
-        for (int r = 0; r < PPL; ++r) {
-            const int e = tid + r * NT;
-            if (e < cnt) {
-                const int g = __ldg(p.ids_sorted + top - e);
-                tma_bulk_g2s(&s_rec[st][e], p.packed + g, (uint32_t)sizeof(PackedGaussian), &s_bar[st]);
-            }
-        }
+        issue_batch<BLEND_THREADS, -1>(s_rec, s_bar, b, tid, p.ids_sorted, p.packed, top, min(BLEND_BATCH, top - range.x + 1));
     };
 
     B200_COUNT_DECL;
@@ -170,7 +154,7 @@ __global__ void __launch_bounds__(BLEND_THREADS / PPL, PPL == 2 ? 5 : (PPL == 4 
     for (int b = 0; b < nb; ++b) {
         const int st = b & 1;
         if (b + 1 < nb) issue(b + 1);
-        mbar_wait(&s_bar[st], (uint32_t)((b >> 1) & 1));
+        wait_batch(s_bar, b);
         const int top = hi - b * BLEND_BATCH;
         const int cnt = min(BLEND_BATCH, top - range.x + 1);
 
@@ -193,70 +177,44 @@ __global__ void __launch_bounds__(BLEND_THREADS / PPL, PPL == 2 ? 5 : (PPL == 4 
                     const float4 C = *reinterpret_cast<const float4 *>(&s_rec[st][k].r);    // r g b thr
                     const float cut = C.w + 1e-4f;
                     float sxx = 0.f, sxy = 0.f, syy = 0.f, gxs = 0.f, gys = 0.f, gxa = 0.f, gya = 0.f, pvx = 0.f, pvy = 0.f,
-                          vop = 0.f;
-                    float cdot[PPL], facsum[PPL], dx0[PPL], dy0[PPL];
+                          vop = 0.f, facsum = 0.f;
+                    const float cdot = C.x * vo0 + C.y * vo1 + C.z * vo2;
+                    const float dx0 = A.x - px, dy0 = A.y - py;
                     const SigmaEntry se = sigma_entry(A, Bq);
-#pragma unroll
-                    for (int q = 0; q < PPL; ++q) {
-                        cdot[q] = C.x * vo[q][0] + C.y * vo[q][1] + C.z * vo[q][2];
-                        facsum[q] = 0.f;
-                        dx0[q] = A.x - px[q]; dy0[q] = A.y - py[q];
-                    }
                     bool any = false;
 #pragma unroll
                     for (int s = 0; s < S; ++s) {
                         if (!(smask & (1u << s))) continue;  // warp-uniform
-                        // The lane's PPL pixels are evaluated side by side in straight-line code (independent
-                        // dependency chains for the scheduler to interleave); invalid pixels are masked, not branched.
-                        float dx[PPL], dy[PPL], sigma[PPL], tau[PPL];
-                        bool ok[PPL], some = false;
-#pragma unroll
-                        for (int q = 0; q < PPL; ++q) {
-                            tau[q] = blur[s] + roll[q];
-                            sigma_eval(se, px[q], py[q], dx0[q], dy0[q], tau[q], dx[q], dy[q], sigma[q]);
-                            ok[q] = (idx <= bin_final[q][s]) && !(sigma[q] > cut || sigma[q] < 0.f);  // backward.cu:252-254,276
-                            some |= ok[q];
-                            if (inside[q]) B200_COUNT(3, 1);
-                        }
-                        if (!some) continue;
-                        float vis[PPL], ov[PPL], alpha[PPL];
-                        some = false;
-#pragma unroll
-                        for (int q = 0; q < PPL; ++q) {
-                            vis[q] = exp_neg_approx(ok[q] ? sigma[q] : 0.f);
-                            ov[q] = Bq.w * vis[q];
-                            alpha[q] = fminf(0.99f, ov[q]);
-                            ok[q] = ok[q] && !(alpha[q] < 1.f / 255.f);
-                            some |= ok[q];
-                            if (ok[q]) B200_COUNT(4, 1);
-                        }
-                        if (!some) continue;
+                        const float tau = blur[s] + roll;
+                        float dx, dy, sigma;
+                        sigma_eval(se, dx0, dy0, tau, dx, dy, sigma);
+                        bool ok = (idx <= bin_final[s]) && !(sigma > cut || sigma < 0.f);  // backward.cu:252-254,276
+                        if (inside) B200_COUNT(3, 1);
+                        if (!ok) continue;
+                        const float vis = exp_neg_approx(sigma);
+                        const float ov = Bq.w * vis;
+                        const float alpha = fminf(0.99f, ov);
+                        ok = !(alpha < 1.f / 255.f);
+                        if (!ok) continue;
+                        B200_COUNT(4, 1);
                         any = true;
-#pragma unroll
-                        for (int q = 0; q < PPL; ++q) {
-                            const float ra = rcp_approx(1.f - alpha[q]);
-                            const float Tn = Tm[q][s] * ra;  // T / S of backward.cu:294-296
-                            const float fac = alpha[q] * Tn;
-                            const float v_alpha = Tn * cdot[q] + ra * D[q][s];  // backward.cu:303-311
-                            // no zeroing when the clamp is active (backward.cu:317); masked pixels contribute exactly 0
-                            const float v_sigma = ok[q] ? -ov[q] * v_alpha : 0.f;
-                            Tm[q][s] = ok[q] ? Tn : Tm[q][s];
-                            D[q][s] = ok[q] ? D[q][s] - fac * cdot[q] : D[q][s];  // running buffer, :313-315
-                            facsum[q] += ok[q] ? fac : 0.f;
-                            const float u = v_sigma * dx[q], w = v_sigma * dy[q];
-                            sxx += u * dx[q]; sxy += u * dy[q]; syy += w * dy[q];
-                            const float gx = Bq.x * u + Bq.y * w;
-                            const float gy = Bq.y * u + Bq.z * w;
-                            gxs += gx; gys += gy; gxa += fabsf(gx); gya += fabsf(gy);
-                            pvx += gx * tau[q]; pvy += gy * tau[q];
-                            vop += ok[q] ? vis[q] * v_alpha : 0.f;
-                        }
+                        const float ra = rcp_approx(1.f - alpha);
+                        const float Tn = Tm[s] * ra;  // T / S of backward.cu:294-296
+                        const float fac = alpha * Tn;
+                        const float v_alpha = Tn * cdot + ra * D[s];  // backward.cu:303-311
+                        const float v_sigma = -ov * v_alpha;  // no zeroing when the clamp is active (backward.cu:317)
+                        Tm[s] = Tn;
+                        D[s] = D[s] - fac * cdot;  // running buffer, :313-315
+                        facsum += fac;
+                        const float u = v_sigma * dx, w = v_sigma * dy;
+                        sxx += u * dx; sxy += u * dy; syy += w * dy;
+                        const float gx = Bq.x * u + Bq.y * w;
+                        const float gy = Bq.y * u + Bq.z * w;
+                        gxs += gx; gys += gy; gxa += fabsf(gx); gya += fabsf(gy);
+                        pvx += gx * tau; pvy += gy * tau;
+                        vop += vis * v_alpha;
                     }
-                    float vr = 0.f, vg = 0.f, vb = 0.f;
-#pragma unroll
-                    for (int q = 0; q < PPL; ++q) {
-                        vr += facsum[q] * vo[q][0]; vg += facsum[q] * vo[q][1]; vb += facsum[q] * vo[q][2];
-                    }
+                    const float vr = facsum * vo0, vg = facsum * vo1, vb = facsum * vo2;
                     if (!__any_sync(0xffffffffu, any)) continue;  // backward.cu:281-283
                     if (lane == 0) B200_COUNT(5, 1);
                     const float v[16] = {vr, vg, vb, 0.5f * sxx, sxy, 0.5f * syy, gxs, gys, gxa, gya, pvx, pvy, vop,
@@ -275,38 +233,26 @@ __global__ void __launch_bounds__(BLEND_THREADS / PPL, PPL == 2 ? 5 : (PPL == 4 
 }
 
 
-// ---- two pixels per lane, packed (PPL = 2, 16x16 tiles): the kernel the train step runs ------------------------------
-// Same walk, staging, cull and reduction as blend_backward_kernel<S, 2>; the lane's two pixels (rows r and r + 4 of the
-// warp's 8x8 block) live in the two halves of packed float pairs (f2, blend_common.cuh), so every FMA-pipe instruction of
-// the sigma evaluation and of the gradient algebra issues once for both.  Per-sample structure:
+// ---- two pixels per lane, paired (16x16 tiles): the kernel the train step runs --------------------------------------
+// Same walk, staging and cull as blend_backward_kernel; the lane's two pixels (rows r and r + 4 of the warp's 8x8 block)
+// live in the two halves of float pairs (f2, blend_common.cuh), so the sigma evaluation and the gradient algebra read as
+// one instruction stream for both.  Per-sample structure:
 //   * warp-uniform skips first: the exact cull's sample bit and idx <= (warp max of that sample's last contributor);
 //   * sigma, exp, alpha for both pixels in straight-line code; pixels that fail a test are masked by zeroing `vis` and
-//     `alpha` (then fac, v_sigma and every accumulated term are exactly 0 and T is kept by a select) -- one vote decides
-//     whether the gradient algebra runs at all.
-// Visit epilogue of the packed kernel: the 13 per-Gaussian sums are reduced over the warp through a shared-memory
-// transposition (B200_BWD_SMEM_REDUCE=1, default) or with the 16-shuffle transposing butterfly above (=0, A/B build).
-#ifndef B200_BWD_SMEM_REDUCE
-#define B200_BWD_SMEM_REDUCE 1
-#endif
-// B200_BWD_T_SELECT=1 (A/B build): keep a masked pixel's transmittance with two selects instead of relying on
-// rcp.approx(1) == 1 (tools/micro/rcp_check.cu checks it on the device)
-#ifndef B200_BWD_T_SELECT
-#define B200_BWD_T_SELECT 0
-#endif
+//     `alpha` (then fac, v_sigma and every accumulated term are exactly 0, and T is kept because rcp.approx(1) == 1
+//     exactly: tools/micro/rcp_check.cu checks it on the device).  With VOTE, one warp vote per sample skips the gradient
+//     algebra when no lane passes (launch_bwd).
+// Visit epilogue: the 13 per-Gaussian sums are reduced over the warp through a shared-memory transposition.
 constexpr int RED_VALUES = 13;  // rgb 3, conic 3, xy 2, |xy| 2, pixel velocity 2, opacity 1
 constexpr int RED_STRIDE = 36;  // floats per row: 32 lanes + 4 of padding (rows stay 16-byte aligned, halves hit distinct banks)
-#ifndef B200_BWD_MIN_CTAS
-#define B200_BWD_MIN_CTAS 5  // 96 registers; A/B of 4 / 6 in DESIGN.md section 9
-#endif
+constexpr int BWD_MIN_CTAS = 5;  // 96 registers
 template <int S, bool VOTE>
-__global__ void __launch_bounds__(128, B200_BWD_MIN_CTAS) blend_backward_kernel2(const BlendBwdParams p) {
+__global__ void __launch_bounds__(128, BWD_MIN_CTAS) blend_backward_kernel2(const BlendBwdParams p) {
     constexpr int NT = 128;
     __shared__ __align__(128) PackedGaussian s_rec[BLEND_STAGES][BLEND_BATCH];
     __shared__ __align__(8) uint64_t s_bar[BLEND_STAGES];
     __shared__ int s_max[NT / 32];
-#if B200_BWD_SMEM_REDUCE
     __shared__ __align__(16) float s_red[NT / 32][RED_VALUES * RED_STRIDE];  // per-warp transposition buffer (visit epilogue)
-#endif
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int tile = p.tile_order ? __ldg(p.tile_order + blockIdx.x) : (int)blockIdx.x;
@@ -326,10 +272,9 @@ __global__ void __launch_bounds__(128, B200_BWD_MIN_CTAS) blend_backward_kernel2
 #pragma unroll
     for (int q = 0; q < 2; ++q) {
         int lx, ly;
-        bool has_pixel;
-        tile_pixel_ppl<2>(p.g.bw, tid, q, lx, ly, has_pixel);
+        tile_pixel_pair(tid, q, lx, ly);
         const int j = tile_x * p.g.bw + lx, i = tile_y * p.g.bw + ly;
-        inside[q] = has_pixel && i < p.g.H && j < p.g.W;
+        inside[q] = i < p.g.H && j < p.g.W;
         px[q] = (float)j + 0.5f; py[q] = (float)i + 0.5f;
         roll[q] = (float)((double)p.g.rs_time * ((double)(py[q] / (float)p.g.H) - 0.5));
         const size_t pix = inside[q] ? (size_t)i * p.g.W + j : 0;
@@ -370,18 +315,15 @@ __global__ void __launch_bounds__(128, B200_BWD_MIN_CTAS) blend_backward_kernel2
 #pragma unroll
     for (int s = 0; s < S; ++s) blur[s] = blur_offset<S>(s, p.g.exposure);
 
-    if (tid == 0) {
-#pragma unroll
-        for (int st = 0; st < BLEND_STAGES; ++st) mbar_init(&s_bar[st], 1);
-        fence_mbar_init();
-    }
-    __syncthreads();
+    init_stages(s_bar, tid);
     int hi = -1;
 #pragma unroll
     for (int w = 0; w < NT / 32; ++w) hi = max(hi, s_max[w]);
     const int total = hi - range.x + 1;
     const int nb = total > 0 ? (total + BLEND_BATCH - 1) / BLEND_BATCH : 0;
 
+    // (the gradient table and the batch issue below are written out here, not taken from grad_lane_dst and
+    // issue_batch: those change this kernel's register allocation)
     float *my_dst = nullptr;
     int my_stride = 0;
     {
@@ -396,12 +338,10 @@ __global__ void __launch_bounds__(128, B200_BWD_MIN_CTAS) blend_backward_kernel2
         }
     }
 
-#if B200_BWD_SMEM_REDUCE
     float *const red_row = &s_red[warp][lane];
     // lanes 26..31 own no sum (my_dst is null): they re-read row 12 (a broadcast) instead of branching
     const float4 *const red_half =
         reinterpret_cast<const float4 *>(&s_red[warp][min(lane >> 1, RED_VALUES - 1) * RED_STRIDE + (lane & 1) * 16]);
-#endif
 
     auto issue = [&](int b) {
         const int st = b & 1;
@@ -423,7 +363,7 @@ __global__ void __launch_bounds__(128, B200_BWD_MIN_CTAS) blend_backward_kernel2
     for (int b = 0; b < nb; ++b) {
         const int st = b & 1;
         if (b + 1 < nb) issue(b + 1);
-        mbar_wait(&s_bar[st], (uint32_t)((b >> 1) & 1));
+        wait_batch(s_bar, b);
         const int top = hi - b * BLEND_BATCH;
         const int cnt = min(BLEND_BATCH, top - range.x + 1);
 
@@ -492,11 +432,7 @@ __global__ void __launch_bounds__(128, B200_BWD_MIN_CTAS) blend_backward_kernel2
                         const f2 v_alpha = f2_fma(Tn, cdot, f2_mul(ra, D[s]));  // backward.cu:303-311
                         // no zeroing when the clamp is active (backward.cu:317)
                         const f2 v_sigma = f2_mul(nov, v_alpha);
-#if B200_BWD_T_SELECT
-                        Tm[s] = f2_make(ok0 ? f2_lo(Tn) : f2_lo(Tm[s]), ok1 ? f2_hi(Tn) : f2_hi(Tm[s]));
-#else
                         Tm[s] = Tn;  // masked pixels: alpha = 0, ra = rcp(1) = 1 exactly (tools/micro/rcp_check.cu), Tn == Tm bit for bit
-#endif
                         D[s] = f2_fma(fac, ncdot, D[s]);                  // running buffer, :313-315
                         facsum = f2_add(facsum, fac);
                         const f2 u = f2_mul(v_sigma, dx), w = f2_mul(v_sigma, dy);
@@ -513,7 +449,6 @@ __global__ void __launch_bounds__(128, B200_BWD_MIN_CTAS) blend_backward_kernel2
                     // (without the votes a visit whose every pixel failed the alpha test reduces 13 exact zeros and the
                     // `tot != 0` guard below drops the atomics: same memory effect as the reference's skip)
                     if (lane == 0) B200_COUNT(5, 1);
-#if B200_BWD_SMEM_REDUCE
                     // lane l parks value j at row j, column l (bank 4 j + l: conflict free); lanes 2 j and 2 j + 1 then add up
                     // the two halves of row j with 4 LDS.128 + 7 paired adds each and meet in one shuffle.  Same owner lane
                     // (2 j) per sum as the butterfly, 13 STS + 4 LDS + 1 SHFL instead of 16 SHFL + 27 selects.
@@ -540,12 +475,6 @@ __global__ void __launch_bounds__(128, B200_BWD_MIN_CTAS) blend_backward_kernel2
                     }
                     tot += __shfl_xor_sync(0xffffffffu, tot, 1);
                     __syncwarp();  // every lane has read its half before the next visit overwrites the rows
-#else
-                    const float v[16] = {f2_sum(f2_mul(facsum, VO0)), f2_sum(f2_mul(facsum, VO1)), f2_sum(f2_mul(facsum, VO2)),
-                                         0.5f * f2_sum(sxx), f2_sum(sxy), 0.5f * f2_sum(syy), f2_sum(gxs), f2_sum(gys), gxa, gya,
-                                         f2_sum(pvx), f2_sum(pvy), f2_sum(vop), 0.f, 0.f, 0.f};
-                    const float tot = butterfly16(v, lane);
-#endif
                     if (my_dst && tot != 0.f) {
                         const int gid = s_rec[st][k].id;
                         atomicAdd(my_dst + (unsigned)gid * (unsigned)my_stride, tot);  // N * 3 < 2^32
@@ -560,21 +489,17 @@ __global__ void __launch_bounds__(128, B200_BWD_MIN_CTAS) blend_backward_kernel2
 
 template <int S>
 static int launch_bwd(const BlendBwdParams &p, cudaStream_t st) {
-    if (p.g.bw == 16 && blend_pixels_per_lane(true) == 4)  // experimental (B200_BLEND_PPL_BWD=4)
-        blend_backward_kernel<S, 4><<<p.g.tbx * p.g.tby, BLEND_THREADS / 4, 0, st>>>(p);
-    else if (p.g.bw == 16 && blend_pixels_per_lane(true) == 2 && blend_packed()) {
+    if (p.g.bw == 16 && !blend_force_one_pixel(true)) {
         // per-sample votes ("does any lane hold a contributing pixel", then skip the gradient algebra): without rolling
         // shutter the exact cull leaves 4 % of the entered sample blocks empty and the vote + branch costs more than the
         // masked arithmetic; with it the warp's time window widens the cull and the skip pays
-        if (B200_SAMPLE_VOTE || p.g.rs_time != 0.f)
+        if (p.g.rs_time != 0.f)
             blend_backward_kernel2<S, true><<<p.g.tbx * p.g.tby, BLEND_THREADS / 2, 0, st>>>(p);
         else
             blend_backward_kernel2<S, false><<<p.g.tbx * p.g.tby, BLEND_THREADS / 2, 0, st>>>(p);
+    } else {
+        blend_backward_kernel<S><<<p.g.tbx * p.g.tby, BLEND_THREADS, 0, st>>>(p);
     }
-    else if (p.g.bw == 16 && blend_pixels_per_lane(true) == 2)  // B200_BLEND_PACKED=0: the scalar two-pixel kernel (A/B)
-        blend_backward_kernel<S, 2><<<p.g.tbx * p.g.tby, BLEND_THREADS / 2, 0, st>>>(p);
-    else
-        blend_backward_kernel<S, 1><<<p.g.tbx * p.g.tby, BLEND_THREADS, 0, st>>>(p);
     B200_LAUNCH_CHECK();
     return B200_OK;
 }
@@ -607,29 +532,16 @@ static int run_blend_backward(int num_points, unsigned img_height, unsigned img_
         B200_CUDA(cudaMemsetAsync(v_opacity, 0, n * sizeof(float), st));
     }
     BlendBwdParams p;
-    p.g = BlendGeom{(int)img_height, (int)img_width, (int)block_width,
-                    (int)((img_width + block_width - 1) / block_width),
-                    (int)((img_height + block_width - 1) / block_width), rolling_shutter_time, exposure_time};
+    p.g = blend_geom(img_height, img_width, block_width, rolling_shutter_time, exposure_time);
     p.ids_sorted = gaussian_ids_sorted;
     p.tile_bins = reinterpret_cast<const int2 *>(tile_bins);
-    p.tile_order = blend_tile_order() ? tile_order : nullptr;
+    p.tile_order = tile_order;
     p.packed = reinterpret_cast<const PackedGaussian *>(packed);
     p.background = background;
     p.final_Ts = final_Ts; p.final_idx = final_idx; p.v_out = v_output; p.v_out_alpha = v_output_alpha;
     p.v_xy = v_xy; p.v_xy_abs = v_xy_abs; p.v_pix_vel = v_pix_vels; p.v_conic = v_conic; p.v_rgb = v_colors;
     p.v_opac = v_opacity;
-    switch (n_blur_samples) {
-        case 1: return launch_bwd<1>(p, st);
-        case 2: return launch_bwd<2>(p, st);
-        case 3: return launch_bwd<3>(p, st);
-        case 4: return launch_bwd<4>(p, st);
-        case 5: return launch_bwd<5>(p, st);
-        case 6: return launch_bwd<6>(p, st);
-        case 7: return launch_bwd<7>(p, st);
-        case 8: return launch_bwd<8>(p, st);
-        case 9: return launch_bwd<9>(p, st);
-        default: return launch_bwd<10>(p, st);
-    }
+    return with_blur_samples(n_blur_samples, [&](auto s) { return launch_bwd<decltype(s)::value>(p, st); });
 }
 
 extern "C" int b200_blend_backward_packed(int num_points, unsigned img_height, unsigned img_width, unsigned block_width,

@@ -1,5 +1,7 @@
 // Shared pieces of the blur / rolling-shutter blend kernels (blend_fwd.cu, blend_bwd.cu).
 #pragma once
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace b200 {
@@ -8,15 +10,11 @@ constexpr int BLEND_THREADS = 256;  // one CTA per tile; 8 warps, each owning an
 constexpr int BLEND_BATCH = 256;    // tile-list entries staged per pipeline stage
 constexpr int BLEND_STAGES = 2;
 
-// 1 or 2 pixels per lane in the blend kernels (B200_BLEND_PPL_FWD / B200_BLEND_PPL_BWD, default 2; only
-// 16x16 tiles can use 2)
-int blend_pixels_per_lane(bool backward);
-// two-pixel kernels: float-pair form (default) or the scalar form (B200_BLEND_PACKED=0)
-bool blend_packed();
-// launch order of the blend CTAs: longest tile list first (default) or raster order (B200_BLEND_TILE_ORDER=0)
-bool blend_tile_order();
+// Test switch: B200_BLEND_PPL_FWD=1 / B200_BLEND_PPL_BWD=1 run the one-pixel kernel on 16x16 tiles too, so the tests can
+// check it on the 16-wide scenes; any other value keeps the paired kernel there
+bool blend_force_one_pixel(bool backward);
 
-// -DB200_BLEND_COUNTERS (A/B build only, see tools/blend_counters.py): the blend kernels count what they execute --
+// -DB200_BLEND_COUNTERS (measurement build only, read by tools/blend_probe.py --counters): the blend kernels count what they execute --
 //   [0] tile-list entries tested by a warp cull   [1] warp visits (entries that survive it)
 //   [2] sample blocks entered (warp, entry, sample)  [3] pixel-sample evaluations executed (sigma computed for a live pixel)
 //   [4] evaluations passing the sigma / alpha >= 1/255 tests (the ones that change a pixel or a gradient)
@@ -40,23 +38,32 @@ extern __device__ unsigned long long g_blend_counters[16];
 #define B200_COUNT_FLUSH(base) ((void)0)
 #endif
 
-// Per-sample "does any lane of the warp hold a contributing pixel" votes in the packed kernels.  With the exact cull in
-// front, 96 % of the sample blocks a warp enters do at config 2 (execution counters, -DB200_BLEND_COUNTERS), so the vote +
-// branch costs more than the masked arithmetic it skips: the forward never votes, the backward votes only with rolling
-// shutter (blend_bwd.cu: launch_bwd).  -DB200_SAMPLE_VOTE=1 restores the votes everywhere (A/B build).
-#ifndef B200_SAMPLE_VOTE
-#define B200_SAMPLE_VOTE 0
-#endif
-
-// Forward: refresh the warp's live-sample set once per 32 list entries (1) or after every visit (0, A/B build)
-#ifndef B200_FWD_ALIVE_PER_CHUNK
-#define B200_FWD_ALIVE_PER_CHUNK 1
-#endif
-
 struct BlendGeom {
     int H, W, bw, tbx, tby;
     float rs_time, exposure;
 };
+
+static inline BlendGeom blend_geom(unsigned H, unsigned W, unsigned bw, float rs_time, float exposure) {
+    return BlendGeom{(int)H, (int)W, (int)bw, (int)((W + bw - 1) / bw), (int)((H + bw - 1) / bw), rs_time, exposure};
+}
+
+// f(std::integral_constant<int, S>{}) for the blur sample count S = n (1 <= n <= B200_MAX_BLUR_SAMPLES): the blend
+// kernels are compiled once per S
+template <class F>
+static int with_blur_samples(unsigned n, F &&f) {
+    switch (n) {
+        case 1: return f(std::integral_constant<int, 1>{});
+        case 2: return f(std::integral_constant<int, 2>{});
+        case 3: return f(std::integral_constant<int, 3>{});
+        case 4: return f(std::integral_constant<int, 4>{});
+        case 5: return f(std::integral_constant<int, 5>{});
+        case 6: return f(std::integral_constant<int, 6>{});
+        case 7: return f(std::integral_constant<int, 7>{});
+        case 8: return f(std::integral_constant<int, 8>{});
+        case 9: return f(std::integral_constant<int, 9>{});
+        default: return f(std::integral_constant<int, 10>{});
+    }
+}
 
 // ---- per-Gaussian packed record -------------------------------------------------------------
 // Gathers the five per-Gaussian arrays the reference blend reads separately (forward.cu:387-394,
@@ -146,24 +153,50 @@ __device__ __forceinline__ void tile_pixel(int bw, int tid, int &lx, int &ly, bo
     }
 }
 
-// PPL pixels per lane (register tiling).  PPL = 2 needs bw == 16: 4 warps per tile, warp w owns the 8x8 block
+// Two pixels per lane in the paired kernels (16x16 tiles only): 4 warps per tile, warp w owns the 8x8 block
 // (w&1, w>>1) and lane l the pixels (l&7, (l>>3) + 4p), p = 0,1 -- half as many (warp, Gaussian) visits, so the
 // per-visit costs (cull, record loads, loop control, the backward's warp reduction + atomics) are paid half as often.
-template <int PPL>
-__device__ __forceinline__ void tile_pixel_ppl(int bw, int tid, int p, int &lx, int &ly, bool &has_pixel) {
-    if (PPL == 1) {
-        tile_pixel(bw, tid, lx, ly, has_pixel);
-    } else if (PPL == 4) {  // experimental: 2 warps per 16x16 tile, each a 16x8 block, 4 pixels per lane
-        const int w = tid >> 5, lane = tid & 31;
-        lx = (lane & 7) + ((p & 1) << 3);
-        ly = (w << 3) + (lane >> 3) + 4 * (p >> 1);
-        has_pixel = true;
-    } else {
-        const int w = tid >> 5, lane = tid & 31;
-        lx = ((w & 1) << 3) + (lane & 7);
-        ly = ((w >> 1) << 3) + (lane >> 3) + 4 * p;
-        has_pixel = true;
+__device__ __forceinline__ void tile_pixel_pair(int tid, int p, int &lx, int &ly) {
+    const int w = tid >> 5, lane = tid & 31;
+    lx = ((w & 1) << 3) + (lane & 7);
+    ly = ((w >> 1) << 3) + (lane >> 3) + 4 * p;
+}
+
+// ---- staging of the tile list: BLEND_BATCH packed records per batch, double buffered -----------------------------
+// Every kernel walks its tile list in batches; batch b is copied into stage b & 1 by one TMA bulk copy per record while
+// the CTA blends batch b - 1, and stage b & 1 is only refilled after a __syncthreads that follows the blend of batch b.
+
+// initialise the stages' mbarriers; every thread returns after the initialisation is visible
+__device__ __forceinline__ void init_stages(uint64_t (&bar)[BLEND_STAGES], int tid) {
+    if (tid == 0) {
+#pragma unroll
+        for (int st = 0; st < BLEND_STAGES; ++st) mbar_init(&bar[st], 1);
+        fence_mbar_init();
     }
+    __syncthreads();
+}
+
+// Stage batch b: its cnt records are those of the list entries first + DIR * t, t = 0 .. cnt - 1 (the forward walks up
+// from range.x, DIR = 1; the backward down from its last contributor, DIR = -1), issued by the NT threads of the CTA.
+template <int NT, int DIR>
+__device__ __forceinline__ void issue_batch(PackedGaussian (&rec)[BLEND_STAGES][BLEND_BATCH], uint64_t (&bar)[BLEND_STAGES],
+                                            int b, int tid, const int32_t *ids, const PackedGaussian *packed, int first,
+                                            int cnt) {
+    const int st = b & 1;
+    if (tid == 0) mbar_arrive_expect_tx(&bar[st], (uint32_t)cnt * (uint32_t)sizeof(PackedGaussian));
+#pragma unroll
+    for (int r = 0; r < BLEND_BATCH / NT; ++r) {
+        const int e = tid + r * NT;
+        if (e < cnt) {
+            const int g = __ldg(ids + first + DIR * e);
+            tma_bulk_g2s(&rec[st][e], packed + g, (uint32_t)sizeof(PackedGaussian), &bar[st]);
+        }
+    }
+}
+
+// wait until batch b has landed in its stage
+__device__ __forceinline__ void wait_batch(uint64_t (&bar)[BLEND_STAGES], int b) {
+    mbar_wait(&bar[b & 1], (uint32_t)((b >> 1) & 1));
 }
 
 __device__ __forceinline__ float warp_min(float v) {
@@ -221,33 +254,23 @@ __device__ __forceinline__ float f2_sum(f2 x) { return x.lo + x.hi; }
 
 // sigma of forward.cu:405-410 / backward.cu:263-268 for one pixel and one blur sample.
 // The pixel-independent parts are hoisted per tile-list entry (half conics) and per pixel (offset at tau = 0) and the
-// quadratic form is evaluated as dx * (a/2 dx + b dy) + c/2 dy^2; -DB200_SIGMA_FACTORED=0 compiles the reference's
-// expression term for term instead (results agree to the last bits of sigma; all parity tests, including the live
-// reference-CUDA pin, pass with either).
-#ifndef B200_SIGMA_FACTORED
-#define B200_SIGMA_FACTORED 1
-#endif
+// quadratic form is evaluated as dx * (a/2 dx + b dy) + c/2 dy^2 (it agrees with the reference's term-for-term
+// expression to the last bits of sigma).
 struct SigmaEntry {  // per tile-list entry
-    float x, y, vx, vy, a, b, c, ha, hc;
+    float vx, vy, b, ha, hc;
 };
 __device__ __forceinline__ SigmaEntry sigma_entry(const float4 &A, const float4 &Bq) {
     SigmaEntry e;
-    e.x = A.x; e.y = A.y; e.vx = A.z; e.vy = A.w; e.a = Bq.x; e.b = Bq.y; e.c = Bq.z;
+    e.vx = A.z; e.vy = A.w; e.b = Bq.y;
     e.ha = 0.5f * Bq.x; e.hc = 0.5f * Bq.z;
     return e;
 }
-__device__ __forceinline__ void sigma_eval(const SigmaEntry &e, float px, float py, float dx0, float dy0, float tau, float &dx,
-                                           float &dy, float &sigma) {
-#if B200_SIGMA_FACTORED
+__device__ __forceinline__ void sigma_eval(const SigmaEntry &e, float dx0, float dy0, float tau, float &dx, float &dy,
+                                           float &sigma) {
     dx = fmaf(tau, e.vx, dx0);
     dy = fmaf(tau, e.vy, dy0);
     const float u = fmaf(e.ha, dx, e.b * dy);
     sigma = fmaf(dx, u, (e.hc * dy) * dy);
-#else
-    dx = e.x + tau * e.vx - px;
-    dy = e.y + tau * e.vy - py;
-    sigma = 0.5f * (e.a * dx * dx + e.c * dy * dy) + e.b * dx * dy;
-#endif
 }
 
 // blur_rel of forward.cu:363 without the rolling-shutter part
@@ -285,9 +308,6 @@ __device__ __forceinline__ unsigned sample_mask(const PackedGaussian &g, const W
 // splat whose bounding box touches the rectangle; this keeps it only where the ellipse itself does.
 // Margins: the blend's fp32 sigma carries rounding of ~1e-7 relative to its LARGEST term (the three terms cancel for
 // needle-shaped splats), so the comparison allows 2e-5 of that magnitude + 1e-3; NaNs keep the entry.
-#ifndef B200_EXACT_CULL
-#define B200_EXACT_CULL 1
-#endif
 __device__ __forceinline__ bool box_may_reach(float a, float b, float c, float nb_inv_a, float nb_inv_c, float thr, float x0,
                                               float x1, float y0, float y1) {
     // the edges of the box that face the origin (if the box straddles an axis either edge of that pair serves: the
@@ -308,7 +328,6 @@ __device__ __forceinline__ bool box_may_reach(float a, float b, float c, float n
 template <int S>
 __device__ __forceinline__ unsigned sample_mask_exact(const PackedGaussian &g, const WarpWindow &w, float exposure) {
     unsigned m = sample_mask<S>(g, w, exposure);
-#if B200_EXACT_CULL
     if (m == 0u || !(g.hx < 3.0e38f)) return m;
     // -b/a, -b/c: the clamped vertex only has to be near the minimiser (sigma is flat to second order there)
     const float nb_inv_a = -g.cb * rcp_approx(g.ca), nb_inv_c = -g.cb * rcp_approx(g.cc);
@@ -324,7 +343,6 @@ __device__ __forceinline__ unsigned sample_mask_exact(const PackedGaussian &g, c
                                         by0 + fminf(ay, by), by1 + fmaxf(ay, by));
         if (!keep) m &= ~(1u << s);
     }
-#endif
     return m;
 }
 

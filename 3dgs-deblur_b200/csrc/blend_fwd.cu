@@ -45,83 +45,49 @@ __device__ __forceinline__ void write_empty_render(const BlendFwdParams &p, bool
     if (p.out_alpha) p.out_alpha[pix] = 1.0f;
 }
 
-template <int S, int PPL>
-__global__ void __launch_bounds__(BLEND_THREADS / PPL, PPL == 2 ? 6 : 1) blend_forward_kernel(const BlendFwdParams p) {
-    constexpr int NT = BLEND_THREADS / PPL;  // threads per tile
+// ---- one pixel per lane: tiles other than 16x16 ---------------------------------------------------------------------
+template <int S>
+__global__ void __launch_bounds__(BLEND_THREADS, 1) blend_forward_kernel(const BlendFwdParams p) {
     __shared__ __align__(128) PackedGaussian s_rec[BLEND_STAGES][BLEND_BATCH];
     __shared__ __align__(8) uint64_t s_bar[BLEND_STAGES];
 
     const int tid = threadIdx.x, lane = tid & 31;
     const int tile = p.tile_order ? __ldg(p.tile_order + blockIdx.x) : (int)blockIdx.x;
     const int tile_x = tile % p.g.tbx, tile_y = tile / p.g.tbx;
-    bool inside[PPL];
-    float px[PPL], py[PPL], roll[PPL];
-    int pi[PPL], pj[PPL];
-#pragma unroll
-    for (int q = 0; q < PPL; ++q) {
-        int lx, ly;
-        bool has_pixel;
-        tile_pixel_ppl<PPL>(p.g.bw, tid, q, lx, ly, has_pixel);
-        pj[q] = tile_x * p.g.bw + lx; pi[q] = tile_y * p.g.bw + ly;
-        inside[q] = has_pixel && pi[q] < p.g.H && pj[q] < p.g.W;
-        px[q] = (float)pj[q] + 0.5f; py[q] = (float)pi[q] + 0.5f;
-        roll[q] = (float)((double)p.g.rs_time * ((double)(py[q] / (float)p.g.H) - 0.5));  // forward.cu:360
-    }
+    int lx, ly;
+    bool has_pixel;
+    tile_pixel(p.g.bw, tid, lx, ly, has_pixel);
+    const int pj = tile_x * p.g.bw + lx, pi = tile_y * p.g.bw + ly;
+    const bool inside = has_pixel && pi < p.g.H && pj < p.g.W;
+    const float px = (float)pj + 0.5f, py = (float)pi + 0.5f;
+    const float roll = (float)((double)p.g.rs_time * ((double)(py / (float)p.g.H) - 0.5));  // forward.cu:360
     if (p.ref_isect && __ldg(p.ref_isect) < 1) {  // block-uniform
-#pragma unroll
-        for (int q = 0; q < PPL; ++q) write_empty_render<S>(p, inside[q], pi[q], pj[q]);
+        write_empty_render<S>(p, inside, pi, pj);
         return;
     }
-    float blur[S];  // blur_rel of forward.cu:363 without the roll part; tau = blur[s] + roll[q]
+    float blur[S];  // blur_rel of forward.cu:363 without the roll part; tau = blur[s] + roll
 #pragma unroll
     for (int s = 0; s < S; ++s) blur[s] = blur_offset<S>(s, p.g.exposure);
 
-    const WarpWindow win = warp_window<PPL>(inside, px, py, roll);
+    const WarpWindow win = warp_window<1>({inside}, {px}, {py}, {roll});
 
     const int2 range = p.tile_bins[tile];
     const int total = range.y - range.x;
     const int nb = (total + BLEND_BATCH - 1) / BLEND_BATCH;
 
-    if (tid == 0) {
-#pragma unroll
-        for (int st = 0; st < BLEND_STAGES; ++st) mbar_init(&s_bar[st], 1);
-        fence_mbar_init();
-    }
-    __syncthreads();
-
+    init_stages(s_bar, tid);
     auto issue = [&](int b) {
-        const int st = b & 1;
         const int start = range.x + b * BLEND_BATCH;
-        const int cnt = min(BLEND_BATCH, range.y - start);
-        if (tid == 0) mbar_arrive_expect_tx(&s_bar[st], (uint32_t)cnt * (uint32_t)sizeof(PackedGaussian));
-#pragma unroll
-        for (int r = 0; r < PPL; ++r) {
-            const int e = tid + r * NT;
-            if (e < cnt) {
-                const int g = __ldg(p.ids_sorted + start + e);
-                tma_bulk_g2s(&s_rec[st][e], p.packed + g, (uint32_t)sizeof(PackedGaussian), &s_bar[st]);
-            }
-        }
+        issue_batch<BLEND_THREADS, 1>(s_rec, s_bar, b, tid, p.ids_sorted, p.packed, start, min(BLEND_BATCH, range.y - start));
     };
 
-    float T[PPL][S];
-    int last[PPL][S];
-    float acc[PPL][3];
-    unsigned alive[PPL];
+    float T[S];
+    int last[S];
+    float acc0 = 0.f, acc1 = 0.f, acc2 = 0.f;
 #pragma unroll
-    for (int q = 0; q < PPL; ++q) {
-#pragma unroll
-        for (int s = 0; s < S; ++s) { T[q][s] = 1.f; last[q][s] = 0; }
-        acc[q][0] = acc[q][1] = acc[q][2] = 0.f;
-        alive[q] = inside[q] ? ((1u << S) - 1u) : 0u;
-    }
+    for (int s = 0; s < S; ++s) { T[s] = 1.f; last[s] = 0; }
+    unsigned alive = inside ? ((1u << S) - 1u) : 0u;
     const float inv_s = 1.0f / (float)S;
-    auto any_alive = [&]() {
-        unsigned a = 0u;
-#pragma unroll
-        for (int q = 0; q < PPL; ++q) a |= alive[q];
-        return a != 0u;
-    };
 
     B200_COUNT_DECL;
     int b = 0;
@@ -130,12 +96,12 @@ __global__ void __launch_bounds__(BLEND_THREADS / PPL, PPL == 2 ? 6 : 1) blend_f
     for (; b < nb; ++b) {
         const int st = b & 1;
         if (b + 1 < nb) issue(b + 1);
-        mbar_wait(&s_bar[st], (uint32_t)((b >> 1) & 1));
+        wait_batch(s_bar, b);
         pending = (b + 1 < nb);
         const int start = range.x + b * BLEND_BATCH;
         const int cnt = min(BLEND_BATCH, range.y - start);
 
-        if (__any_sync(0xffffffffu, any_alive())) {
+        if (__any_sync(0xffffffffu, alive != 0u)) {
             for (int c0 = 0; c0 < cnt; c0 += 32) {
                 const int e = c0 + lane;
                 const unsigned my_mask = (e < cnt) ? sample_mask_exact<S>(s_rec[st][e], win, p.g.exposure) : 0u;
@@ -155,82 +121,73 @@ __global__ void __launch_bounds__(BLEND_THREADS / PPL, PPL == 2 ? 6 : 1) blend_f
                     const float4 C = *reinterpret_cast<const float4 *>(&s_rec[st][k].r);    // r g b thr
                     const float cut = C.w + 1e-4f;
                     const SigmaEntry se = sigma_entry(A, Bq);
-                    float dx0[PPL], dy0[PPL];
-#pragma unroll
-                    for (int q = 0; q < PPL; ++q) { dx0[q] = A.x - px[q]; dy0[q] = A.y - py[q]; }
+                    const float dx0 = A.x - px, dy0 = A.y - py;
 #pragma unroll
                     for (int s = 0; s < S; ++s) {
                         if (!(smask & (1u << s))) continue;  // warp-uniform
-#pragma unroll
-                        for (int q = 0; q < PPL; ++q) {
-                            if (!(alive[q] & (1u << s))) continue;
-                            const float tau = blur[s] + roll[q];
-                            float dx, dy, sigma;
-                            sigma_eval(se, px[q], py[q], dx0[q], dy0[q], tau, dx, dy, sigma);
-                            B200_COUNT(3, 1);
-                            if (sigma > cut || sigma < 0.f) continue;  // alpha < 1/255 guaranteed above thr
-                            const float alpha = fminf(0.999f, Bq.w * exp_neg_approx(sigma));
-                            if (alpha < 1.f / 255.f) continue;
-                            B200_COUNT(4, 1);
+                        if (!(alive & (1u << s))) continue;
+                        const float tau = blur[s] + roll;
+                        float dx, dy, sigma;
+                        sigma_eval(se, dx0, dy0, tau, dx, dy, sigma);
+                        B200_COUNT(3, 1);
+                        if (sigma > cut || sigma < 0.f) continue;  // alpha < 1/255 guaranteed above thr
+                        const float alpha = fminf(0.999f, Bq.w * exp_neg_approx(sigma));
+                        if (alpha < 1.f / 255.f) continue;
+                        B200_COUNT(4, 1);
 #ifdef B200_BLEND_COUNTERS
-                            blended_ = true;
+                        blended_ = true;
 #endif
-                            const float next_T = T[q][s] * (1.f - alpha);
-                            if (next_T <= 1e-4f) {  // forward.cu:421-427: this sample is done, entry not blended
-                                alive[q] &= ~(1u << s);
-                                continue;
-                            }
-                            const float vis = alpha * T[q][s] * inv_s;
-                            acc[q][0] += C.x * vis; acc[q][1] += C.y * vis; acc[q][2] += C.z * vis;
-                            T[q][s] = next_T;
-                            last[q][s] = start + k;
+                        const float next_T = T[s] * (1.f - alpha);
+                        if (next_T <= 1e-4f) {  // forward.cu:421-427: this sample is done, entry not blended
+                            alive &= ~(1u << s);
+                            continue;
                         }
+                        const float vis = alpha * T[s] * inv_s;
+                        acc0 += C.x * vis; acc1 += C.y * vis; acc2 += C.z * vis;
+                        T[s] = next_T;
+                        last[s] = start + k;
                     }
 #ifdef B200_BLEND_COUNTERS
                     if (__any_sync(0xffffffffu, blended_) && lane == 0) B200_COUNT(5, 1);
 #endif
-                    if (!__any_sync(0xffffffffu, any_alive())) { m = 0; c0 = cnt; }
+                    if (!__any_sync(0xffffffffu, alive != 0u)) { m = 0; c0 = cnt; }
                 }
             }
         }
         // all warps are done with stage `st` (it is refilled two batches from now) + early exit vote
-        if (!__syncthreads_or(any_alive())) { ++b; break; }
+        if (!__syncthreads_or(alive != 0u)) { ++b; break; }
     }
-    if (pending && b < nb) mbar_wait(&s_bar[b & 1], (uint32_t)((b >> 1) & 1));  // drain the prefetch before exit
+    if (pending && b < nb) wait_batch(s_bar, b);  // drain the prefetch before exit
     B200_COUNT_FLUSH(0);
 
     const float bg0 = __ldg(p.background), bg1 = __ldg(p.background + 1), bg2 = __ldg(p.background + 2);
+    if (!inside) return;
+    const size_t pix = (size_t)pi * p.g.W + pj;
+    float meanT = 0.f, sumT = 0.f;
 #pragma unroll
-    for (int q = 0; q < PPL; ++q) {
-        if (!inside[q]) continue;
-        const size_t pix = (size_t)pi[q] * p.g.W + pj[q];
-        float meanT = 0.f, sumT = 0.f;
-#pragma unroll
-        for (int s = 0; s < S; ++s) {
-            meanT += T[q][s] * inv_s;
-            sumT += T[q][s];
-            p.final_Ts[pix * S + s] = T[q][s];
-            p.final_idx[pix * S + s] = last[q][s];
-        }
-        p.out_img[3 * pix] = acc[q][0] + meanT * bg0;
-        p.out_img[3 * pix + 1] = acc[q][1] + meanT * bg1;
-        p.out_img[3 * pix + 2] = acc[q][2] + meanT * bg2;
-        if (p.out_alpha) p.out_alpha[pix] = 1.0f - sumT * inv_s;
+    for (int s = 0; s < S; ++s) {
+        meanT += T[s] * inv_s;
+        sumT += T[s];
+        p.final_Ts[pix * S + s] = T[s];
+        p.final_idx[pix * S + s] = last[s];
     }
+    p.out_img[3 * pix] = acc0 + meanT * bg0;
+    p.out_img[3 * pix + 1] = acc1 + meanT * bg1;
+    p.out_img[3 * pix + 2] = acc2 + meanT * bg2;
+    if (p.out_alpha) p.out_alpha[pix] = 1.0f - sumT * inv_s;
 }
 
 
-// ---- two pixels per lane, paired (PPL = 2, 16x16 tiles): the kernel the train step runs ------------------------------
-// Same walk, staging and cull as blend_forward_kernel<S, 2>.  The lane's two pixels live in the halves of float pairs
+// ---- two pixels per lane, paired (16x16 tiles): the kernel the train step runs --------------------------------------
+// Same walk, staging and cull as blend_forward_kernel.  The lane's two pixels live in the halves of float pairs
 // (f2, blend_common.cuh) and are evaluated side by side in straight-line code: the sigma quadratic, alpha * T and the
-// three colour accumulations run for both pixels without branches, failed tests mask instead of branching (alpha = 0
-// leaves T, the colour sums and `last` untouched), and one warp vote per sample skips the blend arithmetic when no lane
-// passes.
-#ifndef B200_FWD_MIN_CTAS
-#define B200_FWD_MIN_CTAS 6  // 80 registers
-#endif
+// three colour accumulations run for both pixels without branches, and failed tests mask instead of branching
+// (alpha = 0 leaves T, the colour sums and `last` untouched).  There is no per-sample "does any lane pass" vote: with
+// the exact cull in front, 96 % of the sample blocks a warp enters at config 2 have a passing lane (execution counters,
+// -DB200_BLEND_COUNTERS), so the vote + branch would cost more than the masked arithmetic it skips.
+constexpr int FWD_MIN_CTAS = 6;  // 80 registers
 template <int S>
-__global__ void __launch_bounds__(128, B200_FWD_MIN_CTAS) blend_forward_kernel2(const BlendFwdParams p) {
+__global__ void __launch_bounds__(128, FWD_MIN_CTAS) blend_forward_kernel2(const BlendFwdParams p) {
     constexpr int NT = 128;
     __shared__ __align__(128) PackedGaussian s_rec[BLEND_STAGES][BLEND_BATCH];
     __shared__ __align__(8) uint64_t s_bar[BLEND_STAGES];
@@ -244,10 +201,9 @@ __global__ void __launch_bounds__(128, B200_FWD_MIN_CTAS) blend_forward_kernel2(
 #pragma unroll
     for (int q = 0; q < 2; ++q) {
         int lx, ly;
-        bool has_pixel;
-        tile_pixel_ppl<2>(p.g.bw, tid, q, lx, ly, has_pixel);
+        tile_pixel_pair(tid, q, lx, ly);
         pj[q] = tile_x * p.g.bw + lx; pi[q] = tile_y * p.g.bw + ly;
-        inside[q] = has_pixel && pi[q] < p.g.H && pj[q] < p.g.W;
+        inside[q] = pi[q] < p.g.H && pj[q] < p.g.W;
         px[q] = (float)pj[q] + 0.5f; py[q] = (float)pi[q] + 0.5f;
         roll[q] = (float)((double)p.g.rs_time * ((double)(py[q] / (float)p.g.H) - 0.5));  // forward.cu:360
     }
@@ -266,26 +222,10 @@ __global__ void __launch_bounds__(128, B200_FWD_MIN_CTAS) blend_forward_kernel2(
     const int total = range.y - range.x;
     const int nb = (total + BLEND_BATCH - 1) / BLEND_BATCH;
 
-    if (tid == 0) {
-#pragma unroll
-        for (int st = 0; st < BLEND_STAGES; ++st) mbar_init(&s_bar[st], 1);
-        fence_mbar_init();
-    }
-    __syncthreads();
-
+    init_stages(s_bar, tid);
     auto issue = [&](int b) {
-        const int st = b & 1;
         const int start = range.x + b * BLEND_BATCH;
-        const int cnt = min(BLEND_BATCH, range.y - start);
-        if (tid == 0) mbar_arrive_expect_tx(&s_bar[st], (uint32_t)cnt * (uint32_t)sizeof(PackedGaussian));
-#pragma unroll
-        for (int r = 0; r < 2; ++r) {
-            const int e = tid + r * NT;
-            if (e < cnt) {
-                const int g = __ldg(p.ids_sorted + start + e);
-                tma_bulk_g2s(&s_rec[st][e], p.packed + g, (uint32_t)sizeof(PackedGaussian), &s_bar[st]);
-            }
-        }
+        issue_batch<NT, 1>(s_rec, s_bar, b, tid, p.ids_sorted, p.packed, start, min(BLEND_BATCH, range.y - start));
     };
 
     const float inv_s = 1.0f / (float)S;
@@ -306,7 +246,7 @@ __global__ void __launch_bounds__(128, B200_FWD_MIN_CTAS) blend_forward_kernel2(
     for (; b < nb; ++b) {
         const int st = b & 1;
         if (b + 1 < nb) issue(b + 1);
-        mbar_wait(&s_bar[st], (uint32_t)((b >> 1) & 1));
+        wait_batch(s_bar, b);
         pending = (b + 1 < nb);
         const int start = range.x + b * BLEND_BATCH;
         const int cnt = min(BLEND_BATCH, range.y - start);
@@ -317,9 +257,7 @@ __global__ void __launch_bounds__(128, B200_FWD_MIN_CTAS) blend_forward_kernel2(
                 const unsigned my_mask = (e < cnt) ? sample_mask_exact<S>(s_rec[st][e], win, p.g.exposure) : 0u;
                 unsigned m = __ballot_sync(0xffffffffu, my_mask != 0u);
                 if (e < cnt) B200_COUNT(0, 1);
-#if B200_FWD_ALIVE_PER_CHUNK
                 const unsigned alive_chunk = alive[0] + alive[1];  // (bits only ever clear: the sum drops iff one did)
-#endif
                 while (m) {
                     const int src = __ffs(m) - 1;
                     const int k = c0 + src;
@@ -336,9 +274,6 @@ __global__ void __launch_bounds__(128, B200_FWD_MIN_CTAS) blend_forward_kernel2(
                     const f2 CR = f2_splat(C.x * inv_s), CG = f2_splat(C.y * inv_s), CBl = f2_splat(C.z * inv_s);
                     const f2 dx0 = f2_sub(f2_splat(A.x), PX), dy0 = f2_sub(f2_splat(A.y), PY);
                     const int idx = start + k;
-#if !B200_FWD_ALIVE_PER_CHUNK
-                    const unsigned alive_before = alive[0] + alive[1];
-#endif
 #ifdef B200_BLEND_COUNTERS
                     bool blended_ = false;
 #endif
@@ -363,9 +298,6 @@ __global__ void __launch_bounds__(128, B200_FWD_MIN_CTAS) blend_forward_kernel2(
                         const float a0 = fminf(0.999f, f2_lo(ov)), a1 = fminf(0.999f, f2_hi(ov));
                         ok0 = ok0 && !(a0 < 1.f / 255.f);
                         ok1 = ok1 && !(a1 < 1.f / 255.f);
-#if B200_SAMPLE_VOTE
-                        if (!__any_sync(0xffffffffu, ok0 || ok1)) continue;
-#endif
                         if (ok0) B200_COUNT(4, 1);
                         if (ok1) B200_COUNT(4, 1);
 #ifdef B200_BLEND_COUNTERS
@@ -387,15 +319,7 @@ __global__ void __launch_bounds__(128, B200_FWD_MIN_CTAS) blend_forward_kernel2(
 #ifdef B200_BLEND_COUNTERS
                     if (__any_sync(0xffffffffu, blended_) && lane == 0) B200_COUNT(5, 1);
 #endif
-#if !B200_FWD_ALIVE_PER_CHUNK
-                    // (bits only ever clear, so the sum of the two masks drops iff one did)
-                    if (__any_sync(0xffffffffu, (alive[0] + alive[1]) != alive_before)) {  // rare: refresh the warp's live set
-                        walive = __reduce_or_sync(0xffffffffu, alive[0] | alive[1]);
-                        if (walive == 0u) { m = 0; c0 = cnt; }
-                    }
-#endif
                 }
-#if B200_FWD_ALIVE_PER_CHUNK
                 // the warp's live-sample set is refreshed once per 32 entries instead of after every visit (a vote + compare
                 // per visit for an event that happens S times per pixel): until then a sample that just finished for every
                 // lane is still entered, fully masked -- no effect on any output
@@ -403,13 +327,12 @@ __global__ void __launch_bounds__(128, B200_FWD_MIN_CTAS) blend_forward_kernel2(
                     walive = __reduce_or_sync(0xffffffffu, alive[0] | alive[1]);
                     if (walive == 0u) c0 = cnt;
                 }
-#endif
             }
         }
         // all warps are done with stage `st` (it is refilled two batches from now) + early exit vote
         if (!__syncthreads_or(walive != 0u)) { ++b; break; }
     }
-    if (pending && b < nb) mbar_wait(&s_bar[b & 1], (uint32_t)((b >> 1) & 1));  // drain the prefetch before exit
+    if (pending && b < nb) wait_batch(s_bar, b);  // drain the prefetch before exit
     B200_COUNT_FLUSH(0);
 
     const float bg0 = __ldg(p.background), bg1 = __ldg(p.background + 1), bg2 = __ldg(p.background + 2);
@@ -437,14 +360,10 @@ __global__ void __launch_bounds__(128, B200_FWD_MIN_CTAS) blend_forward_kernel2(
 template <int S>
 static int launch_fwd(const BlendFwdParams &p, cudaStream_t st) {
     // two pixels per lane when the tile is the full 16x16 (the only size Splatfacto uses, splatfacto.py:815)
-    if (p.g.bw == 16 && blend_pixels_per_lane(false) == 4)  // experimental (B200_BLEND_PPL_FWD=4)
-        blend_forward_kernel<S, 4><<<p.g.tbx * p.g.tby, BLEND_THREADS / 4, 0, st>>>(p);
-    else if (p.g.bw == 16 && blend_pixels_per_lane(false) == 2 && blend_packed())
+    if (p.g.bw == 16 && !blend_force_one_pixel(false))
         blend_forward_kernel2<S><<<p.g.tbx * p.g.tby, BLEND_THREADS / 2, 0, st>>>(p);
-    else if (p.g.bw == 16 && blend_pixels_per_lane(false) == 2)  // B200_BLEND_PACKED=0: the scalar two-pixel kernel (A/B)
-        blend_forward_kernel<S, 2><<<p.g.tbx * p.g.tby, BLEND_THREADS / 2, 0, st>>>(p);
     else
-        blend_forward_kernel<S, 1><<<p.g.tbx * p.g.tby, BLEND_THREADS, 0, st>>>(p);
+        blend_forward_kernel<S><<<p.g.tbx * p.g.tby, BLEND_THREADS, 0, st>>>(p);
     B200_LAUNCH_CHECK();
     return B200_OK;
 }
@@ -505,7 +424,6 @@ using namespace b200;
 extern "C" int b200_blend_tile_order(int num_tiles, const int32_t *tile_bins, int32_t *tile_order, void *stream) {
     B200_REQUIRE(num_tiles >= 1, "num_tiles must be >= 1");
     B200_REQUIRE(tile_bins && tile_order, "null pointer");
-    if (!blend_tile_order()) return B200_OK;  // raster order: the blend entry points ignore tile_order
     tile_order_kernel<<<1, ORDER_THREADS, 0, as_stream(stream)>>>(num_tiles, reinterpret_cast<const int2 *>(tile_bins),
                                                                    tile_order);
     B200_LAUNCH_CHECK();
@@ -526,28 +444,15 @@ static int run_blend_forward(unsigned img_height, unsigned img_width, unsigned b
     B200_REQUIRE(aligned16(packed), "packed records must be 16-byte aligned");
     B200_REQUIRE(out_img && final_Ts && final_idx, "null output pointer");
     BlendFwdParams p;
-    p.g = BlendGeom{(int)img_height, (int)img_width, (int)block_width,
-                    (int)((img_width + block_width - 1) / block_width),
-                    (int)((img_height + block_width - 1) / block_width), rolling_shutter_time, exposure_time};
+    p.g = blend_geom(img_height, img_width, block_width, rolling_shutter_time, exposure_time);
     p.ids_sorted = gaussian_ids_sorted;
     p.tile_bins = reinterpret_cast<const int2 *>(tile_bins);
-    p.tile_order = blend_tile_order() ? tile_order : nullptr;
+    p.tile_order = tile_order;
     p.packed = reinterpret_cast<const PackedGaussian *>(packed);
     p.background = background;
     p.out_img = out_img; p.final_Ts = final_Ts; p.final_idx = final_idx; p.out_alpha = out_alpha;
     p.ref_isect = ref_isect;
-    switch (n_blur_samples) {
-        case 1: return launch_fwd<1>(p, st);
-        case 2: return launch_fwd<2>(p, st);
-        case 3: return launch_fwd<3>(p, st);
-        case 4: return launch_fwd<4>(p, st);
-        case 5: return launch_fwd<5>(p, st);
-        case 6: return launch_fwd<6>(p, st);
-        case 7: return launch_fwd<7>(p, st);
-        case 8: return launch_fwd<8>(p, st);
-        case 9: return launch_fwd<9>(p, st);
-        default: return launch_fwd<10>(p, st);
-    }
+    return with_blur_samples(n_blur_samples, [&](auto s) { return launch_fwd<decltype(s)::value>(p, st); });
 }
 
 extern "C" int b200_pack_records(int num_points, const float *xys, const float *pix_vels, const float *conics,

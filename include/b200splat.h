@@ -195,9 +195,8 @@ B200_API int b200_blend_backward_packed(int num_points, unsigned img_height, uns
  * tiles_y): a permutation of the tiles, longest tile_bins range first, so the costliest tiles start in the first wave
  * instead of trailing the launch.  The _ordered blend entry points run one CTA per tile in that order and otherwise
  * equal b200_blend_forward_packed_status (status may be null: no empty-render branch) and b200_blend_backward_packed:
- * the forward's outputs are bit-identical, the backward's differ only by the order of float atomics.
- * B200_BLEND_TILE_ORDER=0 in the environment restores raster order: b200_blend_tile_order then writes nothing and the
- * _ordered entry points ignore tile_order. */
+ * the forward's outputs are bit-identical, the backward's differ only by the order of float atomics.  The entry points
+ * without tile_order run the tiles in raster order. */
 B200_API int b200_blend_tile_order(int num_tiles, const int32_t *tile_bins, int32_t *tile_order, void *stream);
 B200_API int b200_blend_forward_packed_ordered(unsigned img_height, unsigned img_width, unsigned block_width,
                                                unsigned n_blur_samples, const int32_t *gaussian_ids_sorted,

@@ -133,13 +133,10 @@ def test_public_path_vs_f64(name):
     assert torch.equal(ids_c[fi_c[hit].long()], ids_f[fi_f[hit].long()])
 
 
-@pytest.mark.parametrize("env", [{"B200_BLEND_PACKED": "0"}, {"B200_BLEND_PPL_FWD": "1", "B200_BLEND_PPL_BWD": "1"},
-                                 {"B200_BLEND_PPL_FWD": "4", "B200_BLEND_PPL_BWD": "4"}],
-                         ids=["scalar_two_pixel", "one_pixel", "four_pixel"])
+@pytest.mark.parametrize("env", [{"B200_BLEND_PPL_FWD": "1", "B200_BLEND_PPL_BWD": "1"}], ids=["one_pixel"])
 def test_blend_kernel_variants_vs_f64(env):
-    """The kernel families selected once per process by environment (api.cu): the scalar two-pixel kernels, the
-    one-pixel kernels at block_width 16 and the experimental four-pixel kernels, each through test_raw_kernels_vs_f64
-    in a child process."""
+    """The one-pixel kernels, which otherwise only run on tiles smaller than 16, forced at block_width 16 by the test
+    switch read once per process (api.cu), through test_raw_kernels_vs_f64 in a child process."""
     r = subprocess.run([sys.executable, "-m", "pytest", os.path.abspath(__file__), "-q", "-x", "-m", "gpu", "-p",
                         "no:cacheprovider", "-k", "test_raw_kernels_vs_f64"], env=dict(os.environ, **env),
                        capture_output=True, text=True, timeout=1200)

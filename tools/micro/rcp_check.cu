@@ -1,5 +1,5 @@
-// Does MUFU.RCP return exactly 1 for 1, and MUFU.EX2 exactly 1 for -0?  (masked pixels of the blend backward rely on it when
-// B200_BWD_T_SELECT=0).  nvcc -arch=sm_90a -o rcp_check rcp_check.cu && ./rcp_check
+// Does MUFU.RCP return exactly 1 for 1, and MUFU.EX2 exactly 1 for -0?  The paired blend backward relies on it: a masked
+// pixel's transmittance is kept only because T * rcp.approx(1 - 0) == T.  nvcc -arch=sm_90a -o rcp_check rcp_check.cu && ./rcp_check
 #include <cstdio>
 #include <cstring>
 __global__ void k(float *out, float one, float nzero) {
