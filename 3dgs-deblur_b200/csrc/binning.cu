@@ -13,6 +13,24 @@
 
 namespace b200 {
 
+// The reference's tile rectangle of a Gaussian (int radius r around centre c; forward.cu:90-104) and how many of its
+// tiles get a list slot: the rectangle's area, at most `cap` (the slots the scan reserved for it).  The reserved slots
+// beyond that are the reference's "phantom" entries.  All four fields are 0 when r <= 0 or cap <= 0.  Every binning
+// kernel takes the rectangle from here, so the lists agree on which slots are phantoms.
+struct TileRect {
+    int x0, y0, w, emitted;
+};
+__device__ __forceinline__ TileRect ref_tile_rect(const float2 &c, int r, int cap, int tbx, int tby, float bw) {
+    TileRect t = {0, 0, 0, 0};
+    if (r > 0 && cap > 0) {
+        int x1, y1;
+        tile_bbox(c.x, c.y, (float)r, tbx, tby, bw, t.x0, t.y0, x1, y1);
+        t.w = x1 - t.x0;
+        t.emitted = min(max(0, t.w * (y1 - t.y0)), cap);
+    }
+    return t;
+}
+
 // One warp per Gaussian: lanes stride over the Gaussian's tile rectangle, so a screen-filling splat
 // (thousands of tiles) is emitted with coalesced 8-byte / 4-byte stores instead of one thread looping.
 // Slots reserved by the scan but not covered by the int-radius bbox (the reference's "phantom"
@@ -31,18 +49,12 @@ __global__ void __launch_bounds__(256) map_intersects_kernel(int n, const float2
     const int idx = warp;
     const int start = idx == 0 ? 0 : cum[idx - 1];
     const int end = min(cum[idx], num_intersects);
-    int emitted = 0;
-    const int r = radii[idx];
-    if (r > 0) {
-        const float2 c = xys[idx];
-        int x0, y0, x1, y1;
-        tile_bbox(c.x, c.y, (float)r, tbx, tby, bw, x0, y0, x1, y1);
-        const int w = x1 - x0;
-        emitted = max(0, w * (y1 - y0));
-        emitted = min(emitted, max(0, end - start));
+    const TileRect t = ref_tile_rect(xys[idx], radii[idx], end - start, tbx, tby, bw);
+    const int emitted = t.emitted;
+    if (emitted > 0) {
         const int64_t depth_id = (int64_t)__float_as_int(depths[idx]);
         for (int k = lane; k < emitted; k += 32) {
-            const int ty = y0 + k / w, tx = x0 + k % w;
+            const int ty = t.y0 + k / t.w, tx = t.x0 + k % t.w;
             const int64_t tile = (int64_t)ty * tbx + tx;
             isect_ids[start + k] = (tile << 32) | depth_id;
             gaussian_ids[start + k] = idx;
@@ -85,24 +97,17 @@ __global__ void __launch_bounds__(256) depth_keys_kernel(int n, const float2 *__
                                                          int32_t *__restrict__ vals, int32_t *__restrict__ emitted) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const int r = radii[i], reserved = tiles_hit[i];
-    int e = 0;
-    if (r > 0 && reserved > 0) {
-        const float2 c = xys[i];
-        int x0, y0, x1, y1;
-        tile_bbox(c.x, c.y, (float)r, tbx, tby, bw, x0, y0, x1, y1);
-        e = min(max(0, (x1 - x0) * (y1 - y0)), reserved);
-    }
+    const int e = ref_tile_rect(xys[i], radii[i], tiles_hit[i], tbx, tby, bw).emitted;
     emitted[i] = e;
     keys[i] = e > 0 ? (uint32_t)__float_as_int(depths[i]) : 0xffffffffu;
     vals[i] = i;
 }
 
-__global__ void __launch_bounds__(256) gather_counts_kernel(int n, const int32_t *__restrict__ order,
-                                                            const int32_t *__restrict__ emitted,
-                                                            int32_t *__restrict__ emitted_sorted) {
+// per-Gaussian values in depth order: out[i] = in[order[i]]
+__global__ void __launch_bounds__(256) gather_by_order_kernel(int n, const int32_t *__restrict__ order,
+                                                              const int32_t *__restrict__ in, int32_t *__restrict__ out) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) emitted_sorted[i] = emitted[order[i]];
+    if (i < n) out[i] = in[order[i]];
 }
 
 // one warp per depth-sorted Gaussian; the first warps also zero-fill the phantom prefix
@@ -157,35 +162,35 @@ __global__ void __launch_bounds__(256) tile_bin_edges32_kernel(int m, const uint
     }
 }
 
-static size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
+// Carves a workspace into consecutive buffers, each starting on a 256-byte boundary; `off` ends as the total size.
+struct WsCarver {
+    size_t off = 0;
+    size_t take(size_t bytes) {
+        const size_t o = off;
+        off += (bytes + 255) & ~(size_t)255;
+        return o;
+    }
+};
 
 // cub's temp-size queries run its whole dispatch prologue (device / occupancy attribute look-ups); the culled path
 // asks for the same sizes every step, right after its host sync while the GPU is waiting.  Sizes are memoised per item
 // count, counts rounded up to 64 Ki items (temp storage grows with the item count, so the rounded size is sufficient).
+enum CubQuery { SORT32, SCAN32 };
 static int round_items(int n) { return n <= 0 ? 65536 : (int)std::min<long long>(((long long)n + 65535) & ~65535ll, 0x7fffffffll); }
-static size_t sort32_temp_bytes(int n) {
+static size_t cub_temp_bytes(CubQuery q, int n) {
     static std::mutex mu;
-    static std::map<int, size_t> memo;
-    const int key = round_items(n);
+    static std::map<std::pair<CubQuery, int>, size_t> memo;
+    const std::pair<CubQuery, int> key(q, round_items(n));
     std::lock_guard<std::mutex> lock(mu);
     auto it = memo.find(key);
     if (it != memo.end()) return it->second;
     size_t b = 0;
-    cub::DeviceRadixSort::SortPairs((void *)nullptr, b, (const uint32_t *)nullptr, (uint32_t *)nullptr,
-                                    (const int32_t *)nullptr, (int32_t *)nullptr, key, 0, 32);
+    if (q == SORT32)
+        cub::DeviceRadixSort::SortPairs((void *)nullptr, b, (const uint32_t *)nullptr, (uint32_t *)nullptr,
+                                        (const int32_t *)nullptr, (int32_t *)nullptr, key.second, 0, 32);
+    else
+        cub::DeviceScan::ExclusiveSum((void *)nullptr, b, (const int32_t *)nullptr, (int32_t *)nullptr, key.second);
     if (b) memo[key] = b;  // (0 = no device: do not cache)
-    return b;
-}
-static size_t scan32_temp_bytes(int n) {
-    static std::mutex mu;
-    static std::map<int, size_t> memo;
-    const int key = round_items(n);
-    std::lock_guard<std::mutex> lock(mu);
-    auto it = memo.find(key);
-    if (it != memo.end()) return it->second;
-    size_t b = 0;
-    cub::DeviceScan::ExclusiveSum((void *)nullptr, b, (const int32_t *)nullptr, (int32_t *)nullptr, key);
-    if (b) memo[key] = b;
     return b;
 }
 
@@ -195,16 +200,14 @@ struct BinTilesLayout {
 
 static BinTilesLayout bin_tiles_layout(int n, int m) {
     BinTilesLayout L;
-    size_t off = 0;
-    auto take = [&](size_t bytes) { size_t o = off; off += align256(bytes); return o; };
-    L.keys_a = take(4 * (size_t)n); L.keys_b = take(4 * (size_t)n);
-    L.vals_a = take(4 * (size_t)n); L.vals_b = take(4 * (size_t)n);
-    L.emitted = take(4 * (size_t)n); L.emitted_sorted = take(4 * (size_t)n); L.offs = take(4 * (size_t)n);
-    L.tkeys_a = take(4 * (size_t)m); L.tkeys_b = take(4 * (size_t)m); L.ids_a = take(4 * (size_t)m);
-    const size_t b1 = sort32_temp_bytes(n), b2 = sort32_temp_bytes(m > 0 ? m : 1), b3 = scan32_temp_bytes(n);
-    L.cub_bytes = b1 > b2 ? (b1 > b3 ? b1 : b3) : (b2 > b3 ? b2 : b3);
-    L.cub = take(L.cub_bytes + 256);
-    L.total = off;
+    WsCarver ws;
+    L.keys_a = ws.take(4 * (size_t)n); L.keys_b = ws.take(4 * (size_t)n);
+    L.vals_a = ws.take(4 * (size_t)n); L.vals_b = ws.take(4 * (size_t)n);
+    L.emitted = ws.take(4 * (size_t)n); L.emitted_sorted = ws.take(4 * (size_t)n); L.offs = ws.take(4 * (size_t)n);
+    L.tkeys_a = ws.take(4 * (size_t)m); L.tkeys_b = ws.take(4 * (size_t)m); L.ids_a = ws.take(4 * (size_t)m);
+    L.cub_bytes = std::max({cub_temp_bytes(SORT32, n), cub_temp_bytes(SORT32, m > 0 ? m : 1), cub_temp_bytes(SCAN32, n)}) + 256;
+    L.cub = ws.take(L.cub_bytes);
+    L.total = ws.off;
     return L;
 }
 
@@ -272,25 +275,16 @@ __device__ __forceinline__ bool tile_survives(const PackedGaussian &g, int tx, i
 
 // Depth-sort keys of the culled binning: the depth bits of every Gaussian that reserves at least one real tile slot (the
 // same `emitted_ref > 0` as cull_prep_kernel), 0xffffffff for the rest.  Its own tiny kernel so that the depth sort -- the
-// longest chain of the binning (histogram + 4 onesweep passes) -- can start on the side stream BEFORE cull_prep / scan /
-// count instead of after cull_prep (B200_CULL_EARLY_SORT=0: keys written by cull_prep_kernel, sort forked after it).
-#ifndef B200_CULL_EARLY_SORT
-#define B200_CULL_EARLY_SORT 1
-#endif
+// longest chain of the binning (histogram + 4 onesweep passes) -- can start on the side stream before cull_prep, the scan
+// and the count pass.
 __global__ void __launch_bounds__(256) cull_keys_kernel(int n, const PackedGaussian *__restrict__ rec,
                                                         const float *__restrict__ depths, const int32_t *__restrict__ radii,
                                                         const int32_t *__restrict__ tiles_hit, int tbx, int tby, int bw,
                                                         uint32_t *__restrict__ keys, int32_t *__restrict__ vals) {
     const int g = blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= n) return;
-    const int r = radii[g], reserved = tiles_hit[g];
-    int emitted_ref = 0;
-    if (r > 0 && reserved > 0) {
-        const float2 xy = *reinterpret_cast<const float2 *>(&rec[g].x);
-        int x0, y0, x1, y1;
-        tile_bbox(xy.x, xy.y, (float)r, tbx, tby, (float)bw, x0, y0, x1, y1);
-        emitted_ref = min(max(0, (x1 - x0) * (y1 - y0)), reserved);
-    }
+    const int emitted_ref =
+        ref_tile_rect(*reinterpret_cast<const float2 *>(&rec[g].x), radii[g], tiles_hit[g], tbx, tby, (float)bw).emitted;
     keys[g] = emitted_ref > 0 ? (uint32_t)__float_as_int(depths[g]) : 0xffffffffu;
     vals[g] = g;
 }
@@ -301,35 +295,22 @@ __global__ void __launch_bounds__(256) cull_keys_kernel(int n, const PackedGauss
 // one warp per chunk, chunk -> Gaussian by binary search in the chunk prefix sum, so a handful of huge splats
 // cannot serialise the pass.
 __global__ void __launch_bounds__(256) cull_prep_kernel(int n, const PackedGaussian *__restrict__ rec,
-                                                        const float *__restrict__ depths,
                                                         const int32_t *__restrict__ radii,
                                                         const int32_t *__restrict__ tiles_hit, CullGeom c,
-                                                        uint32_t *__restrict__ keys, int32_t *__restrict__ vals,
                                                         int4 *__restrict__ bbox, int32_t *__restrict__ chunks,
                                                         int32_t *__restrict__ survivors, int32_t *__restrict__ cursor,
                                                         int32_t *__restrict__ counters) {
     const int g = blockIdx.x * blockDim.x + threadIdx.x;
     int reserved = 0, phantom = 0;
     if (g < n) {
-        const int r = radii[g];
         reserved = tiles_hit[g];
-        int x0 = 0, y0 = 0, w = 0, emitted_ref = 0;
-        if (r > 0 && reserved > 0) {
-            const float2 xy = *reinterpret_cast<const float2 *>(&rec[g].x);
-            int x1, y1;
-            tile_bbox(xy.x, xy.y, (float)r, c.tbx, c.tby, (float)c.bw, x0, y0, x1, y1);
-            w = x1 - x0;
-            emitted_ref = min(max(0, w * (y1 - y0)), reserved);
-        }
-        bbox[g] = make_int4(x0, y0, w, emitted_ref);
-        chunks[g] = (emitted_ref + 31) >> 5;
+        const TileRect t =
+            ref_tile_rect(*reinterpret_cast<const float2 *>(&rec[g].x), radii[g], reserved, c.tbx, c.tby, (float)c.bw);
+        bbox[g] = make_int4(t.x0, t.y0, t.w, t.emitted);
+        chunks[g] = (t.emitted + 31) >> 5;
         survivors[g] = 0;
         cursor[g] = 0;
-#if !B200_CULL_EARLY_SORT
-        keys[g] = emitted_ref > 0 ? (uint32_t)__float_as_int(depths[g]) : 0xffffffffu;
-        vals[g] = g;
-#endif
-        phantom = max(0, reserved - emitted_ref);
+        phantom = max(0, reserved - t.emitted);
         if (g == 0) counters[2] = (c.per_sample ? tile_survives<true>(rec[0], 0, 0, c) : tile_survives<false>(rec[0], 0, 0, c)) ? 1 : 0;
     }
     reserved = __reduce_add_sync(0xffffffffu, reserved);
@@ -463,14 +444,6 @@ __global__ void __launch_bounds__(256, 8) cull_chunks_kernel(int n, int total_en
     }
 }
 
-// survivors in depth order
-__global__ void __launch_bounds__(256) gather_survivors_kernel(int n, const int32_t *__restrict__ order,
-                                                               const int32_t *__restrict__ survivors,
-                                                               int32_t *__restrict__ surv_sorted) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) surv_sorted[i] = survivors[order[i]];
-}
-
 // Gaussian -> first slot of its entries (depth order), and the culled entry total for the host
 __global__ void __launch_bounds__(256) cull_finish_kernel(int n, const int32_t *__restrict__ order,
                                                           const int32_t *__restrict__ offs,
@@ -491,6 +464,17 @@ static int key_end_bit(int num_tiles) {
     int bits = 0;
     while ((1ll << bits) < (long long)num_tiles) ++bits;
     return 32 + bits;
+}
+
+// Last step of the 32-bit binnings: stable sort of the m (tile key, Gaussian id) pairs on the low `bits` key bits, then
+// each tile's [start, end) range of the sorted ids into tile_bins (zeroed by the caller).
+static int sort_to_bins(int m, int bits, int num_tiles, uint32_t *tkeys_a, uint32_t *tkeys_b, int32_t *ids_a,
+                        int32_t *gaussian_ids_sorted, int32_t *tile_bins, void *cub_ws, size_t cub_bytes, cudaStream_t st) {
+    B200_CUDA(cub::DeviceRadixSort::SortPairs(cub_ws, cub_bytes, tkeys_a, tkeys_b, ids_a, gaussian_ids_sorted, m, 0, bits, st));
+    count_launch(1 + (bits + 7) / 8);  // onesweep: histogram + one pass per 8-bit digit
+    tile_bin_edges32_kernel<<<ceil_div(m, 256), 256, 0, st>>>(m, tkeys_b, reinterpret_cast<int2 *>(tile_bins), num_tiles);
+    B200_LAUNCH_CHECK();
+    return B200_OK;
 }
 
 }  // namespace b200
@@ -601,7 +585,7 @@ extern "C" int b200_bin_tiles(int num_points, int num_intersects, const float *x
     uint32_t *tkeys_a = (uint32_t *)(base + L.tkeys_a), *tkeys_b = (uint32_t *)(base + L.tkeys_b);
     int32_t *ids_a = (int32_t *)(base + L.ids_a);
     void *cub_ws = base + L.cub;
-    size_t cub_bytes = L.cub_bytes + 256;
+    size_t cub_bytes = L.cub_bytes;
     const int n = num_points, m = num_intersects;
     const int tbx = (int)tiles_x, tby = (int)tiles_y;
     const float bw = (float)block_width;
@@ -611,7 +595,7 @@ extern "C" int b200_bin_tiles(int num_points, int num_intersects, const float *x
     B200_LAUNCH_CHECK();
     B200_CUDA(cub::DeviceRadixSort::SortPairs(cub_ws, cub_bytes, keys_a, keys_b, vals_a, order, n, 0, 32, st));
     count_launch(5);
-    gather_counts_kernel<<<ceil_div(n, 256), 256, 0, st>>>(n, order, emitted, emitted_sorted);
+    gather_by_order_kernel<<<ceil_div(n, 256), 256, 0, st>>>(n, order, emitted, emitted_sorted);
     B200_LAUNCH_CHECK();
     B200_CUDA(cub::DeviceScan::ExclusiveSum(cub_ws, cub_bytes, emitted_sorted, offs, n, st));
     count_launch(2);
@@ -622,13 +606,8 @@ extern "C" int b200_bin_tiles(int num_points, int num_intersects, const float *x
                                                                         tby, bw, tkeys_a, ids_a);
         B200_LAUNCH_CHECK();
     }
-    int bits = key_end_bit(num_tiles) - 32;
-    if (bits < 1) bits = 1;
-    B200_CUDA(cub::DeviceRadixSort::SortPairs(cub_ws, cub_bytes, tkeys_a, tkeys_b, ids_a, gaussian_ids_sorted, m, 0, bits, st));
-    count_launch(1 + (bits + 7) / 8);
-    tile_bin_edges32_kernel<<<ceil_div(m, 256), 256, 0, st>>>(m, tkeys_b, reinterpret_cast<int2 *>(tile_bins), num_tiles);
-    B200_LAUNCH_CHECK();
-    return B200_OK;
+    return sort_to_bins(m, std::max(1, key_end_bit(num_tiles) - 32), num_tiles, tkeys_a, tkeys_b, ids_a, gaussian_ids_sorted,
+                        tile_bins, cub_ws, cub_bytes, st);
 }
 
 // ---- culled binning entry points ---------------------------------------------------------------------------
@@ -652,21 +631,19 @@ static int cull_mask_cap(int n) {
 }
 static CullWsG cull_ws_g(int n) {
     CullWsG L;
-    size_t off = 0;
-    auto take = [&](size_t bytes) { size_t o = off; off += align256(bytes); return o; };
-    L.keys_a = take(4 * (size_t)n); L.keys_b = take(4 * (size_t)n); L.vals_a = take(4 * (size_t)n);
-    L.order = take(4 * (size_t)n); L.survivors = take(4 * (size_t)n); L.surv_sorted = take(4 * (size_t)n);
-    L.offs = take(4 * (size_t)n); L.bbox = take(16 * (size_t)n); L.chunks = take(4 * (size_t)n);
-    L.chunk_off = take(4 * (size_t)n); L.cursor = take(4 * (size_t)n); L.base_of = take(4 * (size_t)n);
-    L.counters = take(256);
+    WsCarver ws;
+    L.keys_a = ws.take(4 * (size_t)n); L.keys_b = ws.take(4 * (size_t)n); L.vals_a = ws.take(4 * (size_t)n);
+    L.order = ws.take(4 * (size_t)n); L.survivors = ws.take(4 * (size_t)n); L.surv_sorted = ws.take(4 * (size_t)n);
+    L.offs = ws.take(4 * (size_t)n); L.bbox = ws.take(16 * (size_t)n); L.chunks = ws.take(4 * (size_t)n);
+    L.chunk_off = ws.take(4 * (size_t)n); L.cursor = ws.take(4 * (size_t)n); L.base_of = ws.take(4 * (size_t)n);
+    L.counters = ws.take(256);
     L.mask_cap = cull_mask_cap(n);
-    L.masks = take(4 * (size_t)(L.mask_cap > 0 ? L.mask_cap : 1));
-    const size_t b1 = sort32_temp_bytes(n), b3 = scan32_temp_bytes(n);
-    L.cub_bytes = b1 + 256;  // depth sort (side stream)
-    L.cub = take(L.cub_bytes);
-    L.cub_scan_bytes = b3 + 256;  // the two scans (main stream), concurrent with the sort
-    L.cub_scan = take(L.cub_scan_bytes);
-    L.total = off;
+    L.masks = ws.take(4 * (size_t)(L.mask_cap > 0 ? L.mask_cap : 1));
+    L.cub_bytes = cub_temp_bytes(SORT32, n) + 256;  // depth sort (side stream)
+    L.cub = ws.take(L.cub_bytes);
+    L.cub_scan_bytes = cub_temp_bytes(SCAN32, n) + 256;  // the two scans (main stream), concurrent with the sort
+    L.cub_scan = ws.take(L.cub_scan_bytes);
+    L.total = ws.off;
     return L;
 }
 struct CullWsE {
@@ -674,13 +651,11 @@ struct CullWsE {
 };
 static CullWsE cull_ws_e(int m) {
     CullWsE L;
-    size_t off = 0;
-    auto take = [&](size_t bytes) { size_t o = off; off += align256(bytes); return o; };
-    L.tkeys_a = take(4 * (size_t)m); L.tkeys_b = take(4 * (size_t)m); L.ids_a = take(4 * (size_t)m);
-    const size_t b2 = sort32_temp_bytes(m);
-    L.cub_bytes = b2 + 256;
-    L.cub = take(L.cub_bytes);
-    L.total = off;
+    WsCarver ws;
+    L.tkeys_a = ws.take(4 * (size_t)m); L.tkeys_b = ws.take(4 * (size_t)m); L.ids_a = ws.take(4 * (size_t)m);
+    L.cub_bytes = cub_temp_bytes(SORT32, m) + 256;
+    L.cub = ws.take(L.cub_bytes);
+    L.total = ws.off;
     return L;
 }
 
@@ -719,10 +694,7 @@ static bool side_stream(SideStream &out) {
 constexpr int CULL_GRID = 132 * 8;  // 8 CTAs per SM of an H100 (132 SMs): persistent warps, grid-stride over the chunk list
 // The counting pass runs beside the depth sort (side stream): 8 CTAs of 256 threads per SM would fill every thread slot
 // and the sort's kernels would only start as the count drains -- 6 per SM leave a quarter of each SM to the sort chain.
-#ifndef B200_CULL_COUNT_CTAS
-#define B200_CULL_COUNT_CTAS 6
-#endif
-constexpr int CULL_COUNT_GRID = 132 * B200_CULL_COUNT_CTAS;
+constexpr int CULL_COUNT_GRID = 132 * 6;
 
 static CullGeom make_cull_geom(unsigned H, unsigned W, unsigned bw, unsigned S, float rs, float exposure) {
     CullGeom c;
@@ -770,7 +742,6 @@ extern "C" int b200_bin_cull_count(int num_points, const void *packed, const flo
     SideStream side;
     B200_REQUIRE(side_stream(side), "could not create the binning side stream");
     B200_CUDA(cudaMemsetAsync(counters, 0, 256, st));
-#if B200_CULL_EARLY_SORT
     // the depth sort only needs depths and the visibility of each Gaussian: it is forked first and runs beside cull_prep,
     // the scan and the tile tests (chains of short kernels, the sort's being the longest)
     {
@@ -784,21 +755,8 @@ extern "C" int b200_bin_cull_count(int num_points, const void *packed, const flo
         count_launch(5);
         B200_CUDA(cudaEventRecord(side.join, side.stream));
     }
-#endif
-    cull_prep_kernel<<<ceil_div(n, 256), 256, 0, st>>>(n, rec, depths, radii, num_tiles_hit, c, keys_a, vals_a, bbox, chunks,
-                                                       survivors, cursor, counters);
+    cull_prep_kernel<<<ceil_div(n, 256), 256, 0, st>>>(n, rec, radii, num_tiles_hit, c, bbox, chunks, survivors, cursor, counters);
     B200_LAUNCH_CHECK();
-#if !B200_CULL_EARLY_SORT
-    // the depth sort only needs the keys: it runs beside the scan + tile tests, both are chains of short kernels
-    {
-        std::lock_guard<std::mutex> lock(side_mu);
-        B200_CUDA(cudaEventRecord(side.fork, st));
-        B200_CUDA(cudaStreamWaitEvent(side.stream, side.fork, 0));
-        B200_CUDA(cub::DeviceRadixSort::SortPairs(cub_ws, cub_bytes, keys_a, keys_b, vals_a, order, n, 0, 32, side.stream));
-        count_launch(5);
-        B200_CUDA(cudaEventRecord(side.join, side.stream));
-    }
-#endif
     B200_CUDA(cub::DeviceScan::ExclusiveSum(scan_ws, scan_bytes, chunks, chunk_off, n, st));
     count_launch(2);
     (c.per_sample ? cull_chunks_kernel<false, true> : cull_chunks_kernel<false, false>)<<<CULL_COUNT_GRID, 256, 0, st>>>(
@@ -806,7 +764,7 @@ extern "C" int b200_bin_cull_count(int num_points, const void *packed, const flo
     B200_LAUNCH_CHECK();
     // (a later record of the shared join event by another caller is ordered after this one on the side stream)
     B200_CUDA(cudaStreamWaitEvent(st, side.join, 0));
-    gather_survivors_kernel<<<ceil_div(n, 256), 256, 0, st>>>(n, order, survivors, surv_sorted);
+    gather_by_order_kernel<<<ceil_div(n, 256), 256, 0, st>>>(n, order, survivors, surv_sorted);
     B200_LAUNCH_CHECK();
     B200_CUDA(cub::DeviceScan::ExclusiveSum(scan_ws, scan_bytes, surv_sorted, offs, n, st));
     count_launch(2);
@@ -815,6 +773,28 @@ extern "C" int b200_bin_cull_count(int num_points, const void *packed, const flo
     if (totals_host_pinned)  // (null in the capacity mode: nothing on the host waits for the totals)
         B200_CUDA(cudaMemcpyAsync(totals_host_pinned, counters, 5 * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
     return B200_OK;
+}
+
+// Emit phase of both emit entry points, after their argument checks and the tile_bins memset.  m is the entry count of
+// b200_bin_cull_emit, or the list capacity in the capacity mode (status != nullptr), whose padding key num_tiles must
+// sort too.
+static int cull_emit(int n, int m, const CullGeom &c, const void *packed, const void *ws_g, void *ws_e, size_t ws_e_bytes,
+                     int32_t *gaussian_ids_sorted, int32_t *tile_bins, int32_t *status, cudaStream_t st) {
+    const int num_tiles = c.tbx * c.tby;
+    const CullWsG G = cull_ws_g(n);
+    const CullWsE E = cull_ws_e(m);
+    B200_REQUIRE(ws_e_bytes >= E.total, "workspace too small: %zu < %zu", ws_e_bytes, E.total);
+    char *gb = static_cast<char *>(const_cast<void *>(ws_g));
+    char *eb = static_cast<char *>(ws_e);
+    uint32_t *tkeys_a = (uint32_t *)(eb + E.tkeys_a), *tkeys_b = (uint32_t *)(eb + E.tkeys_b);
+    int32_t *ids_a = (int32_t *)(eb + E.ids_a);
+    (c.per_sample ? cull_chunks_kernel<true, true> : cull_chunks_kernel<true, false>)<<<CULL_GRID, 256, 0, st>>>(
+        n, m, reinterpret_cast<const PackedGaussian *>(packed), (const int4 *)(gb + G.bbox), (const int32_t *)(gb + G.chunk_off),
+        (const int32_t *)(gb + G.chunks), c, (const int32_t *)(gb + G.counters), (uint32_t *)(gb + G.masks), G.mask_cap, nullptr,
+        (const int32_t *)(gb + G.base_of), (int32_t *)(gb + G.cursor), tkeys_a, ids_a, status ? (uint32_t)num_tiles : 0u, status);
+    B200_LAUNCH_CHECK();
+    const int bits = std::max(1, key_end_bit(status ? num_tiles + 1 : num_tiles) - 32);
+    return sort_to_bins(m, bits, num_tiles, tkeys_a, tkeys_b, ids_a, gaussian_ids_sorted, tile_bins, eb + E.cub, E.cub_bytes, st);
 }
 
 extern "C" int b200_bin_cull_emit(int num_points, int num_entries, const void *packed, const int32_t *radii,
@@ -826,39 +806,12 @@ extern "C" int b200_bin_cull_emit(int num_points, int num_entries, const void *p
     B200_REQUIRE(block_width > 1 && block_width <= 16, "block_width must be between 2 and 16");
     B200_REQUIRE(tile_bins && ws_g, "null pointer");
     const CullGeom c = make_cull_geom(img_height, img_width, block_width, n_blur_samples, rolling_shutter_time, exposure_time);
-    const int num_tiles = c.tbx * c.tby;
     cudaStream_t st = as_stream(stream);
-    B200_CUDA(cudaMemsetAsync(tile_bins, 0, sizeof(int32_t) * 2 * (size_t)num_tiles, st));
+    B200_CUDA(cudaMemsetAsync(tile_bins, 0, sizeof(int32_t) * 2 * (size_t)(c.tbx * c.tby), st));
     if (num_entries == 0) return B200_OK;
     B200_REQUIRE(packed && radii && num_tiles_hit && gaussian_ids_sorted && ws_e, "null pointer");
     B200_REQUIRE((reinterpret_cast<uintptr_t>(ws_e) & 255u) == 0, "workspace must be 256-byte aligned");
-    const int n = num_points, m = num_entries;
-    const CullWsG G = cull_ws_g(n);
-    const CullWsE E = cull_ws_e(m);
-    B200_REQUIRE(ws_e_bytes >= E.total, "workspace too small: %zu < %zu", ws_e_bytes, E.total);
-    const char *gb = static_cast<const char *>(ws_g);
-    const int32_t *counters = (const int32_t *)(gb + G.counters);
-    const int4 *bbox = (const int4 *)(gb + G.bbox);
-    const int32_t *chunk_off = (const int32_t *)(gb + G.chunk_off), *base_of = (const int32_t *)(gb + G.base_of);
-    const int32_t *chunks = (const int32_t *)(gb + G.chunks);
-    int32_t *cursor = (int32_t *)(const_cast<char *>(gb) + G.cursor);
-    uint32_t *masks = (uint32_t *)(const_cast<char *>(gb) + G.masks);
-    char *eb = static_cast<char *>(ws_e);
-    uint32_t *tkeys_a = (uint32_t *)(eb + E.tkeys_a), *tkeys_b = (uint32_t *)(eb + E.tkeys_b);
-    int32_t *ids_a = (int32_t *)(eb + E.ids_a);
-    void *cub_ws = eb + E.cub;
-    size_t cub_bytes = E.cub_bytes;
-    (c.per_sample ? cull_chunks_kernel<true, true> : cull_chunks_kernel<true, false>)<<<CULL_GRID, 256, 0, st>>>(
-        n, m, reinterpret_cast<const PackedGaussian *>(packed), bbox, chunk_off, chunks, c, counters, masks, G.mask_cap, nullptr,
-        base_of, cursor, tkeys_a, ids_a, 0u, nullptr);
-    B200_LAUNCH_CHECK();
-    int bits = key_end_bit(num_tiles) - 32;
-    if (bits < 1) bits = 1;
-    B200_CUDA(cub::DeviceRadixSort::SortPairs(cub_ws, cub_bytes, tkeys_a, tkeys_b, ids_a, gaussian_ids_sorted, m, 0, bits, st));
-    count_launch(1 + (bits + 7) / 8);
-    tile_bin_edges32_kernel<<<ceil_div(m, 256), 256, 0, st>>>(m, tkeys_b, reinterpret_cast<int2 *>(tile_bins), num_tiles);
-    B200_LAUNCH_CHECK();
-    return B200_OK;
+    return cull_emit(num_points, num_entries, c, packed, ws_g, ws_e, ws_e_bytes, gaussian_ids_sorted, tile_bins, nullptr, st);
 }
 
 
@@ -881,34 +834,7 @@ extern "C" int b200_bin_cull_emit_capacity(int num_points, int capacity, const v
     B200_REQUIRE(packed && radii && num_tiles_hit && gaussian_ids_sorted && ws_e, "null pointer");
     B200_REQUIRE((reinterpret_cast<uintptr_t>(ws_e) & 255u) == 0, "workspace must be 256-byte aligned");
     const CullGeom c = make_cull_geom(img_height, img_width, block_width, n_blur_samples, rolling_shutter_time, exposure_time);
-    const int num_tiles = c.tbx * c.tby;
     cudaStream_t st = as_stream(stream);
-    B200_CUDA(cudaMemsetAsync(tile_bins, 0, sizeof(int32_t) * 2 * (size_t)num_tiles, st));
-    const int n = num_points, m = capacity;
-    const CullWsG G = cull_ws_g(n);
-    const CullWsE E = cull_ws_e(m);
-    B200_REQUIRE(ws_e_bytes >= E.total, "workspace too small: %zu < %zu", ws_e_bytes, E.total);
-    const char *gb = static_cast<const char *>(ws_g);
-    const int32_t *counters = (const int32_t *)(gb + G.counters);
-    const int4 *bbox = (const int4 *)(gb + G.bbox);
-    const int32_t *chunk_off = (const int32_t *)(gb + G.chunk_off), *base_of = (const int32_t *)(gb + G.base_of);
-    const int32_t *chunks = (const int32_t *)(gb + G.chunks);
-    int32_t *cursor = (int32_t *)(const_cast<char *>(gb) + G.cursor);
-    uint32_t *masks = (uint32_t *)(const_cast<char *>(gb) + G.masks);
-    char *eb = static_cast<char *>(ws_e);
-    uint32_t *tkeys_a = (uint32_t *)(eb + E.tkeys_a), *tkeys_b = (uint32_t *)(eb + E.tkeys_b);
-    int32_t *ids_a = (int32_t *)(eb + E.ids_a);
-    void *cub_ws = eb + E.cub;
-    size_t cub_bytes = E.cub_bytes;
-    (c.per_sample ? cull_chunks_kernel<true, true> : cull_chunks_kernel<true, false>)<<<CULL_GRID, 256, 0, st>>>(
-        n, m, reinterpret_cast<const PackedGaussian *>(packed), bbox, chunk_off, chunks, c, counters, masks, G.mask_cap, nullptr,
-        base_of, cursor, tkeys_a, ids_a, (uint32_t)num_tiles, status);
-    B200_LAUNCH_CHECK();
-    int bits = key_end_bit(num_tiles + 1) - 32;  // the padding key num_tiles must sort too
-    if (bits < 1) bits = 1;
-    B200_CUDA(cub::DeviceRadixSort::SortPairs(cub_ws, cub_bytes, tkeys_a, tkeys_b, ids_a, gaussian_ids_sorted, m, 0, bits, st));
-    count_launch(1 + (bits + 7) / 8);
-    tile_bin_edges32_kernel<<<ceil_div(m, 256), 256, 0, st>>>(m, tkeys_b, reinterpret_cast<int2 *>(tile_bins), num_tiles);
-    B200_LAUNCH_CHECK();
-    return B200_OK;
+    B200_CUDA(cudaMemsetAsync(tile_bins, 0, sizeof(int32_t) * 2 * (size_t)(c.tbx * c.tby), st));
+    return cull_emit(num_points, capacity, c, packed, ws_g, ws_e, ws_e_bytes, gaussian_ids_sorted, tile_bins, status, st);
 }

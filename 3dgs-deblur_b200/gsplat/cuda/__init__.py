@@ -249,6 +249,27 @@ def pack_records(xys, pix_vels, conics, colors, opacities):
     return packed
 
 
+def _bin_cull_count(packed, depths, radii, num_tiles_hit, img_height, img_width, block_width, n_blur_samples,
+                    rolling_shutter_time, exposure_time, totals_host_ptr):
+    """Count phase of bin_cull / bin_cull_capacity on the current device and stream -> (ws_g, bins, emit_args).
+    The deferred quaternion check rides along: its word is copied to the host with the totals when `totals_host_ptr` is
+    given, else it stays on the device (polled by the trainer).  `emit_args` are the arguments both emit entry points
+    take after the entry count; ws_g must outlive the emit call."""
+    lib = _lib.load()
+    dev = depths.device
+    n = depths.numel()
+    H, W, bw, S = int(img_height), int(img_width), int(block_width), int(n_blur_samples)
+    rs, ex = float(rolling_shutter_time), float(exposure_time)
+    ws_bytes = lib.b200_bin_cull_ws_bytes(n)
+    ws_g = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
+    flag = _lib.take_pending_flag(dev)
+    tiles = ((W + bw - 1) // bw) * ((H + bw - 1) // bw)
+    bins = torch.empty((tiles, 2), dtype=torch.int32, device=dev)
+    check(lib.b200_bin_cull_count(n, ptr(packed), ptr(_f32(depths)), ptr(radii), ptr(num_tiles_hit), H, W, bw, S, rs, ex,
+                                  ptr(ws_g), ws_bytes, totals_host_ptr, ptr(flag), stream()))
+    return ws_g, bins, (ptr(packed), ptr(radii), ptr(num_tiles_hit), H, W, bw, S, rs, ex, ptr(ws_g))
+
+
 def bin_cull(packed, depths, radii, num_tiles_hit, img_height, img_width, block_width, n_blur_samples,
              rolling_shutter_time, exposure_time):
     """Extension: culled two-level binning -> (num_intersects_reference, gaussian_ids_sorted (M,), tile_bins (tiles,2)).
@@ -257,17 +278,9 @@ def bin_cull(packed, depths, radii, num_tiles_hit, img_height, img_width, block_
     dev = depths.device
     with on_device(dev):
         lib = _lib.load()
-        n = depths.numel()
-        H, W, bw, S = int(img_height), int(img_width), int(block_width), int(n_blur_samples)
-        rs, ex = float(rolling_shutter_time), float(exposure_time)
-        ws_bytes = lib.b200_bin_cull_ws_bytes(n)
-        ws_g = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
         host_ptr, host = _lib.host_scratch_np(dev)
-        flag = _lib.take_pending_flag(dev)
-        tiles = ((W + bw - 1) // bw) * ((H + bw - 1) // bw)
-        bins = torch.empty((tiles, 2), dtype=torch.int32, device=dev)
-        check(lib.b200_bin_cull_count(n, ptr(packed), ptr(_f32(depths)), ptr(radii), ptr(num_tiles_hit), H, W, bw, S, rs, ex,
-                                      ptr(ws_g), ws_bytes, host_ptr, ptr(flag), stream()))
+        ws_g, bins, emit_args = _bin_cull_count(packed, depths, radii, num_tiles_hit, img_height, img_width, block_width,
+                                                n_blur_samples, rolling_shutter_time, exposure_time, host_ptr)
         torch.cuda.current_stream().synchronize()  # the one host sync of the path
         # (the GPU idles from here until the emit kernels are queued: keep this stretch short)
         if host[4]:
@@ -276,8 +289,7 @@ def bin_cull(packed, depths, radii, num_tiles_hit, img_height, img_width, block_
         ids = torch.empty((m,), dtype=torch.int32, device=dev)
         e_bytes = lib.b200_bin_cull_emit_ws_bytes(m)
         ws_e = torch.empty((e_bytes,), dtype=torch.uint8, device=dev)
-        check(lib.b200_bin_cull_emit(n, m, ptr(packed), ptr(radii), ptr(num_tiles_hit), H, W, bw, S, rs, ex, ptr(ws_g), ptr(ws_e),
-                                     e_bytes, ptr(ids), ptr(bins), stream()))
+        check(lib.b200_bin_cull_emit(depths.numel(), m, *emit_args, ptr(ws_e), e_bytes, ptr(ids), ptr(bins), stream()))
     return total_ref, ids, bins
 
 
@@ -290,22 +302,14 @@ def bin_cull_capacity(packed, depths, radii, num_tiles_hit, img_height, img_widt
     dev = depths.device
     with on_device(dev):
         lib = _lib.load()
-        n = depths.numel()
-        H, W, bw, S = int(img_height), int(img_width), int(block_width), int(n_blur_samples)
-        rs, ex = float(rolling_shutter_time), float(exposure_time)
         cap = int(capacity)
-        ws_bytes = lib.b200_bin_cull_ws_bytes(n)
-        ws_g = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
-        flag = _lib.take_pending_flag(dev)  # the deferred quaternion check stays on the device (polled by the trainer)
-        tiles = ((W + bw - 1) // bw) * ((H + bw - 1) // bw)
-        bins = torch.empty((tiles, 2), dtype=torch.int32, device=dev)
+        ws_g, bins, emit_args = _bin_cull_count(packed, depths, radii, num_tiles_hit, img_height, img_width, block_width,
+                                                n_blur_samples, rolling_shutter_time, exposure_time, None)
         ids = torch.empty((cap,), dtype=torch.int32, device=dev)
-        check(lib.b200_bin_cull_count(n, ptr(packed), ptr(_f32(depths)), ptr(radii), ptr(num_tiles_hit), H, W, bw, S, rs, ex,
-                                      ptr(ws_g), ws_bytes, None, ptr(flag), stream()))
         e_bytes = lib.b200_bin_cull_emit_ws_bytes(cap)
         ws_e = torch.empty((e_bytes,), dtype=torch.uint8, device=dev)
-        check(lib.b200_bin_cull_emit_capacity(n, cap, ptr(packed), ptr(radii), ptr(num_tiles_hit), H, W, bw, S, rs, ex, ptr(ws_g),
-                                              ptr(ws_e), e_bytes, ptr(ids), ptr(bins), ptr(status), stream()))
+        check(lib.b200_bin_cull_emit_capacity(depths.numel(), cap, *emit_args, ptr(ws_e), e_bytes, ptr(ids), ptr(bins),
+                                              ptr(status), stream()))
     return ids, bins
 
 

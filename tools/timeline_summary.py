@@ -17,7 +17,7 @@ CLASSES = [
     ("nccl", ("ncclDevKernel",)), ("adam", ("adam_state", "adam_prepare", "adam_kernel")),
     ("projection/sh", ("fused_forward", "fused_backward", "fused_colors", "project_forward", "project_backward", "sh_forward",
                        "sh_backward", "set_record_colors", "pack_records")),
-    ("binning", ("cull_", "DeviceRadixSort", "DeviceScan", "gather_survivors", "tile_bin_edges", "memset32")),
+    ("binning", ("cull_", "DeviceRadixSort", "DeviceScan", "gather_by_order","tile_bin_edges", "memset32")),
     ("loss", ("l1_loss", "ssim")), ("copies/memsets", ("Memcpy", "Memset", "memcpy32")), ("torch glue", ("at::native",)),
 ]
 
