@@ -162,22 +162,11 @@ __global__ void __launch_bounds__(256) tile_bin_edges32_kernel(int m, const uint
     }
 }
 
-// Carves a workspace into consecutive buffers, each starting on a 256-byte boundary; `off` ends as the total size.
-struct WsCarver {
-    size_t off = 0;
-    size_t take(size_t bytes) {
-        const size_t o = off;
-        off += (bytes + 255) & ~(size_t)255;
-        return o;
-    }
-};
-
 // cub's temp-size queries run its whole dispatch prologue (device / occupancy attribute look-ups); the culled path
 // asks for the same sizes every step, right after its host sync while the GPU is waiting.  Sizes are memoised per item
 // count, counts rounded up to 64 Ki items (temp storage grows with the item count, so the rounded size is sufficient).
-enum CubQuery { SORT32, SCAN32 };
 static int round_items(int n) { return n <= 0 ? 65536 : (int)std::min<long long>(((long long)n + 65535) & ~65535ll, 0x7fffffffll); }
-static size_t cub_temp_bytes(CubQuery q, int n) {
+size_t cub_temp_bytes(CubQuery q, int n) {
     static std::mutex mu;
     static std::map<std::pair<CubQuery, int>, size_t> memo;
     const std::pair<CubQuery, int> key(q, round_items(n));
@@ -460,15 +449,16 @@ __global__ void __launch_bounds__(256) cull_finish_kernel(int n, const int32_t *
     }
 }
 
-static int key_end_bit(int num_tiles) {
+int key_end_bit(int num_tiles) {
     int bits = 0;
     while ((1ll << bits) < (long long)num_tiles) ++bits;
     return 32 + bits;
 }
 
 // Last step of the 32-bit binnings: stable sort of the m (tile key, Gaussian id) pairs on the low `bits` key bits, then
-// each tile's [start, end) range of the sorted ids into tile_bins (zeroed by the caller).
-static int sort_to_bins(int m, int bits, int num_tiles, uint32_t *tkeys_a, uint32_t *tkeys_b, int32_t *ids_a,
+// each tile's [start, end) range of the sorted ids into tile_bins (zeroed by the caller).  The deterministic blend
+// backward (blend_bwd.cu) reuses it with (Gaussian id, list position) pairs to group list positions by Gaussian.
+int sort_to_bins(int m, int bits, int num_tiles, uint32_t *tkeys_a, uint32_t *tkeys_b, int32_t *ids_a,
                         int32_t *gaussian_ids_sorted, int32_t *tile_bins, void *cub_ws, size_t cub_bytes, cudaStream_t st) {
     B200_CUDA(cub::DeviceRadixSort::SortPairs(cub_ws, cub_bytes, tkeys_a, tkeys_b, ids_a, gaussian_ids_sorted, m, 0, bits, st));
     count_launch(1 + (bits + 7) / 8);  // onesweep: histogram + one pass per 8-bit digit

@@ -16,6 +16,8 @@
 //   * the same per-warp rectangle cull and TMA-bulk staged 64-byte records as the forward, and the same
 //     longest-list-first CTA order (blend_fwd.cu: tile_order_kernel).
 // Bound: FP32 issue, MUFU, LSU and L2 atomic throughput -- not HBM; see DESIGN.md section 4.
+#include <algorithm>
+
 #include "blend_common.cuh"
 
 namespace b200 {
@@ -32,7 +34,10 @@ struct BlendBwdParams {
     const float *v_out;        // (H,W,3)
     const float *v_out_alpha;  // (H,W), or null for a zero cotangent
     float *v_xy, *v_xy_abs, *v_pix_vel, *v_conic, *v_rgb, *v_opac;
+    float *slots;  // DET kernels only: the 13 sums of each warp visit, at (list position, warp) (b200_blend_backward_packed_deterministic)
 };
+
+constexpr int RED_VALUES = 13;  // rgb 3, conic 3, xy 2, |xy| 2, pixel velocity 2, opacity 1
 
 // The warp reduction leaves per-Gaussian sum k (rgb 3, conic 3, xy 2, |xy| 2, pixel velocity 2, opacity 1) on lane 2k,
 // which adds it at dst[id * stride] of the array returned here; the other lanes get null.
@@ -83,7 +88,8 @@ __device__ __forceinline__ float butterfly16(const float (&v)[16], int lane) {
 }
 
 // ---- one pixel per lane: tiles other than 16x16 ---------------------------------------------------------------------
-template <int S>
+// DET: the visit epilogue stores its sums to p.slots instead of adding them to the gradient arrays (deterministic mode)
+template <int S, bool DET>
 __global__ void __launch_bounds__(BLEND_THREADS, 3) blend_backward_kernel(const BlendBwdParams p) {
     __shared__ __align__(128) PackedGaussian s_rec[BLEND_STAGES][BLEND_BATCH];
     __shared__ __align__(8) uint64_t s_bar[BLEND_STAGES];
@@ -220,7 +226,9 @@ __global__ void __launch_bounds__(BLEND_THREADS, 3) blend_backward_kernel(const 
                     const float v[16] = {vr, vg, vb, 0.5f * sxx, sxy, 0.5f * syy, gxs, gys, gxa, gya, pvx, pvy, vop,
                                          0.f, 0.f, 0.f};
                     const float tot = butterfly16(v, lane);
-                    if (my_dst && tot != 0.f) {
+                    if constexpr (DET) {
+                        if (my_dst) p.slots[((size_t)idx * (BLEND_THREADS / 32) + warp) * RED_VALUES + (lane >> 1)] = tot;
+                    } else if (my_dst && tot != 0.f) {
                         const int gid = s_rec[st][k].id;
                         atomicAdd(my_dst + (unsigned)gid * (unsigned)my_stride, tot);  // N * 3 < 2^32
                     }
@@ -242,11 +250,11 @@ __global__ void __launch_bounds__(BLEND_THREADS, 3) blend_backward_kernel(const 
 //     `alpha` (then fac, v_sigma and every accumulated term are exactly 0, and T is kept because rcp.approx(1) == 1
 //     exactly: tools/micro/rcp_check.cu checks it on the device).  With VOTE, one warp vote per sample skips the gradient
 //     algebra when no lane passes (launch_bwd).
-// Visit epilogue: the 13 per-Gaussian sums are reduced over the warp through a shared-memory transposition.
-constexpr int RED_VALUES = 13;  // rgb 3, conic 3, xy 2, |xy| 2, pixel velocity 2, opacity 1
+// Visit epilogue: the 13 per-Gaussian sums are reduced over the warp through a shared-memory transposition.  DET as in
+// blend_backward_kernel.
 constexpr int RED_STRIDE = 36;  // floats per row: 32 lanes + 4 of padding (rows stay 16-byte aligned, halves hit distinct banks)
 constexpr int BWD_MIN_CTAS = 5;  // 96 registers
-template <int S, bool VOTE>
+template <int S, bool VOTE, bool DET>
 __global__ void __launch_bounds__(128, BWD_MIN_CTAS) blend_backward_kernel2(const BlendBwdParams p) {
     constexpr int NT = 128;
     __shared__ __align__(128) PackedGaussian s_rec[BLEND_STAGES][BLEND_BATCH];
@@ -475,7 +483,9 @@ __global__ void __launch_bounds__(128, BWD_MIN_CTAS) blend_backward_kernel2(cons
                     }
                     tot += __shfl_xor_sync(0xffffffffu, tot, 1);
                     __syncwarp();  // every lane has read its half before the next visit overwrites the rows
-                    if (my_dst && tot != 0.f) {
+                    if constexpr (DET) {
+                        if (my_dst) p.slots[((size_t)idx * (NT / 32) + warp) * RED_VALUES + (lane >> 1)] = tot;
+                    } else if (my_dst && tot != 0.f) {
                         const int gid = s_rec[st][k].id;
                         atomicAdd(my_dst + (unsigned)gid * (unsigned)my_stride, tot);  // N * 3 < 2^32
                     }
@@ -487,21 +497,82 @@ __global__ void __launch_bounds__(128, BWD_MIN_CTAS) blend_backward_kernel2(cons
     B200_COUNT_FLUSH(8);
 }
 
-template <int S>
+static bool paired_bwd(unsigned block_width) { return block_width == 16 && !blend_force_one_pixel(true); }
+
+// warps per CTA of the backward kernel launch_bwd runs: the slots per list position of the deterministic mode
+static int bwd_warps(unsigned block_width) { return paired_bwd(block_width) ? BLEND_THREADS / 2 / 32 : BLEND_THREADS / 32; }
+
+template <int S, bool DET>
 static int launch_bwd(const BlendBwdParams &p, cudaStream_t st) {
-    if (p.g.bw == 16 && !blend_force_one_pixel(true)) {
+    if (paired_bwd(p.g.bw)) {
         // per-sample votes ("does any lane hold a contributing pixel", then skip the gradient algebra): without rolling
         // shutter the exact cull leaves 4 % of the entered sample blocks empty and the vote + branch costs more than the
         // masked arithmetic; with it the warp's time window widens the cull and the skip pays
         if (p.g.rs_time != 0.f)
-            blend_backward_kernel2<S, true><<<p.g.tbx * p.g.tby, BLEND_THREADS / 2, 0, st>>>(p);
+            blend_backward_kernel2<S, true, DET><<<p.g.tbx * p.g.tby, BLEND_THREADS / 2, 0, st>>>(p);
         else
-            blend_backward_kernel2<S, false><<<p.g.tbx * p.g.tby, BLEND_THREADS / 2, 0, st>>>(p);
+            blend_backward_kernel2<S, false, DET><<<p.g.tbx * p.g.tby, BLEND_THREADS / 2, 0, st>>>(p);
     } else {
-        blend_backward_kernel<S><<<p.g.tbx * p.g.tby, BLEND_THREADS, 0, st>>>(p);
+        blend_backward_kernel<S, DET><<<p.g.tbx * p.g.tby, BLEND_THREADS, 0, st>>>(p);
     }
     B200_LAUNCH_CHECK();
     return B200_OK;
+}
+
+// ---- deterministic mode: per-Gaussian sums in a fixed order ------------------------------------------------------------
+// The DET kernels store each warp visit's 13 sums at slot (list position, warp); every list entry belongs to one tile
+// and is visited by each warp of that CTA at most once, so no two writers share a slot.  The positions are then grouped
+// by Gaussian (stable sort of (Gaussian id, position) pairs: ascending position within a Gaussian) and each Gaussian's
+// slots are summed in ascending position, then ascending warp.  The result depends on the lists and the inputs only,
+// not on the CTA order or scheduling.
+
+// key = Gaussian id of list position i, or num_points (sorts last, opens no range) for capacity-mode padding
+__global__ void __launch_bounds__(256) det_keys_kernel(int m, int num_points, const int32_t *__restrict__ ids,
+                                                       const int32_t *__restrict__ status, uint32_t *__restrict__ keys,
+                                                       int32_t *__restrict__ pos) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= m) return;
+    const int real = status ? min(max(__ldg(status + 1), 0), m) : m;
+    keys[i] = i < real ? (uint32_t)__ldg(ids + i) : (uint32_t)num_points;
+    pos[i] = i;
+}
+
+// 16 threads per Gaussian, thread k < 13 owns sum k (grad_lane_dst of lane 2k); every Gaussian's row is written
+__global__ void __launch_bounds__(256) det_reduce_kernel(int num_points, int warps, const float *__restrict__ slots,
+                                                         const int32_t *__restrict__ pos_sorted,
+                                                         const int2 *__restrict__ seg, float *v_rgb, float *v_conic,
+                                                         float *v_xy, float *v_xy_abs, float *v_pix_vel, float *v_opac) {
+    const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const int g = (int)(t >> 4), k = (int)(t & 15);
+    if (g >= num_points) return;
+    int stride;
+    float *const dst = grad_lane_dst(2 * k, v_rgb, v_conic, v_xy, v_xy_abs, v_pix_vel, v_opac, stride);
+    if (!dst) return;
+    const int2 r = seg[g];
+    float acc = 0.f;
+    for (int i = r.x; i < r.y; ++i) {
+        const float *s = slots + (size_t)__ldg(pos_sorted + i) * warps * RED_VALUES + k;
+        for (int w = 0; w < warps; ++w) acc += s[w * RED_VALUES];
+    }
+    dst[(size_t)g * stride] = acc;
+}
+
+struct DetBwdLayout {
+    size_t slots, slot_bytes, keys_a, keys_b, pos_a, pos_sorted, seg, cub, cub_bytes, total;
+};
+
+static DetBwdLayout det_bwd_layout(int n, int m, int warps) {
+    DetBwdLayout L;
+    WsCarver ws;
+    L.slot_bytes = (size_t)m * warps * RED_VALUES * sizeof(float);
+    L.slots = ws.take(L.slot_bytes);
+    L.keys_a = ws.take(4 * (size_t)m); L.keys_b = ws.take(4 * (size_t)m);
+    L.pos_a = ws.take(4 * (size_t)m); L.pos_sorted = ws.take(4 * (size_t)m);
+    L.seg = ws.take(8 * (size_t)n);
+    L.cub_bytes = cub_temp_bytes(SORT32, m > 0 ? m : 1) + 256;
+    L.cub = ws.take(L.cub_bytes);
+    L.total = ws.off;
+    return L;
 }
 
 }  // namespace b200
@@ -514,7 +585,7 @@ static int run_blend_backward(int num_points, unsigned img_height, unsigned img_
                               const float *background, const float *final_Ts, const int32_t *final_idx,
                               const float *v_output, const float *v_output_alpha, float *v_xy, float *v_xy_abs,
                               float *v_pix_vels, float *v_conic, float *v_colors, float *v_opacity, bool outputs_are_zero,
-                              cudaStream_t st, const int32_t *tile_order = nullptr) {
+                              cudaStream_t st, const int32_t *tile_order = nullptr, float *slots = nullptr) {
     B200_REQUIRE(n_blur_samples > 0 && n_blur_samples <= B200_MAX_BLUR_SAMPLES, "unsupported blur size");
     B200_REQUIRE(num_points >= 1, "num_points must be >= 1");
     B200_REQUIRE(block_width > 1 && block_width <= 16, "block_width must be between 2 and 16");
@@ -541,7 +612,10 @@ static int run_blend_backward(int num_points, unsigned img_height, unsigned img_
     p.final_Ts = final_Ts; p.final_idx = final_idx; p.v_out = v_output; p.v_out_alpha = v_output_alpha;
     p.v_xy = v_xy; p.v_xy_abs = v_xy_abs; p.v_pix_vel = v_pix_vels; p.v_conic = v_conic; p.v_rgb = v_colors;
     p.v_opac = v_opacity;
-    return with_blur_samples(n_blur_samples, [&](auto s) { return launch_bwd<decltype(s)::value>(p, st); });
+    p.slots = slots;
+    return with_blur_samples(n_blur_samples, [&](auto s) {
+        return slots ? launch_bwd<decltype(s)::value, true>(p, st) : launch_bwd<decltype(s)::value, false>(p, st);
+    });
 }
 
 extern "C" int b200_blend_backward_packed(int num_points, unsigned img_height, unsigned img_width, unsigned block_width,
@@ -573,6 +647,59 @@ extern "C" int b200_blend_backward_packed_ordered(int num_points, unsigned img_h
                               tile_bins, packed, rolling_shutter_time, exposure_time, background, final_Ts, final_idx,
                               v_output, v_output_alpha, v_xy, v_xy_abs, v_pix_vels, v_conic, v_colors, v_opacity,
                               outputs_are_zero != 0, as_stream(stream), tile_order);
+}
+
+extern "C" size_t b200_blend_backward_deterministic_ws_bytes(int num_points, int num_entries, unsigned block_width) {
+    if (num_points < 1 || num_entries < 0) return 0;
+    return det_bwd_layout(num_points, num_entries, bwd_warps(block_width)).total;
+}
+
+extern "C" int b200_blend_backward_packed_deterministic(int num_points, int num_entries, unsigned img_height,
+                                                        unsigned img_width, unsigned block_width, unsigned n_blur_samples,
+                                                        const int32_t *gaussian_ids_sorted, const int32_t *tile_bins,
+                                                        const void *packed, float rolling_shutter_time,
+                                                        float exposure_time, const float *background,
+                                                        const float *final_Ts, const int32_t *final_idx,
+                                                        const float *v_output, const float *v_output_alpha,
+                                                        const int32_t *status, const int32_t *tile_order, void *ws,
+                                                        size_t ws_bytes, float *v_xy, float *v_xy_abs, float *v_pix_vels,
+                                                        float *v_conic, float *v_colors, float *v_opacity, void *stream) {
+    B200_REQUIRE(num_points >= 1, "num_points must be >= 1");
+    B200_REQUIRE(num_entries >= 0, "num_entries must be >= 0");
+    B200_REQUIRE(num_entries == 0 || gaussian_ids_sorted, "null gaussian_ids_sorted");
+    B200_REQUIRE(ws && (reinterpret_cast<uintptr_t>(ws) & 255u) == 0, "ws must be a 256-byte aligned workspace");
+    const int warps = bwd_warps(block_width);
+    const DetBwdLayout L = det_bwd_layout(num_points, num_entries, warps);
+    B200_REQUIRE(ws_bytes >= L.total, "ws too small: %zu bytes, b200_blend_backward_deterministic_ws_bytes gives %zu",
+                 ws_bytes, L.total);
+    B200_REQUIRE(v_xy && v_xy_abs && v_pix_vels && v_conic && v_colors && v_opacity, "null output pointer");
+    cudaStream_t st = as_stream(stream);
+    char *base = static_cast<char *>(ws);
+    float *slots = reinterpret_cast<float *>(base + L.slots);
+    const int32_t *pos_sorted = reinterpret_cast<const int32_t *>(base + L.pos_sorted);
+    int2 *seg = reinterpret_cast<int2 *>(base + L.seg);
+    B200_CUDA(cudaMemsetAsync(seg, 0, 8 * (size_t)num_points, st));
+    if (num_entries > 0) {
+        B200_CUDA(cudaMemsetAsync(slots, 0, L.slot_bytes, st));  // slots no warp visits read as zero
+        int rc = run_blend_backward(num_points, img_height, img_width, block_width, n_blur_samples, gaussian_ids_sorted,
+                                    tile_bins, packed, rolling_shutter_time, exposure_time, background, final_Ts,
+                                    final_idx, v_output, v_output_alpha, v_xy, v_xy_abs, v_pix_vels, v_conic, v_colors,
+                                    v_opacity, true, st, tile_order, slots);
+        if (rc) return rc;
+        uint32_t *keys_a = reinterpret_cast<uint32_t *>(base + L.keys_a);
+        int32_t *pos_a = reinterpret_cast<int32_t *>(base + L.pos_a);
+        det_keys_kernel<<<ceil_div(num_entries, 256), 256, 0, st>>>(num_entries, num_points, gaussian_ids_sorted, status,
+                                                                    keys_a, pos_a);
+        B200_LAUNCH_CHECK();
+        rc = sort_to_bins(num_entries, std::max(1, key_end_bit(num_points + 1) - 32), num_points, keys_a,
+                          reinterpret_cast<uint32_t *>(base + L.keys_b), pos_a, const_cast<int32_t *>(pos_sorted),
+                          reinterpret_cast<int32_t *>(seg), base + L.cub, L.cub_bytes, st);
+        if (rc) return rc;
+    }
+    det_reduce_kernel<<<(unsigned)(((long long)num_points * 16 + 255) / 256), 256, 0, st>>>(
+        num_points, warps, slots, pos_sorted, seg, v_colors, v_conic, v_xy, v_xy_abs, v_pix_vels, v_opacity);
+    B200_LAUNCH_CHECK();
+    return B200_OK;
 }
 
 extern "C" int b200_rasterize_backward(int num_points, unsigned img_height, unsigned img_width, unsigned block_width,

@@ -39,6 +39,25 @@ static inline cudaStream_t as_stream(void *s) { return reinterpret_cast<cudaStre
 static inline bool aligned16(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 static inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 
+// Carves a workspace into consecutive buffers, each starting on a 256-byte boundary; `off` ends as the total size.
+struct WsCarver {
+    size_t off = 0;
+    size_t take(size_t bytes) {
+        const size_t o = off;
+        off += (bytes + 255) & ~(size_t)255;
+        return o;
+    }
+};
+
+// binning.cu: memoised cub temp sizes, the bit count of tile keys (32 depth bits + ceil(log2(num_tiles))), and the
+// stable (u32 key, i32 value) radix sort + [start, end) range per key that ends every binning (keys >= num_keys are
+// padding: they sort last and open no range).
+enum CubQuery { SORT32, SCAN32 };
+size_t cub_temp_bytes(CubQuery q, int n);
+int key_end_bit(int num_tiles);
+int sort_to_bins(int m, int bits, int num_tiles, uint32_t *tkeys_a, uint32_t *tkeys_b, int32_t *ids_a,
+                 int32_t *gaussian_ids_sorted, int32_t *tile_bins, void *cub_ws, size_t cub_bytes, cudaStream_t st);
+
 // ---------------------------------------------------------------- packed blend record
 // One 64-byte record per Gaussian, built by pack_records_kernel (blend_common.cuh) and gathered
 // into shared memory by cp.async.bulk.  Field order is what the blend loops read.

@@ -99,6 +99,7 @@ struct FusedBwdIO {
     float *g_means, *g_log_scales, *g_quats, *g_opacity, *g_sh_dc, *g_sh_rest;
     float *g_lin, *g_ang, *g_viewmat;  // optional, pre-zeroed accumulators
     bool gq_al;                        // g_quats is 16-byte aligned
+    float *cam_partials;               // DET only: 18 floats per block (cam_partials_sum_kernel)
 };
 
 // Coalesced store of a block's contiguous chunk of `row`-float rows staged in shared memory with pitch `pitch`.
@@ -110,7 +111,8 @@ __device__ __forceinline__ void store_rows(float *dst, const float *s, int row, 
     }
 }
 
-template <int DEG_USE>
+// DET: the camera partials of the block are stored to io.cam_partials instead of added to the outputs (deterministic mode)
+template <int DEG_USE, bool DET>
 __global__ void __launch_bounds__(FUSED_THREADS) fused_backward_kernel(FusedParams f, FusedBwdIO io) {
     constexpr int KU = (DEG_USE + 1) * (DEG_USE + 1);
     extern __shared__ __align__(16) float s_rows[];  // [FUSED_THREADS][pitch] gradient rows of sh_rest
@@ -207,10 +209,14 @@ __global__ void __launch_bounds__(FUSED_THREADS) fused_backward_kernel(FusedPara
             float s = 0.f;
 #pragma unroll
             for (int w = 0; w < FUSED_THREADS / 32; ++w) s += s_red[w][t];
-            float *dst = t < 3 ? (io.g_lin ? io.g_lin + t : nullptr)
-                       : t < 6 ? (io.g_ang ? io.g_ang + (t - 3) : nullptr)
-                               : (io.g_viewmat ? io.g_viewmat + (t - 6) : nullptr);
-            if (dst && s != 0.f) atomicAdd(dst, s);
+            if constexpr (DET) {
+                io.cam_partials[18 * (size_t)blockIdx.x + t] = s;
+            } else {
+                float *dst = t < 3 ? (io.g_lin ? io.g_lin + t : nullptr)
+                           : t < 6 ? (io.g_ang ? io.g_ang + (t - 3) : nullptr)
+                                   : (io.g_viewmat ? io.g_viewmat + (t - 6) : nullptr);
+                if (dst && s != 0.f) atomicAdd(dst, s);
+            }
         }
     }
 }
@@ -311,6 +317,62 @@ extern "C" int b200_fused_colors_forward(int num_points, const float *means, con
     return B200_OK;
 }
 
+// cam_ws != null: deterministic camera sums (b200_fused_preprocess_backward_deterministic)
+static int run_fused_backward(int num_points, const float *means, const float *log_scales, const float *quats,
+                              const float *opacity_logit, const float *sh_dc, const float *sh_rest, int sh_bases,
+                              int degrees_to_use, const float *viewmat, const float *cam_pos, const float *lin_vel,
+                              const float *ang_vel, float rolling_shutter_time, float exposure_time, float fx, float fy,
+                              float cx, float cy, unsigned img_height, unsigned img_width, unsigned block_width,
+                              float clip_thresh, const void *packed, const int32_t *radii, const float *v_xy,
+                              const float *v_pix_vel, const float *v_conic, const float *v_colors,
+                              const float *v_opacity, float *g_means, float *g_log_scales, float *g_quats,
+                              float *g_opacity_logit, float *g_sh_dc, float *g_sh_rest, float *g_lin_vel,
+                              float *g_ang_vel, float *g_viewmat, float *cam_ws, cudaStream_t st) {
+    FusedParams f;
+    int rc = fill_fused(f, num_points, means, log_scales, quats, opacity_logit, sh_dc, sh_rest, sh_bases, degrees_to_use,
+                        viewmat, cam_pos, lin_vel, ang_vel, rolling_shutter_time, exposure_time, fx, fy, cx, cy, img_height,
+                        img_width, block_width, clip_thresh);
+    if (rc) return rc;
+    B200_REQUIRE(packed && radii && v_xy && v_pix_vel && v_conic && v_colors && v_opacity, "null input pointer");
+    B200_REQUIRE(g_means && g_log_scales && g_quats && g_opacity_logit && g_sh_dc && (sh_bases == 1 || g_sh_rest),
+                 "null gradient pointer");
+    // deterministic camera sums: the blocks store partials and cam_partials_sum_kernel overwrites the outputs
+    const bool det = cam_ws && (g_lin_vel || g_ang_vel || g_viewmat);
+    if (!det) {
+        if (g_lin_vel) B200_CUDA(cudaMemsetAsync(g_lin_vel, 0, 3 * sizeof(float), st));
+        if (g_ang_vel) B200_CUDA(cudaMemsetAsync(g_ang_vel, 0, 3 * sizeof(float), st));
+        if (g_viewmat) B200_CUDA(cudaMemsetAsync(g_viewmat, 0, 12 * sizeof(float), st));
+    }
+    FusedBwdIO io{reinterpret_cast<const PackedGaussian *>(packed), radii, v_xy, v_pix_vel, v_conic, v_colors, v_opacity,
+                  g_means, g_log_scales, g_quats, g_opacity_logit, g_sh_dc, g_sh_rest, g_lin_vel, g_ang_vel, g_viewmat,
+                  aligned16(g_quats), cam_ws};
+    const int rest_row = 3 * (sh_bases - 1);
+    const int pitch = (rest_row & 1) ? rest_row : rest_row + 1;
+    const size_t smem = sizeof(float) * FUSED_THREADS * (size_t)(pitch > 0 ? pitch : 1);
+    const int blocks = ceil_div(num_points, FUSED_THREADS);
+    if (det) {
+        switch (degrees_to_use) {
+            case 0: fused_backward_kernel<0, true><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
+            case 1: fused_backward_kernel<1, true><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
+            case 2: fused_backward_kernel<2, true><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
+            case 3: fused_backward_kernel<3, true><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
+            default: fused_backward_kernel<4, true><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
+        }
+        B200_LAUNCH_CHECK();
+        cam_partials_sum_kernel<<<1, 32, 0, st>>>(blocks, cam_ws, g_lin_vel, g_ang_vel, g_viewmat);
+    } else {
+        switch (degrees_to_use) {
+            case 0: fused_backward_kernel<0, false><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
+            case 1: fused_backward_kernel<1, false><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
+            case 2: fused_backward_kernel<2, false><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
+            case 3: fused_backward_kernel<3, false><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
+            default: fused_backward_kernel<4, false><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
+        }
+    }
+    B200_LAUNCH_CHECK();
+    return B200_OK;
+}
+
 extern "C" int b200_fused_preprocess_backward(int num_points, const float *means, const float *log_scales,
                                               const float *quats, const float *opacity_logit, const float *sh_dc,
                                               const float *sh_rest, int sh_bases, int degrees_to_use,
@@ -323,32 +385,34 @@ extern "C" int b200_fused_preprocess_backward(int num_points, const float *means
                                               const float *v_opacity, float *g_means, float *g_log_scales,
                                               float *g_quats, float *g_opacity_logit, float *g_sh_dc, float *g_sh_rest,
                                               float *g_lin_vel, float *g_ang_vel, float *g_viewmat, void *stream) {
-    FusedParams f;
-    int rc = fill_fused(f, num_points, means, log_scales, quats, opacity_logit, sh_dc, sh_rest, sh_bases, degrees_to_use,
-                        viewmat, cam_pos, lin_vel, ang_vel, rolling_shutter_time, exposure_time, fx, fy, cx, cy, img_height,
-                        img_width, block_width, clip_thresh);
-    if (rc) return rc;
-    B200_REQUIRE(packed && radii && v_xy && v_pix_vel && v_conic && v_colors && v_opacity, "null input pointer");
-    B200_REQUIRE(g_means && g_log_scales && g_quats && g_opacity_logit && g_sh_dc && (sh_bases == 1 || g_sh_rest),
-                 "null gradient pointer");
-    cudaStream_t st = as_stream(stream);
-    if (g_lin_vel) B200_CUDA(cudaMemsetAsync(g_lin_vel, 0, 3 * sizeof(float), st));
-    if (g_ang_vel) B200_CUDA(cudaMemsetAsync(g_ang_vel, 0, 3 * sizeof(float), st));
-    if (g_viewmat) B200_CUDA(cudaMemsetAsync(g_viewmat, 0, 12 * sizeof(float), st));
-    FusedBwdIO io{reinterpret_cast<const PackedGaussian *>(packed), radii, v_xy, v_pix_vel, v_conic, v_colors, v_opacity,
-                  g_means, g_log_scales, g_quats, g_opacity_logit, g_sh_dc, g_sh_rest, g_lin_vel, g_ang_vel, g_viewmat,
-                  aligned16(g_quats)};
-    const int rest_row = 3 * (sh_bases - 1);
-    const int pitch = (rest_row & 1) ? rest_row : rest_row + 1;
-    const size_t smem = sizeof(float) * FUSED_THREADS * (size_t)(pitch > 0 ? pitch : 1);
-    const int blocks = ceil_div(num_points, FUSED_THREADS);
-    switch (degrees_to_use) {
-        case 0: fused_backward_kernel<0><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
-        case 1: fused_backward_kernel<1><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
-        case 2: fused_backward_kernel<2><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
-        case 3: fused_backward_kernel<3><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
-        default: fused_backward_kernel<4><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
-    }
-    B200_LAUNCH_CHECK();
-    return B200_OK;
+    return run_fused_backward(num_points, means, log_scales, quats, opacity_logit, sh_dc, sh_rest, sh_bases,
+                              degrees_to_use, viewmat, cam_pos, lin_vel, ang_vel, rolling_shutter_time, exposure_time, fx,
+                              fy, cx, cy, img_height, img_width, block_width, clip_thresh, packed, radii, v_xy, v_pix_vel,
+                              v_conic, v_colors, v_opacity, g_means, g_log_scales, g_quats, g_opacity_logit, g_sh_dc,
+                              g_sh_rest, g_lin_vel, g_ang_vel, g_viewmat, nullptr, as_stream(stream));
+}
+
+extern "C" size_t b200_fused_preprocess_backward_ws_bytes(int num_points) {
+    return num_points < 1 ? 0 : 18 * sizeof(float) * (size_t)ceil_div(num_points, FUSED_THREADS);
+}
+
+extern "C" int b200_fused_preprocess_backward_deterministic(
+    int num_points, const float *means, const float *log_scales, const float *quats, const float *opacity_logit,
+    const float *sh_dc, const float *sh_rest, int sh_bases, int degrees_to_use, const float *viewmat,
+    const float *cam_pos, const float *lin_vel, const float *ang_vel, float rolling_shutter_time, float exposure_time,
+    float fx, float fy, float cx, float cy, unsigned img_height, unsigned img_width, unsigned block_width,
+    float clip_thresh, const void *packed, const int32_t *radii, const float *v_xy, const float *v_pix_vel,
+    const float *v_conic, const float *v_colors, const float *v_opacity, float *g_means, float *g_log_scales,
+    float *g_quats, float *g_opacity_logit, float *g_sh_dc, float *g_sh_rest, float *g_lin_vel, float *g_ang_vel,
+    float *g_viewmat, void *ws, size_t ws_bytes, void *stream) {
+    B200_REQUIRE(num_points >= 1, "num_points must be >= 1");
+    B200_REQUIRE(ws && aligned16(ws), "ws must be a 16-byte aligned workspace");
+    const size_t need = b200_fused_preprocess_backward_ws_bytes(num_points);
+    B200_REQUIRE(ws_bytes >= need, "ws too small: %zu bytes, b200_fused_preprocess_backward_ws_bytes gives %zu",
+                 ws_bytes, need);
+    return run_fused_backward(num_points, means, log_scales, quats, opacity_logit, sh_dc, sh_rest, sh_bases,
+                              degrees_to_use, viewmat, cam_pos, lin_vel, ang_vel, rolling_shutter_time, exposure_time, fx,
+                              fy, cx, cy, img_height, img_width, block_width, clip_thresh, packed, radii, v_xy, v_pix_vel,
+                              v_conic, v_colors, v_opacity, g_means, g_log_scales, g_quats, g_opacity_logit, g_sh_dc,
+                              g_sh_rest, g_lin_vel, g_ang_vel, g_viewmat, static_cast<float *>(ws), as_stream(stream));
 }

@@ -84,9 +84,11 @@ struct ProjBwdIO {
     float *v_cov2d, *v_cov3d;  // optional
     float *v_mean, *v_scale, *v_quat;
     float *v_lin, *v_ang, *v_viewmat;  // optional accumulators (pre-zeroed)
+    float *cam_partials;               // DET only: 18 floats per block (cam_partials_sum_kernel)
 };
 
-template <bool VEC, bool EXACT>
+// DET: the camera partials of the block are stored to io.cam_partials instead of added to the outputs (deterministic mode)
+template <bool VEC, bool EXACT, bool DET>
 __global__ void __launch_bounds__(PROJ_THREADS) project_backward_kernel(ProjCommon p, ProjBwdIO io) {
     __shared__ __align__(16) float s_means[3 * PROJ_THREADS];
     __shared__ __align__(16) float s_scales[3 * PROJ_THREADS];
@@ -152,10 +154,14 @@ __global__ void __launch_bounds__(PROJ_THREADS) project_backward_kernel(ProjComm
             float s = 0.f;
 #pragma unroll
             for (int w = 0; w < PROJ_THREADS / 32; ++w) s += s_red[w][t];
-            float *dst = t < 3 ? (io.v_lin ? io.v_lin + t : nullptr)
-                       : t < 6 ? (io.v_ang ? io.v_ang + (t - 3) : nullptr)
-                               : (io.v_viewmat ? io.v_viewmat + (t - 6) : nullptr);
-            if (dst && s != 0.f) atomicAdd(dst, s);
+            if constexpr (DET) {
+                io.cam_partials[18 * (size_t)blockIdx.x + t] = s;
+            } else {
+                float *dst = t < 3 ? (io.v_lin ? io.v_lin + t : nullptr)
+                           : t < 6 ? (io.v_ang ? io.v_ang + (t - 3) : nullptr)
+                                   : (io.v_viewmat ? io.v_viewmat + (t - 6) : nullptr);
+                if (dst && s != 0.f) atomicAdd(dst, s);
+            }
         }
     }
 }
@@ -208,6 +214,58 @@ extern "C" int b200_project_gaussians_forward(int num_points, const float *means
     return B200_OK;
 }
 
+// cam_ws != null: deterministic camera sums (b200_project_gaussians_backward_deterministic)
+static int run_project_backward(int num_points, const float *means3d, const float *scales, float glob_scale,
+                                const float *quats, const float *lin_vel, const float *ang_vel,
+                                float rolling_shutter_time, float exposure_time, const float *viewmat, float fx, float fy,
+                                float cx, float cy, unsigned img_height, unsigned img_width, const float *cov3d,
+                                const int32_t *radii, const float *conics, const float *compensation, const float *v_xy,
+                                const float *v_depth, const float *v_pix_vel, const float *v_conic,
+                                const float *v_compensation, unsigned flags, float *v_cov2d, float *v_cov3d,
+                                float *v_mean3d, float *v_scale, float *v_quat, float *v_lin_vel, float *v_ang_vel,
+                                float *v_viewmat, float *cam_ws, cudaStream_t st) {
+    ProjCommon p;
+    int rc = fill_common(p, num_points, means3d, scales, glob_scale, quats, lin_vel, ang_vel, rolling_shutter_time,
+                         exposure_time, viewmat, fx, fy, cx, cy, img_height, img_width, 16, 0.f);
+    if (rc) return rc;
+    B200_REQUIRE(cov3d && radii && conics && compensation, "null saved-forward pointer");
+    B200_REQUIRE(v_xy && v_depth && v_pix_vel && v_conic && v_compensation, "null cotangent pointer");
+    B200_REQUIRE(v_mean3d && v_scale && v_quat, "null gradient output pointer");
+    B200_REQUIRE(aligned16(v_quat), "v_quat must be 16-byte aligned");
+    // deterministic camera sums: the blocks store partials and cam_partials_sum_kernel overwrites the outputs
+    const bool det = cam_ws && (v_lin_vel || v_ang_vel || v_viewmat);
+    if (!det) {
+        if (v_lin_vel && v_ang_vel == v_lin_vel + 3 && (!v_viewmat || v_viewmat == v_lin_vel + 6)) {
+            // the three accumulators are one 6- or 18-float block (what gsplat/cuda allocates): one memset
+            B200_CUDA(cudaMemsetAsync(v_lin_vel, 0, (v_viewmat ? 18 : 6) * sizeof(float), st));
+        } else {
+            if (v_lin_vel) B200_CUDA(cudaMemsetAsync(v_lin_vel, 0, 3 * sizeof(float), st));
+            if (v_ang_vel) B200_CUDA(cudaMemsetAsync(v_ang_vel, 0, 3 * sizeof(float), st));
+            if (v_viewmat) B200_CUDA(cudaMemsetAsync(v_viewmat, 0, 12 * sizeof(float), st));
+        }
+    }
+    ProjBwdIO io{cov3d, conics, compensation, radii, v_xy, v_depth, v_pix_vel, v_conic, v_compensation,
+                 v_cov2d, v_cov3d, v_mean3d, v_scale, v_quat, v_lin_vel, v_ang_vel, v_viewmat, cam_ws};
+    const int blocks = ceil_div(num_points, PROJ_THREADS);
+    const bool vec = aligned16(means3d) && aligned16(scales) && aligned16(quats);
+    const bool exact = (flags & B200_PROJ_EXACT) != 0;
+    if (det) {
+        if (vec && exact) project_backward_kernel<true, true, true><<<blocks, PROJ_THREADS, 0, st>>>(p, io);
+        else if (vec) project_backward_kernel<true, false, true><<<blocks, PROJ_THREADS, 0, st>>>(p, io);
+        else if (exact) project_backward_kernel<false, true, true><<<blocks, PROJ_THREADS, 0, st>>>(p, io);
+        else project_backward_kernel<false, false, true><<<blocks, PROJ_THREADS, 0, st>>>(p, io);
+        B200_LAUNCH_CHECK();
+        cam_partials_sum_kernel<<<1, 32, 0, st>>>(blocks, cam_ws, v_lin_vel, v_ang_vel, v_viewmat);
+    } else {
+        if (vec && exact) project_backward_kernel<true, true, false><<<blocks, PROJ_THREADS, 0, st>>>(p, io);
+        else if (vec) project_backward_kernel<true, false, false><<<blocks, PROJ_THREADS, 0, st>>>(p, io);
+        else if (exact) project_backward_kernel<false, true, false><<<blocks, PROJ_THREADS, 0, st>>>(p, io);
+        else project_backward_kernel<false, false, false><<<blocks, PROJ_THREADS, 0, st>>>(p, io);
+    }
+    B200_LAUNCH_CHECK();
+    return B200_OK;
+}
+
 extern "C" int b200_project_gaussians_backward(int num_points, const float *means3d, const float *scales,
                                                float glob_scale, const float *quats, const float *lin_vel,
                                                const float *ang_vel, float rolling_shutter_time, float exposure_time,
@@ -219,34 +277,34 @@ extern "C" int b200_project_gaussians_backward(int num_points, const float *mean
                                                float *v_cov2d, float *v_cov3d, float *v_mean3d, float *v_scale,
                                                float *v_quat, float *v_lin_vel, float *v_ang_vel, float *v_viewmat,
                                                void *stream) {
-    ProjCommon p;
-    int rc = fill_common(p, num_points, means3d, scales, glob_scale, quats, lin_vel, ang_vel, rolling_shutter_time,
-                         exposure_time, viewmat, fx, fy, cx, cy, img_height, img_width, 16, 0.f);
-    if (rc) return rc;
-    B200_REQUIRE(cov3d && radii && conics && compensation, "null saved-forward pointer");
-    B200_REQUIRE(v_xy && v_depth && v_pix_vel && v_conic && v_compensation, "null cotangent pointer");
-    B200_REQUIRE(v_mean3d && v_scale && v_quat, "null gradient output pointer");
-    B200_REQUIRE(aligned16(v_quat), "v_quat must be 16-byte aligned");
-    cudaStream_t st = as_stream(stream);
-    if (v_lin_vel && v_ang_vel == v_lin_vel + 3 && (!v_viewmat || v_viewmat == v_lin_vel + 6)) {
-        // the three accumulators are one 6- or 18-float block (what gsplat/cuda allocates): one memset
-        B200_CUDA(cudaMemsetAsync(v_lin_vel, 0, (v_viewmat ? 18 : 6) * sizeof(float), st));
-    } else {
-        if (v_lin_vel) B200_CUDA(cudaMemsetAsync(v_lin_vel, 0, 3 * sizeof(float), st));
-        if (v_ang_vel) B200_CUDA(cudaMemsetAsync(v_ang_vel, 0, 3 * sizeof(float), st));
-        if (v_viewmat) B200_CUDA(cudaMemsetAsync(v_viewmat, 0, 12 * sizeof(float), st));
-    }
-    ProjBwdIO io{cov3d, conics, compensation, radii, v_xy, v_depth, v_pix_vel, v_conic, v_compensation,
-                 v_cov2d, v_cov3d, v_mean3d, v_scale, v_quat, v_lin_vel, v_ang_vel, v_viewmat};
-    const int blocks = ceil_div(num_points, PROJ_THREADS);
-    const bool vec = aligned16(means3d) && aligned16(scales) && aligned16(quats);
-    const bool exact = (flags & B200_PROJ_EXACT) != 0;
-    if (vec && exact) project_backward_kernel<true, true><<<blocks, PROJ_THREADS, 0, st>>>(p, io);
-    else if (vec) project_backward_kernel<true, false><<<blocks, PROJ_THREADS, 0, st>>>(p, io);
-    else if (exact) project_backward_kernel<false, true><<<blocks, PROJ_THREADS, 0, st>>>(p, io);
-    else project_backward_kernel<false, false><<<blocks, PROJ_THREADS, 0, st>>>(p, io);
-    B200_LAUNCH_CHECK();
-    return B200_OK;
+    return run_project_backward(num_points, means3d, scales, glob_scale, quats, lin_vel, ang_vel, rolling_shutter_time,
+                                exposure_time, viewmat, fx, fy, cx, cy, img_height, img_width, cov3d, radii, conics,
+                                compensation, v_xy, v_depth, v_pix_vel, v_conic, v_compensation, flags, v_cov2d, v_cov3d,
+                                v_mean3d, v_scale, v_quat, v_lin_vel, v_ang_vel, v_viewmat, nullptr, as_stream(stream));
+}
+
+extern "C" size_t b200_project_gaussians_backward_ws_bytes(int num_points) {
+    return num_points < 1 ? 0 : 18 * sizeof(float) * (size_t)ceil_div(num_points, PROJ_THREADS);
+}
+
+extern "C" int b200_project_gaussians_backward_deterministic(
+    int num_points, const float *means3d, const float *scales, float glob_scale, const float *quats,
+    const float *lin_vel, const float *ang_vel, float rolling_shutter_time, float exposure_time, const float *viewmat,
+    float fx, float fy, float cx, float cy, unsigned img_height, unsigned img_width, const float *cov3d,
+    const int32_t *radii, const float *conics, const float *compensation, const float *v_xy, const float *v_depth,
+    const float *v_pix_vel, const float *v_conic, const float *v_compensation, unsigned flags, float *v_cov2d,
+    float *v_cov3d, float *v_mean3d, float *v_scale, float *v_quat, float *v_lin_vel, float *v_ang_vel, float *v_viewmat,
+    void *ws, size_t ws_bytes, void *stream) {
+    B200_REQUIRE(num_points >= 1, "num_points must be >= 1 (got %d)", num_points);
+    B200_REQUIRE(ws && aligned16(ws), "ws must be a 16-byte aligned workspace");
+    const size_t need = b200_project_gaussians_backward_ws_bytes(num_points);
+    B200_REQUIRE(ws_bytes >= need, "ws too small: %zu bytes, b200_project_gaussians_backward_ws_bytes gives %zu",
+                 ws_bytes, need);
+    return run_project_backward(num_points, means3d, scales, glob_scale, quats, lin_vel, ang_vel, rolling_shutter_time,
+                                exposure_time, viewmat, fx, fy, cx, cy, img_height, img_width, cov3d, radii, conics,
+                                compensation, v_xy, v_depth, v_pix_vel, v_conic, v_compensation, flags, v_cov2d, v_cov3d,
+                                v_mean3d, v_scale, v_quat, v_lin_vel, v_ang_vel, v_viewmat, static_cast<float *>(ws),
+                                as_stream(stream));
 }
 
 extern "C" int b200_compute_cov2d_bounds(int num_pts, const float *cov2d, float *conics, float *radii, void *stream) {

@@ -314,4 +314,19 @@ __device__ __forceinline__ void project_backward_one(const ProjCommon &p, bool w
 
 }
 
+// Deterministic mode of the camera gradients: block b of a projection / fused backward stores its 18 partial sums
+// (lin_vel 3, ang_vel 3, viewmat 12) at partials[18 b + c] instead of adding them to the outputs; this kernel (one warp)
+// sums each component in block order and OVERWRITES the non-null outputs.
+static __global__ void __launch_bounds__(32) cam_partials_sum_kernel(int blocks, const float *__restrict__ partials,
+                                                                     float *v_lin, float *v_ang, float *v_viewmat) {
+    const int c = threadIdx.x;
+    if (c >= 18) return;
+    float s = 0.f;
+    for (int b = 0; b < blocks; ++b) s += partials[18 * (size_t)b + c];
+    float *dst = c < 3 ? (v_lin ? v_lin + c : nullptr)
+               : c < 6 ? (v_ang ? v_ang + (c - 3) : nullptr)
+                       : (v_viewmat ? v_viewmat + (c - 6) : nullptr);
+    if (dst) *dst = s;
+}
+
 }  // namespace b200

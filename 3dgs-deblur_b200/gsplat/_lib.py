@@ -76,6 +76,17 @@ SIGNATURES = {
     "b200_l1_loss": (_i, [C.c_longlong, _p, _p, _p, _p, _p, _i, _p]),
     "b200_l1_loss_gamma": (_i, [C.c_longlong, _p, _p, _f, _p, _p, _p, _i, _p]),
     "b200_l1_loss_u8": (_i, [C.c_longlong, _i, _p, _p, _p, _f, _f, _p, _p, _p, _p, _p, _i, _p]),
+    "b200_blend_backward_deterministic_ws_bytes": (_sz, [_i, _i, _u]),
+    "b200_blend_backward_packed_deterministic": (_i, [_i, _i, _u, _u, _u, _u, _p, _p, _p, _f, _f, _p, _p, _p, _p, _p, _p,
+                                                      _p, _p, _sz, _p, _p, _p, _p, _p, _p, _p]),
+    "b200_project_gaussians_backward_ws_bytes": (_sz, [_i]),
+    "b200_project_gaussians_backward_deterministic": (_i, [_i, _p, _p, _f, _p, _p, _p, _f, _f, _p, _f, _f, _f, _f, _u, _u,
+                                                           _p, _p, _p, _p, _p, _p, _p, _p, _p, _u,
+                                                           _p, _p, _p, _p, _p, _p, _p, _p, _p, _sz, _p]),
+    "b200_fused_preprocess_backward_ws_bytes": (_sz, [_i]),
+    "b200_fused_preprocess_backward_deterministic": (_i, [_i, _p, _p, _p, _p, _p, _p, _i, _i, _p, _p, _p, _p, _f, _f, _f, _f,
+                                                          _f, _f, _u, _u, _u, _f, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p,
+                                                          _p, _p, _p, _p, _p, _p, _p, _sz, _p]),
     "b200_nd_rasterize_forward": (_i, [_i, _u, _u, _u, _u, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
     "b200_nd_rasterize_backward": (_i, [_i, _u, _u, _u, _u, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p,
                                         _p, _p, _p, _p, _p, _p]),
@@ -109,6 +120,41 @@ def check(rc):
     """0 -> ok; otherwise raise like the reference's TORCH_CHECK / AT_ERROR (RuntimeError)."""
     if rc != 0:
         raise RuntimeError(load().b200_last_error().decode("utf-8", "replace"))
+
+
+def deterministic():
+    """True under torch.use_deterministic_algorithms(True): the operators then take the entry points whose sums run in a
+    fixed order (include/b200splat.h, deterministic mode) and give bit-identical gradients from call to call."""
+    return torch.are_deterministic_algorithms_enabled()
+
+
+def alert_not_deterministic(caller):
+    """What torch's own CUDA ops without a deterministic implementation do under the flag: raise, or warn when the
+    flag was set with warn_only=True."""
+    if not torch.are_deterministic_algorithms_enabled():
+        return
+    msg = (f"{caller} does not have a deterministic implementation, but you set "
+           "'torch.use_deterministic_algorithms(True)'. You can turn off determinism just for this operation, or you "
+           "can use the 'warn_only=True' option, if that's acceptable for your application.")
+    if torch.is_deterministic_algorithms_warn_only_enabled():
+        import warnings
+
+        warnings.warn(msg)
+    else:
+        raise RuntimeError(msg)
+
+
+def workspace(nbytes, device):
+    """Uninitialised uint8 scratch: the library writes or clears what it reads, so torch's NaN fill of new tensors
+    under the deterministic flag would only cost a pass over it."""
+    from torch.utils import deterministic as _det
+
+    fill = _det.fill_uninitialized_memory
+    _det.fill_uninitialized_memory = False
+    try:
+        return torch.empty((max(int(nbytes), 16),), dtype=torch.uint8, device=device)
+    finally:
+        _det.fill_uninitialized_memory = fill
 
 
 def ptr(t):

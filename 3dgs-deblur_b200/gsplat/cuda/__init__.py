@@ -8,7 +8,7 @@ PyTorch and handed to the C ABI (include/b200splat.h) as raw device pointers on 
 import torch
 
 from .. import _lib
-from .._lib import check, on_device, ptr, require_cuda, stream
+from .._lib import check, deterministic, on_device, ptr, require_cuda, stream
 
 __all__ = [
     "nd_rasterize_forward", "nd_rasterize_backward", "rasterize_forward", "rasterize_backward",
@@ -94,13 +94,18 @@ def project_gaussians_backward(num_points, means3d, scales, glob_scale, quats, l
                 v_vm = acc[6:18].view(3, 4)
         elif _want_viewmat:
             v_vm = torch.empty((3, 4), **f32)
-        check(_lib.load().b200_project_gaussians_backward(
-            n, ptr(_f32(means3d)), ptr(_f32(scales)), float(glob_scale), ptr(_f32(quats)), ptr(lin), ptr(ang),
-            float(rolling_shutter_time), float(exposure_time), ptr(_f32(viewmat)), float(fx), float(fy), float(cx),
-            float(cy), int(img_height), int(img_width), ptr(cov3d), ptr(radii), ptr(conics), ptr(compensation),
-            ptr(v_xy), ptr(v_depth), ptr(v_pix_vel), ptr(v_conic), ptr(v_compensation), 1 if _exact else 0,
-            ptr(v_cov2d), ptr(v_cov3d), ptr(v_mean3d), ptr(v_scale), ptr(v_quat), ptr(v_lin), ptr(v_ang), ptr(v_vm),
-            stream()))
+        lib = _lib.load()
+        args = (n, ptr(_f32(means3d)), ptr(_f32(scales)), float(glob_scale), ptr(_f32(quats)), ptr(lin), ptr(ang),
+                float(rolling_shutter_time), float(exposure_time), ptr(_f32(viewmat)), float(fx), float(fy), float(cx),
+                float(cy), int(img_height), int(img_width), ptr(cov3d), ptr(radii), ptr(conics), ptr(compensation),
+                ptr(v_xy), ptr(v_depth), ptr(v_pix_vel), ptr(v_conic), ptr(v_compensation), 1 if _exact else 0,
+                ptr(v_cov2d), ptr(v_cov3d), ptr(v_mean3d), ptr(v_scale), ptr(v_quat), ptr(v_lin), ptr(v_ang), ptr(v_vm))
+        if deterministic() and (_want_vel or _want_viewmat):  # camera sums in block order
+            nbytes = lib.b200_project_gaussians_backward_ws_bytes(n)
+            ws = _lib.workspace(nbytes, dev)
+            check(lib.b200_project_gaussians_backward_deterministic(*args, ptr(ws), nbytes, stream()))
+        else:
+            check(lib.b200_project_gaussians_backward(*args, stream()))
     out = (v_cov2d, v_cov3d, v_mean3d, v_scale, v_quat)
     if _want_vel:
         out = out + (v_lin, v_ang)
@@ -346,8 +351,11 @@ def blend_forward_packed(img_height, img_width, block_width, n_blur_samples, gau
 
 def blend_backward_packed(num_points, img_height, img_width, block_width, n_blur_samples, gaussian_ids_sorted, tile_bins,
                           packed, rolling_shutter_time, exposure_time, background, final_Ts, final_idx, v_output,
-                          v_output_alpha):
-    """Extension: blend backward on prepacked records -> (v_xy, v_xy_abs, v_pix_vels, v_conic, v_colors, v_opacity)."""
+                          v_output_alpha, *, status=None):
+    """Extension: blend backward on prepacked records -> (v_xy, v_xy_abs, v_pix_vels, v_conic, v_colors, v_opacity).
+    Under torch.use_deterministic_algorithms(True) the per-Gaussian sums are added in a fixed order
+    (b200_blend_backward_packed_deterministic): bit-identical from call to call.  `status`: the capacity-mode status
+    block the lists were built with (its entry count marks where the padding starts); only read in that mode."""
     require_cuda(gaussian_ids_sorted, tile_bins, packed, background)
     dev = packed.device
     with on_device(dev):
@@ -355,6 +363,11 @@ def blend_backward_packed(num_points, img_height, img_width, block_width, n_blur
         f32 = dict(dtype=torch.float32, device=dev)
         v_output = _f32(v_output).contiguous()
         v_output_alpha = _f32(v_output_alpha).contiguous() if v_output_alpha is not None else None
+        if deterministic():
+            return _blend_backward_deterministic(n, int(img_height), int(img_width), int(block_width),
+                                                 int(n_blur_samples), gaussian_ids_sorted, tile_bins, packed,
+                                                 float(rolling_shutter_time), float(exposure_time), _f32(background),
+                                                 _f32(final_Ts), final_idx, v_output, v_output_alpha, status)
         # one zero-filled allocation for the 13 floats per Gaussian the kernel accumulates into (each array 64-byte
         # aligned inside it): one fill instead of six memsets
         pitch = (n + 15) & ~15
@@ -369,6 +382,36 @@ def blend_backward_packed(num_points, img_height, img_width, block_width, n_blur
             ptr(_f32(final_Ts)), ptr(final_idx), ptr(v_output), ptr(v_output_alpha), ptr(order), ptr(v_xy), ptr(v_xy_abs),
             ptr(v_pix), ptr(v_conic), ptr(v_colors), ptr(v_opacity), 1, stream()))
     return v_xy, v_xy_abs, v_pix, v_conic, v_colors, v_opacity
+
+
+def _blend_backward_deterministic(n, H, W, bw, S, ids, bins, packed, rs, ex, bg, final_Ts, final_idx, v_output,
+                                  v_output_alpha, status):
+    lib = _lib.load()
+    dev = packed.device
+    f32 = dict(dtype=torch.float32, device=dev)
+    m = ids.numel()
+    nbytes = lib.b200_blend_backward_deterministic_ws_bytes(n, m, bw)
+    ws = _lib.workspace(nbytes, dev)
+    outs = (torch.empty((n, 2), **f32), torch.empty((n, 2), **f32), torch.empty((n, 2), **f32),
+            torch.empty((n, 3), **f32), torch.empty((n, 3), **f32), torch.empty((n, 1), **f32))
+    order = _tile_order(bins, H, W, bw)
+    check(lib.b200_blend_backward_packed_deterministic(
+        n, m, H, W, bw, S, ptr(ids), ptr(bins), ptr(packed), rs, ex, ptr(bg), ptr(final_Ts), ptr(final_idx),
+        ptr(v_output), ptr(v_output_alpha), ptr(status), ptr(order), ptr(ws), nbytes, *[ptr(t) for t in outs], stream()))
+    return outs
+
+
+def fused_preprocess_backward(device, *args):
+    """b200_fused_preprocess_backward with `args` as in include/b200splat.h up to the stream; under
+    torch.use_deterministic_algorithms(True) the camera sums go through the _deterministic entry point."""
+    lib = _lib.load()
+    n, g_cam = int(args[0]), args[-3:]
+    if deterministic() and any(p is not None for p in g_cam):
+        nbytes = lib.b200_fused_preprocess_backward_ws_bytes(n)
+        ws = _lib.workspace(nbytes, device)
+        check(lib.b200_fused_preprocess_backward_deterministic(*args, ptr(ws), nbytes, stream()))
+    else:
+        check(lib.b200_fused_preprocess_backward(*args, stream()))
 
 
 def _tile_order(tile_bins, H, W, bw):
@@ -458,7 +501,11 @@ def nd_rasterize_forward(tile_bounds, block, img_size, n_blur_samples, gaussian_
 def nd_rasterize_backward(img_height, img_width, block_width, n_blur_samples, gaussian_ids_sorted, tile_bins, xys,
                           pix_vels, rolling_shutter_time, exposure_time, conics, colors, opacities, background,
                           final_Ts, final_idx, v_output, v_output_alpha):
-    """-> (v_xy, v_xy_abs, v_pix_vels (zeros), v_conic, v_colors, v_opacity)  [bindings.cu:596-682]"""
+    """-> (v_xy, v_xy_abs, v_pix_vels (zeros), v_conic, v_colors, v_opacity)  [bindings.cu:596-682]
+
+    Adds per-pixel contributions with float atomics: under torch.use_deterministic_algorithms(True) it raises (or warns
+    with warn_only=True) like torch's own nondeterministic CUDA ops."""
+    _lib.alert_not_deterministic("nd_rasterize_backward")
     require_cuda(xys, colors)
     if not (int(n_blur_samples) == 1 and exposure_time == 0):
         raise RuntimeError("blur not supported here")

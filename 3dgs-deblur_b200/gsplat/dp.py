@@ -17,6 +17,7 @@ The densification statistics (xys.absgrad norms, visibility counts, max 2D radiu
 splatfacto.py:417-434) are exposed by `reduce_densify_stats` with the matching sum / sum / max
 reductions so a caller can keep topology changes identical across ranks.
 """
+import gc
 import math
 import os
 from typing import Dict, List, Optional
@@ -464,15 +465,15 @@ def fused_shading_phase(model: FlatGaussians, geo: Dict, scene: Dict, target: to
         (v_rgb,) = torch.autograd.grad(loss, rgb)
     with torch.no_grad(), _lib.on_device(dev):
         v_xy, v_abs, v_pix, v_conic, v_col, v_op = _C.blend_backward_packed(
-            n, H, W, bw, S, geo["ids"], geo["bins"], packed, rs, ex, bg, Ts, fi, v_rgb, None)
+            n, H, W, bw, S, geo["ids"], geo["bins"], packed, rs, ex, bg, Ts, fi, v_rgb, None, status=geo["status"])
         g = {name: model.flat_grad[a:b_] for name, (a, b_) in model.slices.items()}
         g_vel = torch.empty(6, dtype=torch.float32, device=dev) if model.cam_vel is not None else None
-        check(lib.b200_fused_preprocess_backward(
-            n, ptr(p["means"]), ptr(p["log_scales"]), ptr(p["quats"]), ptr(p["opacity_logit"]), ptr(p["sh_dc"]),
+        _C.fused_preprocess_backward(
+            dev, n, ptr(p["means"]), ptr(p["log_scales"]), ptr(p["quats"]), ptr(p["opacity_logit"]), ptr(p["sh_dc"]),
             ptr(p["sh_rest"]), K, sh_degree_to_use, ptr(cam), ptr(cam_pos), ptr(vel[:3]), ptr(vel[3:]), rs, ex, fx, fy, cx, cy,
             H, W, bw, _CLIP_THRESH, ptr(packed), ptr(radii), ptr(v_xy), ptr(v_pix), ptr(v_conic), ptr(v_col), ptr(v_op),
             ptr(g["means"]), ptr(g["log_scales"]), ptr(g["quats"]), ptr(g["opacity_logit"]), ptr(g["sh_dc"]), ptr(g["sh_rest"]),
-            ptr(g_vel[:3]) if g_vel is not None else None, ptr(g_vel[3:]) if g_vel is not None else None, None, stream()))
+            ptr(g_vel[:3]) if g_vel is not None else None, ptr(g_vel[3:]) if g_vel is not None else None, None)
         if g_vel is not None:
             g["cam_vel"].view(-1, 6).index_add_(0, geo["cam_index"], g_vel.view(1, 6))
     geo["absgrad"] = v_abs   # the `xys.absgrad` side channel of the drop-in operator (densification statistic)
@@ -649,8 +650,10 @@ class PipelinedTrainer:
     # ---- phases (eager or captured) ------------------------------------------------------------------------------
     def _key(self):
         s = self.scene
+        # the deterministic mode records other kernels (and workspaces): toggling torch's flag captures new graphs
         return (s["H"], s["W"], s["fx"], s["fy"], s["cx"], s["cy"], s["block_width"], s["blur_samples"], s["exposure_time"],
-                s["rolling_shutter_time"], self.sh_degree, self.capacity, self.model.N)
+                s["rolling_shutter_time"], self.sh_degree, self.capacity, self.model.N,
+                torch.are_deterministic_algorithms_enabled())
 
     def _entry(self, target_shape_dtype):
         key = self._key() + (target_shape_dtype,)
@@ -671,6 +674,9 @@ class PipelinedTrainer:
             return
         if self.use_graphs and e["warm"] >= 2:  # two eager warm-up rounds (allocator, lazy inits), then capture
             g = torch.cuda.CUDAGraph()
+            # torch does not collect garbage before a capture: an unreachable trainer's pinned host buffers, released by
+            # a collection in the middle of the capture, would invalidate it
+            gc.collect()
             n0 = self._lib_launches()
             with torch.cuda.graph(g, stream=self.main):
                 e["geo"] = self.geometry_fn(self.model, self.st, self.scene, self.capacity, self.status)
@@ -692,6 +698,7 @@ class PipelinedTrainer:
             e["target"] = torch.empty_like(target)
             e["target"].copy_(target)
             g = torch.cuda.CUDAGraph()
+            gc.collect()  # (see _run_A)
             n0 = self._lib_launches()
             with torch.cuda.graph(g, stream=self.main):
                 tgt = self._as_target(e["target"])

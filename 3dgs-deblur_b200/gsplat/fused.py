@@ -149,12 +149,12 @@ class _FusedRender(Function):
             g_lin = torch.empty(3, **f32) if want_vel else None
             g_ang = torch.empty(3, **f32) if want_vel else None
             g_vm = torch.empty(3, 4, **f32) if want_vm else None
-            check(lib.b200_fused_preprocess_backward(
-                n, ptr(means), ptr(log_scales), ptr(quats), ptr(opacity_logit), ptr(sh_dc), ptr(sh_rest), K, deg,
+            _C.fused_preprocess_backward(
+                dev, n, ptr(means), ptr(log_scales), ptr(quats), ptr(opacity_logit), ptr(sh_dc), ptr(sh_rest), K, deg,
                 ptr(viewmat), ptr(cam_pos), ptr(lin_d), ptr(ang_d), rs, ex, fx, fy, cx, cy, H, W, bw, clip, ptr(packed),
                 ptr(radii), ptr(v_xy), ptr(v_pix), ptr(v_conic), ptr(v_col), ptr(v_op), ptr(out["means"]),
                 ptr(out["log_scales"]), ptr(out["quats"]), ptr(out["opacity_logit"]), ptr(out["sh_dc"]), ptr(out["sh_rest"]),
-                ptr(g_lin), ptr(g_ang), ptr(g_vm), stream()))
+                ptr(g_lin), ptr(g_ang), ptr(g_vm))
         ret = [None if name in sink else out[name].view_as(like)
                for name, like in (("means", means), ("log_scales", log_scales), ("quats", quats),
                                   ("opacity_logit", opacity_logit), ("sh_dc", sh_dc), ("sh_rest", sh_rest))]
@@ -166,5 +166,8 @@ class _FusedRender(Function):
         v_ang = g_ang.reshape(ctx.vel_shapes[1]).to(ctx.vel_devs[1]) if (want_vel and ctx.needs_input_grad[9]) else None
         v_bg = None
         if ctx.needs_input_grad[10]:
-            v_bg = torch.matmul(v_rgb.float().reshape(-1, 3).t(), Ts.mean(dim=-1).float().reshape(-1, 1)).squeeze()
+            if torch.are_deterministic_algorithms_enabled():  # a fixed-order reduction instead of cuBLAS
+                v_bg = (v_rgb.float() * Ts.mean(dim=-1).float()[..., None]).sum((0, 1))
+            else:
+                v_bg = torch.matmul(v_rgb.float().reshape(-1, 3).t(), Ts.mean(dim=-1).float().reshape(-1, 1)).squeeze()
         return (*ret, v_viewmat, None, v_lin, v_ang, v_bg, None, None, None)

@@ -151,6 +151,7 @@ class _RasterizeGaussians(Function):
                                                                       rolling_shutter_time, exposure_time, background,
                                                                       want_alpha=True, status=prepared.status)
             ctx.cfg = (H, W, bw, blur_samples, rolling_shutter_time, exposure_time, 1, True)
+            ctx.status = prepared.status  # where the capacity-sized lists' padding starts (deterministic backward)
             ctx.save_for_backward(ids_sorted, tile_bins, xys, pix_vels, conics, colors, opacity, background, final_Ts,
                                   final_idx, packed)
             ctx.set_materialize_grads(False)
@@ -216,9 +217,10 @@ class _RasterizeGaussians(Function):
                 torch.zeros_like(t) for t in (xys, xys, pix_vels, conics, colors, opacity))
         elif has_packed:
             # grad_alpha None = zero alpha cotangent: the kernel then reads no (H, W) buffer for it
+            capacity_lists = {"status": ctx.status} if hasattr(ctx, "status") else {}
             v_xy, v_xy_abs, v_pix_vels, v_conic, v_colors, v_opacity = _C.blend_backward_packed(
                 xys.size(0), H, W, bw, n_samples, ids_sorted, tile_bins, packed, rs_time, exposure, background, final_Ts,
-                final_idx, grad_img.contiguous(), grad_alpha)
+                final_idx, grad_img.contiguous(), grad_alpha, **capacity_lists)
             v_opacity = v_opacity.reshape(opacity.shape)
         else:
             v_xy, v_xy_abs, v_pix_vels, v_conic, v_colors, v_opacity = _C.nd_rasterize_backward(
@@ -229,8 +231,11 @@ class _RasterizeGaussians(Function):
         v_background = None
         if background.requires_grad:  # d img / d background = mean_s(final T) per pixel
             t_mean = final_Ts.mean(dim=-1) if final_Ts.dim() == 3 else final_Ts
-            v_background = torch.matmul(grad_img.float().reshape(-1, background.shape[0]).t(),
-                                        t_mean.float().reshape(-1, 1)).squeeze()
+            if torch.are_deterministic_algorithms_enabled():  # a fixed-order reduction instead of cuBLAS
+                v_background = (grad_img.float() * t_mean.float()[..., None]).sum((0, 1))
+            else:
+                v_background = torch.matmul(grad_img.float().reshape(-1, background.shape[0]).t(),
+                                            t_mean.float().reshape(-1, 1)).squeeze()
 
         xys.absgrad = v_xy_abs  # AbsGS split criterion side channel (rasterize.py:272-275)
 

@@ -214,6 +214,56 @@ B200_API int b200_blend_backward_packed_ordered(int num_points, unsigned img_hei
                                                 float *v_pix_vels, float *v_conic, float *v_colors, float *v_opacity,
                                                 int outputs_are_zero, void *stream);
 
+/* ---- deterministic mode ----------------------------------------------------------------------------------------------
+ * The backward entry points above add per-Gaussian (blend) and per-block (camera) partial sums with float atomics, so
+ * their last bits depend on scheduling.  These variants compute the same gradients with every sum in a fixed order, so
+ * repeated calls on the same inputs are bit-identical (gsplat uses them under torch.use_deterministic_algorithms).
+ *
+ * b200_blend_backward_packed_deterministic = b200_blend_backward_packed_ordered, except: each warp visit stores its 13
+ * sums to the workspace at (list position, warp) instead of adding them; the list positions are grouped by Gaussian
+ * (stable radix sort of (Gaussian id, position)); each Gaussian's sums are added in ascending position, then ascending
+ * warp.  The six outputs are written for every Gaussian (zeros where it has no entry).  num_entries = length of
+ * gaussian_ids_sorted; status (may be null) = the capacity-mode status of b200_bin_cull_emit_capacity: positions from
+ * status[1] on are padding and join no Gaussian.  tile_order may be null (raster order); the result does not depend on
+ * it.  ws: 256-byte aligned, b200_blend_backward_deterministic_ws_bytes(num_points, num_entries, block_width) bytes:
+ * 52 bytes per (entry, warp) with 4 warps per entry at block_width 16 (8 otherwise), plus 16 bytes per entry, 8 per
+ * Gaussian and the sort's temporary storage.
+ *
+ * b200_project_gaussians_backward_deterministic / b200_fused_preprocess_backward_deterministic = the entry points
+ * without the suffix; each block stores its 18 camera partials to ws and one more small kernel sums them in block
+ * order.  ws: 16-byte aligned, *_ws_bytes(num_points) bytes (18 floats per block of 256 / 128 Gaussians); unused when
+ * no camera gradient is requested. */
+B200_API size_t b200_blend_backward_deterministic_ws_bytes(int num_points, int num_entries, unsigned block_width);
+B200_API int b200_blend_backward_packed_deterministic(int num_points, int num_entries, unsigned img_height,
+                                                      unsigned img_width, unsigned block_width, unsigned n_blur_samples,
+                                                      const int32_t *gaussian_ids_sorted, const int32_t *tile_bins,
+                                                      const void *packed, float rolling_shutter_time, float exposure_time,
+                                                      const float *background, const float *final_Ts,
+                                                      const int32_t *final_idx, const float *v_output,
+                                                      const float *v_output_alpha, const int32_t *status,
+                                                      const int32_t *tile_order, void *ws, size_t ws_bytes, float *v_xy,
+                                                      float *v_xy_abs, float *v_pix_vels, float *v_conic,
+                                                      float *v_colors, float *v_opacity, void *stream);
+B200_API size_t b200_project_gaussians_backward_ws_bytes(int num_points);
+B200_API int b200_project_gaussians_backward_deterministic(
+    int num_points, const float *means3d, const float *scales, float glob_scale, const float *quats,
+    const float *lin_vel, const float *ang_vel, float rolling_shutter_time, float exposure_time, const float *viewmat,
+    float fx, float fy, float cx, float cy, unsigned img_height, unsigned img_width, const float *cov3d,
+    const int32_t *radii, const float *conics, const float *compensation, const float *v_xy, const float *v_depth,
+    const float *v_pix_vel, const float *v_conic, const float *v_compensation, unsigned flags, float *v_cov2d,
+    float *v_cov3d, float *v_mean3d, float *v_scale, float *v_quat, float *v_lin_vel, float *v_ang_vel, float *v_viewmat,
+    void *ws, size_t ws_bytes, void *stream);
+B200_API size_t b200_fused_preprocess_backward_ws_bytes(int num_points);
+B200_API int b200_fused_preprocess_backward_deterministic(
+    int num_points, const float *means, const float *log_scales, const float *quats, const float *opacity_logit,
+    const float *sh_dc, const float *sh_rest, int sh_bases, int degrees_to_use, const float *viewmat,
+    const float *cam_pos, const float *lin_vel, const float *ang_vel, float rolling_shutter_time, float exposure_time,
+    float fx, float fy, float cx, float cy, unsigned img_height, unsigned img_width, unsigned block_width,
+    float clip_thresh, const void *packed, const int32_t *radii, const float *v_xy, const float *v_pix_vel,
+    const float *v_conic, const float *v_colors, const float *v_opacity, float *g_means, float *g_log_scales,
+    float *g_quats, float *g_opacity_logit, float *g_sh_dc, float *g_sh_rest, float *g_lin_vel, float *g_ang_vel,
+    float *g_viewmat, void *ws, size_t ws_bytes, void *stream);
+
 /* ---- blend (blur + rolling shutter), 3 channels ------------------------------------------
  * replaces rasterize_forward_tensor (bindings.h:110-127, bindings.cu:424-503; kernel forward.cu:306-456).
  * packed_ws: scratch of num_points * b200_packed_record_bytes() bytes, 16-byte aligned (filled here).
