@@ -33,6 +33,11 @@ __device__ __forceinline__ float4 load_quat(const FusedParams &f, int i) {
 
 __device__ __forceinline__ float sigmoidf_(float x) { return 1.f / (1.f + __expf(-x)); }
 
+// clamp(c + 0.5, min=0) of the record, with the clamp's side kept in the sign bit: -0 where the clamp cut the colour, +0
+// where c + 0.5 is exactly 0.  torch.clamp passes the gradient at the boundary, so the backward gates on !signbit; the
+// blend only multiplies the colour, so -0 changes no image bit.
+__device__ __forceinline__ float clamp_colour(float c) { return c >= 0.f ? c : -0.f; }
+
 // SH colour of Gaussian i before the + 0.5 / clamp (splatfacto.py:840-846): "fast" basis, dc and rest tensors read apart.
 template <int DEG_USE>
 __device__ __forceinline__ void sh_colour(const FusedParams &f, int i, const float *m, float &c0, float &c1, float &c2) {
@@ -73,7 +78,7 @@ __global__ void __launch_bounds__(FUSED_THREADS) fused_forward_kernel(FusedParam
         if constexpr (DEG_USE >= 0) sh_colour<DEG_USE>(f, i, m, c0, c1, c2);
         const float opac = sigmoidf_(f.opacity_logit[i]) * r.comp;  // splatfacto.py:853-854 ("antialiased")
         g = make_record(i, r.xy[0], r.xy[1], r.vel[0], r.vel[1], r.conic[0], r.conic[1], r.conic[2], opac,
-                        fmaxf(c0 + 0.5f, 0.f), fmaxf(c1 + 0.5f, 0.f), fmaxf(c2 + 0.5f, 0.f));  // :846
+                        clamp_colour(c0 + 0.5f), clamp_colour(c1 + 0.5f), clamp_colour(c2 + 0.5f));  // :846
     } else {
         g = make_record(i, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f);  // hx = -1: never blended
     }
@@ -89,7 +94,7 @@ __global__ void __launch_bounds__(FUSED_THREADS) fused_colors_kernel(FusedParams
     if (i >= f.proj.n || radii[i] <= 0) return;
     float c0, c1, c2;
     sh_colour<DEG_USE>(f, i, f.proj.means + 3 * (size_t)i, c0, c1, c2);
-    rec[i].r = fmaxf(c0 + 0.5f, 0.f); rec[i].g = fmaxf(c1 + 0.5f, 0.f); rec[i].b = fmaxf(c2 + 0.5f, 0.f);
+    rec[i].r = clamp_colour(c0 + 0.5f); rec[i].g = clamp_colour(c1 + 0.5f); rec[i].b = clamp_colour(c2 + 0.5f);
 }
 
 struct FusedBwdIO {
@@ -148,9 +153,10 @@ __global__ void __launch_bounds__(FUSED_THREADS) fused_backward_kernel(FusedPara
         ProjGaussOut r;
         project_forward_one(f.proj, in, r);  // recompute instead of saving 40 B per Gaussian
         const float4 C = *reinterpret_cast<const float4 *>(&io.rec[i].r);  // clamped colour of the forward
-        // colour: clamp gate, then basis outer product (sh.cuh:467-498)
-        const float v0 = C.x > 0.f ? io.v_colors[3 * (size_t)i] : 0.f, v1 = C.y > 0.f ? io.v_colors[3 * (size_t)i + 1] : 0.f,
-                    v2 = C.z > 0.f ? io.v_colors[3 * (size_t)i + 2] : 0.f;
+        // colour: clamp gate (see clamp_colour), then basis outer product (sh.cuh:467-498)
+        const float v0 = !signbit(C.x) ? io.v_colors[3 * (size_t)i] : 0.f,
+                    v1 = !signbit(C.y) ? io.v_colors[3 * (size_t)i + 1] : 0.f,
+                    v2 = !signbit(C.z) ? io.v_colors[3 * (size_t)i + 2] : 0.f;
         float B[KU];
         sh_basis<B200_SH_FAST>(DEG_USE, m[0] - __ldg(f.cam_pos), m[1] - __ldg(f.cam_pos + 1), m[2] - __ldg(f.cam_pos + 2), B);
         g_dc[0] = B[0] * v0; g_dc[1] = B[0] * v1; g_dc[2] = B[0] * v2;

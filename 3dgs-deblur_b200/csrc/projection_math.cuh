@@ -189,7 +189,9 @@ __device__ __forceinline__ void project_backward_one(const ProjCommon &p, bool w
             const float comp = sv.comp;
             const float inv_det = ca * cc - cb * cb;
             const float om = 1.f - comp * comp;
-            const float vsq = ct.v_comp * 0.5f / (comp + 1e-6f);
+            // d sqrt(r) / dr = 0.5 / sqrt(r), and 0 where r <= 0 clamps comp to 0.  The reference CUDA backward
+            // (EXACT = false) divides by comp + 1e-6 instead.
+            const float vsq = EXACT ? (comp > 0.f ? ct.v_comp * 0.5f / comp : 0.f) : ct.v_comp * 0.5f / (comp + 1e-6f);
             vc2[0] += vsq * (om * ca - 0.3f * inv_det);
             vc2[1] += 2.f * vsq * (om * cb);
             vc2[2] += vsq * (om * cc - 0.3f * inv_det);

@@ -295,6 +295,10 @@ B200_API int b200_rasterize_backward(int num_points, unsigned img_height, unsign
  *             parameters, every row written (zeros for culled Gaussians), plus optional camera gradients
  *             (g_lin_vel[3], g_ang_vel[3], g_viewmat[12]; overwritten).  Projection gradients are the clamp-aware
  *             "exact" ones (B200_PROJ_EXACT).
+ * Colour clamp: the forward stores a colour the clamp cut as -0.0f and an exact rgb + 0.5 == 0 as +0.0f, and the backward
+ * passes the colour gradient where the record's colour has a clear sign bit (torch.clamp(min=0) is inclusive).  So the
+ * backward expects `packed` as the fused forward kernels wrote it: records built by b200_pack_records, or recoloured by
+ * b200_set_record_colors from clamped colours, hold +0 for cut colours and would pass their gradient.
  * sh_dc (N,3) and sh_rest (N,K-1,3) are the two Splatfacto tensors (no torch.cat needed); sh_bases = K. */
 B200_API int b200_fused_preprocess_forward(int num_points, const float *means, const float *log_scales,
                                            const float *quats, const float *opacity_logit, const float *sh_dc,
@@ -306,7 +310,8 @@ B200_API int b200_fused_preprocess_forward(int num_points, const float *means, c
                                            int32_t *num_tiles_hit, void *stream);
 /* The forward in two halves, for a trainer that projects and bins image k+1 while the SH coefficients of step k are still
  * being exchanged / updated (gsplat.dp.PipelinedTrainer): b200_fused_geometry_forward reads the geometry parameters only
- * and leaves the records' colours 0; b200_fused_colors_forward fills clamp(SH colour + 0.5, 0) into the records of the
+ * and leaves the records' colours 0; b200_fused_colors_forward fills clamp(SH colour + 0.5, 0) (a cut colour as -0, see
+ * above) into the records of the
  * Gaussians with radii > 0 afterwards (the binning does not read colours).  Together they write what
  * b200_fused_preprocess_forward writes; b200_fused_preprocess_backward serves both. */
 B200_API int b200_fused_geometry_forward(int num_points, const float *means, const float *log_scales, const float *quats,

@@ -35,7 +35,10 @@ def _oracle_backward_chain(d, r, v_out, v_alpha):
     rb = O.rasterize_backward(d["H"], d["W"], 16, d["S"], b["gaussian_ids_sorted"], b["tile_bins"], r["proj"]["xys"],
                               r["proj"]["pix_vels"], d["rs"], d["exposure"], r["proj"]["conics"], r["colors"], r["opac"],
                               d["background"], r["final_Ts"], r["final_idx"], v_out, v_alpha)
-    gate = (r["colors"] > 0).astype(np.float32)  # clamp(rgb + 0.5, min=0)
+    # clamp(rgb + 0.5, min=0) passes the gradient where rgb + 0.5 >= 0 (inclusive, like torch.clamp); r["colors"] is
+    # already clamped, so the gate is taken on the colour before the clamp
+    raw = O.sh_forward("fast", 3, d["means"] - d["cam_pos"][None], d["sh"]) + np.float32(0.5)
+    gate = (raw >= 0).astype(np.float32)
     v_sh = O.sh_backward("fast", 3, 3, d["means"] - d["cam_pos"][None], rb["v_colors"] * gate)
     pb = O.project_backward(d["means"], d["scales"], 1.0, d["quats"], d["lin_vel"], d["ang_vel"], d["rs"], d["exposure"],
                             d["viewmat"], d["fx"], d["fy"], r["proj"]["cov3d"], r["proj"]["radii"], r["proj"]["conics"],
