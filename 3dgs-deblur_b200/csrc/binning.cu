@@ -278,20 +278,29 @@ __global__ void __launch_bounds__(256) cull_keys_kernel(int n, const PackedGauss
     vals[g] = g;
 }
 
-// counters: [0] = sum of reserved slots (the reference's num_intersects), [1] = phantom slots,
-//           [2] = 1 if Gaussian 0 can touch tile 0, [3] = number of list entries after culling (filled later),
+// counters (cull_finish_kernel fills the batch words from the per-view ones):
+//   [0] = sum of reserved slots over the views (the reference's num_intersects of one view), [1] = phantom slots,
+//   [2] = 1 if Gaussian 0 of view 0 can touch tile 0, [3] = number of list entries after culling, [4] = deferred
+//   input-check word, [5] = phantom entries kept (ahead of the real ones), [6] = 1 if [0] overflowed int32;
+//   from CULL_VIEW_WORDS on, 4 words per view v: reserved slots, phantom slots, Gaussian v * n_view can touch tile 0
+//   of the view, first list slot of the view's phantom entries.
 // Work is split into chunks of 32 candidate tiles (a screen-filling splat reserves 2500 of them, most reserve < 16):
 // one warp per chunk, chunk -> Gaussian by binary search in the chunk prefix sum, so a handful of huge splats
 // cannot serialise the pass.
-__global__ void __launch_bounds__(256) cull_prep_kernel(int n, const PackedGaussian *__restrict__ rec,
+constexpr int CULL_VIEW_WORDS = 8;
+// Grid (ceil(n_view / 256), views): a warp never spans two views.  Record g = v * n_view + (index within the view).
+__global__ void __launch_bounds__(256) cull_prep_kernel(int n_view, const PackedGaussian *__restrict__ rec,
                                                         const int32_t *__restrict__ radii,
                                                         const int32_t *__restrict__ tiles_hit, CullGeom c,
                                                         int4 *__restrict__ bbox, int32_t *__restrict__ chunks,
                                                         int32_t *__restrict__ survivors, int32_t *__restrict__ cursor,
                                                         int32_t *__restrict__ counters) {
-    const int g = blockIdx.x * blockDim.x + threadIdx.x;
+    const int gl = blockIdx.x * blockDim.x + threadIdx.x;
+    const int v = blockIdx.y;
+    const int g = v * n_view + gl;
+    int32_t *vc = counters + CULL_VIEW_WORDS + 4 * v;
     int reserved = 0, phantom = 0;
-    if (g < n) {
+    if (gl < n_view) {
         reserved = tiles_hit[g];
         const TileRect t =
             ref_tile_rect(*reinterpret_cast<const float2 *>(&rec[g].x), radii[g], reserved, c.tbx, c.tby, (float)c.bw);
@@ -300,13 +309,13 @@ __global__ void __launch_bounds__(256) cull_prep_kernel(int n, const PackedGauss
         survivors[g] = 0;
         cursor[g] = 0;
         phantom = max(0, reserved - t.emitted);
-        if (g == 0) counters[2] = (c.per_sample ? tile_survives<true>(rec[0], 0, 0, c) : tile_survives<false>(rec[0], 0, 0, c)) ? 1 : 0;
+        if (gl == 0) vc[2] = (c.per_sample ? tile_survives<true>(rec[g], 0, 0, c) : tile_survives<false>(rec[g], 0, 0, c)) ? 1 : 0;
     }
     reserved = __reduce_add_sync(0xffffffffu, reserved);
     phantom = __reduce_add_sync(0xffffffffu, phantom);
     if ((threadIdx.x & 31) == 0) {
-        if (reserved) atomicAdd(counters + 0, reserved);
-        if (phantom) atomicAdd(counters + 1, phantom);
+        if (reserved) atomicAdd(vc + 0, reserved);
+        if (phantom) atomicAdd(vc + 1, phantom);
     }
 }
 
@@ -338,8 +347,9 @@ __device__ __forceinline__ int next_owner(const int32_t *__restrict__ chunk_off,
 // One warp per contiguous span of chunks.  The count pass tests every candidate tile once and keeps the 32-bit
 // survival mask of each chunk (the first `mask_cap` chunks; later ones are simply re-tested), the emit pass expands
 // the stored masks into (tile, Gaussian) entries without repeating the geometry, skipping dead chunks outright.
+// n = views * n_view records; the tile keys of view v are v * num_tiles + (tile in the view).
 template <bool EMIT, bool PER_SAMPLE>
-__global__ void __launch_bounds__(256, 8) cull_chunks_kernel(int n, int total_entries,
+__global__ void __launch_bounds__(256, 8) cull_chunks_kernel(int n, int n_view, int views, int total_entries,
                                                           const PackedGaussian *__restrict__ rec,
                                                           const int4 *__restrict__ bbox,
                                                           const int32_t *__restrict__ chunk_off,
@@ -355,11 +365,17 @@ __global__ void __launch_bounds__(256, 8) cull_chunks_kernel(int n, int total_en
     const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int warps = (gridDim.x * blockDim.x) >> 5;
     const int total_chunks = __ldg(chunk_off + n - 1) + __ldg(chunks + n - 1);
-    const int phantoms = counters[2] ? counters[1] : 0;
+    const int num_tiles = c.tbx * c.tby;
+    const int phantoms = counters[5];
     if (EMIT) {
-        for (int k = blockIdx.x * blockDim.x + threadIdx.x; k < min(phantoms, total_entries); k += gridDim.x * blockDim.x) {
-            tile_keys[k] = 0u;
-            ids[k] = 0;
+        // every view's phantom entries (key: the view's tile 0, id: the view's Gaussian 0), ahead of all real entries
+        for (int v = 0; v < views; ++v) {
+            const int32_t *vc = counters + CULL_VIEW_WORDS + 4 * v;
+            const int cnt = vc[2] ? vc[1] : 0, first = vc[3];
+            for (int k = blockIdx.x * blockDim.x + threadIdx.x; k < min(cnt, total_entries - first); k += gridDim.x * blockDim.x) {
+                tile_keys[first + k] = (uint32_t)(v * num_tiles);
+                ids[first + k] = v * n_view;
+            }
         }
         if (status) {
             // capacity mode (b200_bin_cull_emit_capacity): `total_entries` is the caller's list capacity, the real entry
@@ -382,6 +398,7 @@ __global__ void __launch_bounds__(256, 8) cull_chunks_kernel(int n, int total_en
     const int per = (total_chunks + warps - 1) / warps;
     const int c0 = warp * per, c1 = min(total_chunks, c0 + per);
     int g = -1, g_first = 0, g_chunks = 0;
+    uint32_t key_base = 0u;  // view of record g times num_tiles
     int4 bb = make_int4(0, 0, 1, 0);
     for (int cb = c0; cb < c1; cb += 32) {
         uint32_t stored = 0u;
@@ -399,6 +416,7 @@ __global__ void __launch_bounds__(256, 8) cull_chunks_kernel(int n, int total_en
                 bb = bbox[g];
                 g_first = __ldg(chunk_off + g);
                 g_chunks = (bb.w + 31) >> 5;
+                if (views > 1) key_base = (uint32_t)((g / n_view) * num_tiles);
             }
             const int k = ((chunk - g_first) << 5) + lane;
             bool keep = false;
@@ -424,7 +442,7 @@ __global__ void __launch_bounds__(256, 8) cull_chunks_kernel(int n, int total_en
                 if (keep) {
                     const int dst = base + __popc(m & ((1u << lane) - 1u));
                     if (dst < total_entries) {
-                        tile_keys[dst] = (uint32_t)(ty * c.tbx + tx);
+                        tile_keys[dst] = key_base + (uint32_t)(ty * c.tbx + tx);
                         ids[dst] = g;
                     }
                 }
@@ -433,18 +451,35 @@ __global__ void __launch_bounds__(256, 8) cull_chunks_kernel(int n, int total_en
     }
 }
 
-// Gaussian -> first slot of its entries (depth order), and the culled entry total for the host
-__global__ void __launch_bounds__(256) cull_finish_kernel(int n, const int32_t *__restrict__ order,
+// Gaussian -> first slot of its entries (depth order), and the culled entry total for the host.  The last thread also
+// lays out the views' phantom entries (view order) and sums the per-view counters into the batch words; view_isect
+// (DEVICE int32[views] or null) receives every view's reference num_intersects.
+__global__ void __launch_bounds__(256) cull_finish_kernel(int n, int views, const int32_t *__restrict__ order,
                                                           const int32_t *__restrict__ offs,
                                                           const int32_t *__restrict__ surv_sorted,
                                                           int32_t *__restrict__ base_of, int32_t *__restrict__ counters,
-                                                          const int32_t *__restrict__ flag) {
+                                                          const int32_t *__restrict__ flag, int32_t *__restrict__ view_isect) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) {
         base_of[order[i]] = offs[i];
         if (i == n - 1) {
-            counters[3] = (counters[2] ? counters[1] : 0) + offs[i] + surv_sorted[i];
+            long long reserved = 0, phantom_slots = 0;
+            int phantoms = 0;
+            for (int v = 0; v < views; ++v) {
+                int32_t *vc = counters + CULL_VIEW_WORDS + 4 * v;
+                reserved += vc[0];
+                phantom_slots += vc[1];
+                vc[3] = phantoms;
+                phantoms += vc[2] ? vc[1] : 0;  // (<= reserved: fits while [6] is clear)
+                if (view_isect) view_isect[v] = vc[0];
+            }
+            counters[0] = (int32_t)min(reserved, 0x7fffffffll);
+            counters[1] = (int32_t)min(phantom_slots, 0x7fffffffll);
+            counters[2] = counters[CULL_VIEW_WORDS + 2];
+            counters[3] = phantoms + offs[i] + surv_sorted[i];
             counters[4] = flag ? *flag : 0;  // deferred input-check word rides along with the totals
+            counters[5] = phantoms;
+            counters[6] = reserved > 0x7fffffffll ? 1 : 0;
         }
     }
 }
@@ -619,14 +654,14 @@ static int cull_mask_cap(int n) {
     if (forced >= 0) return (int)std::min<long long>(forced, 1ll << 30);
     return (int)std::min<long long>(4ll * n + 65536ll, 1ll << 28);
 }
-static CullWsG cull_ws_g(int n) {
+static CullWsG cull_ws_g(int n, int views = 1) {
     CullWsG L;
     WsCarver ws;
     L.keys_a = ws.take(4 * (size_t)n); L.keys_b = ws.take(4 * (size_t)n); L.vals_a = ws.take(4 * (size_t)n);
     L.order = ws.take(4 * (size_t)n); L.survivors = ws.take(4 * (size_t)n); L.surv_sorted = ws.take(4 * (size_t)n);
     L.offs = ws.take(4 * (size_t)n); L.bbox = ws.take(16 * (size_t)n); L.chunks = ws.take(4 * (size_t)n);
     L.chunk_off = ws.take(4 * (size_t)n); L.cursor = ws.take(4 * (size_t)n); L.base_of = ws.take(4 * (size_t)n);
-    L.counters = ws.take(256);
+    L.counters = ws.take(4 * (size_t)(CULL_VIEW_WORDS + 4 * views));
     L.mask_cap = cull_mask_cap(n);
     L.masks = ws.take(4 * (size_t)(L.mask_cap > 0 ? L.mask_cap : 1));
     L.cub_bytes = cub_temp_bytes(SORT32, n) + 256;  // depth sort (side stream)
@@ -650,6 +685,10 @@ static CullWsE cull_ws_e(int m) {
 }
 
 extern "C" size_t b200_bin_cull_ws_bytes(int num_points) { return cull_ws_g(num_points > 0 ? num_points : 1).total; }
+extern "C" size_t b200_bin_cull_views_ws_bytes(int num_views, int num_points) {
+    if (num_views < 1 || num_points < 1 || (long long)num_views * num_points > 0x7fffffffll) return 0;
+    return cull_ws_g(num_views * num_points, num_views).total;
+}
 extern "C" size_t b200_bin_cull_emit_ws_bytes(int num_entries) { return cull_ws_e(num_entries > 0 ? num_entries : 1).total; }
 
 // One non-blocking helper stream + fork/join events per device, created on first use and kept for the process.
@@ -700,18 +739,22 @@ static CullGeom make_cull_geom(unsigned H, unsigned W, unsigned bw, unsigned S, 
     return c;
 }
 
-extern "C" int b200_bin_cull_count(int num_points, const void *packed, const float *depths, const int32_t *radii,
-                                   const int32_t *num_tiles_hit, unsigned img_height, unsigned img_width,
-                                   unsigned block_width, unsigned n_blur_samples, float rolling_shutter_time,
-                                   float exposure_time, void *ws_g, size_t ws_g_bytes, int32_t *totals_host_pinned,
-                                   const int32_t *flag_dev, void *stream) {
+// Count phase over views * num_points records (view v's Gaussian g is record v * num_points + g).
+static int cull_count(int views, int num_points, const void *packed, const float *depths, const int32_t *radii,
+                      const int32_t *num_tiles_hit, unsigned img_height, unsigned img_width, unsigned block_width,
+                      unsigned n_blur_samples, float rolling_shutter_time, float exposure_time, void *ws_g,
+                      size_t ws_g_bytes, int32_t *totals_host_pinned, int32_t *view_isect, const int32_t *flag_dev,
+                      void *stream) {
+    B200_REQUIRE(views >= 1, "num_views must be >= 1");
+    B200_REQUIRE(views <= 65535, "num_views must be <= 65535");
     B200_REQUIRE(num_points >= 1, "num_points must be >= 1");
+    B200_REQUIRE((long long)views * num_points <= 0x7fffffffll, "num_views * num_points exceeds int32");
     B200_REQUIRE(block_width > 1 && block_width <= 16, "block_width must be between 2 and 16");
     B200_REQUIRE(n_blur_samples > 0 && n_blur_samples <= B200_MAX_BLUR_SAMPLES, "unsupported blur size");
     B200_REQUIRE(packed && depths && radii && num_tiles_hit && ws_g, "null pointer");
     B200_REQUIRE((reinterpret_cast<uintptr_t>(ws_g) & 255u) == 0, "workspace must be 256-byte aligned");
-    const int n = num_points;
-    const CullWsG L = cull_ws_g(n);
+    const int n = views * num_points;
+    const CullWsG L = cull_ws_g(n, views);
     B200_REQUIRE(ws_g_bytes >= L.total, "workspace too small: %zu < %zu", ws_g_bytes, L.total);
     char *base = static_cast<char *>(ws_g);
     uint32_t *keys_a = (uint32_t *)(base + L.keys_a), *keys_b = (uint32_t *)(base + L.keys_b);
@@ -731,7 +774,7 @@ extern "C" int b200_bin_cull_count(int num_points, const void *packed, const flo
     const PackedGaussian *rec = reinterpret_cast<const PackedGaussian *>(packed);
     SideStream side;
     B200_REQUIRE(side_stream(side), "could not create the binning side stream");
-    B200_CUDA(cudaMemsetAsync(counters, 0, 256, st));
+    B200_CUDA(cudaMemsetAsync(counters, 0, 4 * (size_t)(CULL_VIEW_WORDS + 4 * views), st));
     // the depth sort only needs depths and the visibility of each Gaussian: it is forked first and runs beside cull_prep,
     // the scan and the tile tests (chains of short kernels, the sort's being the longest)
     {
@@ -745,12 +788,14 @@ extern "C" int b200_bin_cull_count(int num_points, const void *packed, const flo
         count_launch(5);
         B200_CUDA(cudaEventRecord(side.join, side.stream));
     }
-    cull_prep_kernel<<<ceil_div(n, 256), 256, 0, st>>>(n, rec, radii, num_tiles_hit, c, bbox, chunks, survivors, cursor, counters);
+    cull_prep_kernel<<<dim3(ceil_div(num_points, 256), views), 256, 0, st>>>(num_points, rec, radii, num_tiles_hit, c, bbox,
+                                                                           chunks, survivors, cursor, counters);
     B200_LAUNCH_CHECK();
     B200_CUDA(cub::DeviceScan::ExclusiveSum(scan_ws, scan_bytes, chunks, chunk_off, n, st));
     count_launch(2);
     (c.per_sample ? cull_chunks_kernel<false, true> : cull_chunks_kernel<false, false>)<<<CULL_COUNT_GRID, 256, 0, st>>>(
-        n, 0, rec, bbox, chunk_off, chunks, c, counters, masks, L.mask_cap, survivors, nullptr, nullptr, nullptr, nullptr, 0u, nullptr);
+        n, num_points, views, 0, rec, bbox, chunk_off, chunks, c, counters, masks, L.mask_cap, survivors, nullptr, nullptr,
+        nullptr, nullptr, 0u, nullptr);
     B200_LAUNCH_CHECK();
     // (a later record of the shared join event by another caller is ordered after this one on the side stream)
     B200_CUDA(cudaStreamWaitEvent(st, side.join, 0));
@@ -758,20 +803,46 @@ extern "C" int b200_bin_cull_count(int num_points, const void *packed, const flo
     B200_LAUNCH_CHECK();
     B200_CUDA(cub::DeviceScan::ExclusiveSum(scan_ws, scan_bytes, surv_sorted, offs, n, st));
     count_launch(2);
-    cull_finish_kernel<<<ceil_div(n, 256), 256, 0, st>>>(n, order, offs, surv_sorted, base_of, counters, flag_dev);
+    cull_finish_kernel<<<ceil_div(n, 256), 256, 0, st>>>(n, views, order, offs, surv_sorted, base_of, counters, flag_dev,
+                                                          view_isect);
     B200_LAUNCH_CHECK();
     if (totals_host_pinned)  // (null in the capacity mode: nothing on the host waits for the totals)
-        B200_CUDA(cudaMemcpyAsync(totals_host_pinned, counters, 5 * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+        B200_CUDA(cudaMemcpyAsync(totals_host_pinned, counters, (views > 1 ? 7 : 5) * sizeof(int32_t),
+                                  cudaMemcpyDeviceToHost, st));
     return B200_OK;
+}
+
+extern "C" int b200_bin_cull_count(int num_points, const void *packed, const float *depths, const int32_t *radii,
+                                   const int32_t *num_tiles_hit, unsigned img_height, unsigned img_width,
+                                   unsigned block_width, unsigned n_blur_samples, float rolling_shutter_time,
+                                   float exposure_time, void *ws_g, size_t ws_g_bytes, int32_t *totals_host_pinned,
+                                   const int32_t *flag_dev, void *stream) {
+    return cull_count(1, num_points, packed, depths, radii, num_tiles_hit, img_height, img_width, block_width,
+                      n_blur_samples, rolling_shutter_time, exposure_time, ws_g, ws_g_bytes, totals_host_pinned, nullptr,
+                      flag_dev, stream);
+}
+
+extern "C" int b200_bin_cull_count_views(int num_views, int num_points, const void *packed, const float *depths,
+                                         const int32_t *radii, const int32_t *num_tiles_hit, unsigned img_height,
+                                         unsigned img_width, unsigned block_width, unsigned n_blur_samples,
+                                         float rolling_shutter_time, float exposure_time, void *ws_g, size_t ws_g_bytes,
+                                         int32_t *totals_host_pinned, int32_t *view_isect, const int32_t *flag_dev,
+                                         void *stream) {
+    B200_REQUIRE(view_isect, "null per-view array");
+    return cull_count(num_views, num_points, packed, depths, radii, num_tiles_hit, img_height, img_width, block_width,
+                      n_blur_samples, rolling_shutter_time, exposure_time, ws_g, ws_g_bytes, totals_host_pinned, view_isect,
+                      flag_dev, stream);
 }
 
 // Emit phase of both emit entry points, after their argument checks and the tile_bins memset.  m is the entry count of
 // b200_bin_cull_emit, or the list capacity in the capacity mode (status != nullptr), whose padding key num_tiles must
 // sort too.
-static int cull_emit(int n, int m, const CullGeom &c, const void *packed, const void *ws_g, void *ws_e, size_t ws_e_bytes,
-                     int32_t *gaussian_ids_sorted, int32_t *tile_bins, int32_t *status, cudaStream_t st) {
-    const int num_tiles = c.tbx * c.tby;
-    const CullWsG G = cull_ws_g(n);
+// views > 1: n_view Gaussians per view, the lists of view v's tiles at v * tiles_x * tiles_y on.
+static int cull_emit(int views, int n_view, int m, const CullGeom &c, const void *packed, const void *ws_g, void *ws_e,
+                     size_t ws_e_bytes, int32_t *gaussian_ids_sorted, int32_t *tile_bins, int32_t *status, cudaStream_t st) {
+    const int n = views * n_view;
+    const int num_tiles = views * c.tbx * c.tby;
+    const CullWsG G = cull_ws_g(n, views);
     const CullWsE E = cull_ws_e(m);
     B200_REQUIRE(ws_e_bytes >= E.total, "workspace too small: %zu < %zu", ws_e_bytes, E.total);
     char *gb = static_cast<char *>(const_cast<void *>(ws_g));
@@ -779,7 +850,7 @@ static int cull_emit(int n, int m, const CullGeom &c, const void *packed, const 
     uint32_t *tkeys_a = (uint32_t *)(eb + E.tkeys_a), *tkeys_b = (uint32_t *)(eb + E.tkeys_b);
     int32_t *ids_a = (int32_t *)(eb + E.ids_a);
     (c.per_sample ? cull_chunks_kernel<true, true> : cull_chunks_kernel<true, false>)<<<CULL_GRID, 256, 0, st>>>(
-        n, m, reinterpret_cast<const PackedGaussian *>(packed), (const int4 *)(gb + G.bbox), (const int32_t *)(gb + G.chunk_off),
+        n, n_view, views, m, reinterpret_cast<const PackedGaussian *>(packed), (const int4 *)(gb + G.bbox), (const int32_t *)(gb + G.chunk_off),
         (const int32_t *)(gb + G.chunks), c, (const int32_t *)(gb + G.counters), (uint32_t *)(gb + G.masks), G.mask_cap, nullptr,
         (const int32_t *)(gb + G.base_of), (int32_t *)(gb + G.cursor), tkeys_a, ids_a, status ? (uint32_t)num_tiles : 0u, status);
     B200_LAUNCH_CHECK();
@@ -801,7 +872,33 @@ extern "C" int b200_bin_cull_emit(int num_points, int num_entries, const void *p
     if (num_entries == 0) return B200_OK;
     B200_REQUIRE(packed && radii && num_tiles_hit && gaussian_ids_sorted && ws_e, "null pointer");
     B200_REQUIRE((reinterpret_cast<uintptr_t>(ws_e) & 255u) == 0, "workspace must be 256-byte aligned");
-    return cull_emit(num_points, num_entries, c, packed, ws_g, ws_e, ws_e_bytes, gaussian_ids_sorted, tile_bins, nullptr, st);
+    return cull_emit(1, num_points, num_entries, c, packed, ws_g, ws_e, ws_e_bytes, gaussian_ids_sorted, tile_bins, nullptr, st);
+}
+
+extern "C" int b200_bin_cull_emit_views(int num_views, int num_points, int num_entries, const void *packed,
+                                        const int32_t *radii, const int32_t *num_tiles_hit, unsigned img_height,
+                                        unsigned img_width, unsigned block_width, unsigned n_blur_samples,
+                                        float rolling_shutter_time, float exposure_time, const void *ws_g, void *ws_e,
+                                        size_t ws_e_bytes, int32_t *gaussian_ids_sorted, int32_t *tile_bins,
+                                        void *stream) {
+    B200_REQUIRE(num_views >= 1, "num_views must be >= 1");
+    B200_REQUIRE(num_points >= 1 && num_entries >= 0, "bad sizes");
+    B200_REQUIRE((long long)num_views * num_points <= 0x7fffffffll, "num_views * num_points exceeds int32");
+    B200_REQUIRE(block_width > 1 && block_width <= 16, "block_width must be between 2 and 16");
+    B200_REQUIRE(tile_bins && ws_g, "null pointer");
+    const CullGeom c = make_cull_geom(img_height, img_width, block_width, n_blur_samples, rolling_shutter_time, exposure_time);
+    B200_REQUIRE((long long)num_views * c.tbx * c.tby < 0x7fffffffll, "num_views * tiles exceeds int32");
+    if (num_entries > 0) {
+        B200_REQUIRE(packed && radii && num_tiles_hit && gaussian_ids_sorted && ws_e, "null pointer");
+        B200_REQUIRE((reinterpret_cast<uintptr_t>(ws_e) & 255u) == 0, "workspace must be 256-byte aligned");
+        const size_t need = cull_ws_e(num_entries).total;
+        B200_REQUIRE(ws_e_bytes >= need, "workspace too small: %zu < %zu", ws_e_bytes, need);
+    }
+    cudaStream_t st = as_stream(stream);
+    B200_CUDA(cudaMemsetAsync(tile_bins, 0, sizeof(int32_t) * 2 * (size_t)num_views * (size_t)(c.tbx * c.tby), st));
+    if (num_entries == 0) return B200_OK;
+    return cull_emit(num_views, num_points, num_entries, c, packed, ws_g, ws_e, ws_e_bytes, gaussian_ids_sorted, tile_bins,
+                     nullptr, st);
 }
 
 
@@ -826,5 +923,5 @@ extern "C" int b200_bin_cull_emit_capacity(int num_points, int capacity, const v
     const CullGeom c = make_cull_geom(img_height, img_width, block_width, n_blur_samples, rolling_shutter_time, exposure_time);
     cudaStream_t st = as_stream(stream);
     B200_CUDA(cudaMemsetAsync(tile_bins, 0, sizeof(int32_t) * 2 * (size_t)(c.tbx * c.tby), st));
-    return cull_emit(num_points, capacity, c, packed, ws_g, ws_e, ws_e_bytes, gaussian_ids_sorted, tile_bins, status, st);
+    return cull_emit(1, num_points, capacity, c, packed, ws_g, ws_e, ws_e_bytes, gaussian_ids_sorted, tile_bins, status, st);
 }

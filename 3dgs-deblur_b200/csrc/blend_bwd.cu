@@ -35,7 +35,16 @@ struct BlendBwdParams {
     const float *v_out_alpha;  // (H,W), or null for a zero cotangent
     float *v_xy, *v_xy_abs, *v_pix_vel, *v_conic, *v_rgb, *v_opac;
     float *slots;  // DET kernels only: the 13 sums of each warp visit, at (list position, warp) (b200_blend_backward_packed_deterministic)
+    int views;     // images of the launch, laid out as in BlendFwdParams (tile v * tbx * tby + t, rows v * H + i)
 };
+
+// CTA -> (image, tile within the image)
+__device__ __forceinline__ void cta_tile(const int32_t *tile_order, const BlendGeom &g, int &view, int &tile) {
+    const int t = tile_order ? __ldg(tile_order + blockIdx.x) : (int)blockIdx.x;
+    const int per_view = g.tbx * g.tby;
+    view = t / per_view;
+    tile = t - view * per_view;
+}
 
 constexpr int RED_VALUES = 13;  // rgb 3, conic 3, xy 2, |xy| 2, pixel velocity 2, opacity 1
 
@@ -96,9 +105,10 @@ __global__ void __launch_bounds__(BLEND_THREADS, 3) blend_backward_kernel(const 
     __shared__ int s_max[BLEND_THREADS / 32];
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int tile = p.tile_order ? __ldg(p.tile_order + blockIdx.x) : (int)blockIdx.x;
+    int view, tile;
+    cta_tile(p.tile_order, p.g, view, tile);
     const int tile_x = tile % p.g.tbx, tile_y = tile / p.g.tbx;
-    const int2 range = p.tile_bins[tile];
+    const int2 range = p.tile_bins[view * (p.g.tbx * p.g.tby) + tile];
     const float inv_s = 1.0f / (float)S;
     const float bg0 = __ldg(p.background), bg1 = __ldg(p.background + 1), bg2 = __ldg(p.background + 2);
 
@@ -110,7 +120,7 @@ __global__ void __launch_bounds__(BLEND_THREADS, 3) blend_backward_kernel(const 
     const float px = (float)j + 0.5f, py = (float)i + 0.5f;
     const float roll = (float)((double)p.g.rs_time * ((double)(py / (float)p.g.H) - 0.5));
     // per-pixel cotangents and per-sample state (backward.cu:198-217)
-    const size_t pix = inside ? (size_t)i * p.g.W + j : 0;
+    const size_t pix = inside ? (size_t)(view * p.g.H + i) * p.g.W + j : 0;
     float vo0 = 0.f, vo1 = 0.f, vo2 = 0.f, voa = 0.f;
     if (inside) {
         vo0 = p.v_out[3 * pix]; vo1 = p.v_out[3 * pix + 1]; vo2 = p.v_out[3 * pix + 2];
@@ -263,9 +273,10 @@ __global__ void __launch_bounds__(128, BWD_MIN_CTAS) blend_backward_kernel2(cons
     __shared__ __align__(16) float s_red[NT / 32][RED_VALUES * RED_STRIDE];  // per-warp transposition buffer (visit epilogue)
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int tile = p.tile_order ? __ldg(p.tile_order + blockIdx.x) : (int)blockIdx.x;
+    int view, tile;
+    cta_tile(p.tile_order, p.g, view, tile);
     const int tile_x = tile % p.g.tbx, tile_y = tile / p.g.tbx;
-    const int2 range = p.tile_bins[tile];
+    const int2 range = p.tile_bins[view * (p.g.tbx * p.g.tby) + tile];
     const float inv_s = 1.0f / (float)S;
     const float bg0 = __ldg(p.background), bg1 = __ldg(p.background + 1), bg2 = __ldg(p.background + 2);
 
@@ -285,7 +296,7 @@ __global__ void __launch_bounds__(128, BWD_MIN_CTAS) blend_backward_kernel2(cons
         inside[q] = i < p.g.H && j < p.g.W;
         px[q] = (float)j + 0.5f; py[q] = (float)i + 0.5f;
         roll[q] = (float)((double)p.g.rs_time * ((double)(py[q] / (float)p.g.H) - 0.5));
-        const size_t pix = inside[q] ? (size_t)i * p.g.W + j : 0;
+        const size_t pix = inside[q] ? (size_t)(view * p.g.H + i) * p.g.W + j : 0;
         float voa = 0.f;
         vo[q][0] = vo[q][1] = vo[q][2] = 0.f;
         if (inside[q]) {
@@ -504,16 +515,17 @@ static int bwd_warps(unsigned block_width) { return paired_bwd(block_width) ? BL
 
 template <int S, bool DET>
 static int launch_bwd(const BlendBwdParams &p, cudaStream_t st) {
+    const int ctas = p.views * p.g.tbx * p.g.tby;
     if (paired_bwd(p.g.bw)) {
         // per-sample votes ("does any lane hold a contributing pixel", then skip the gradient algebra): without rolling
         // shutter the exact cull leaves 4 % of the entered sample blocks empty and the vote + branch costs more than the
         // masked arithmetic; with it the warp's time window widens the cull and the skip pays
         if (p.g.rs_time != 0.f)
-            blend_backward_kernel2<S, true, DET><<<p.g.tbx * p.g.tby, BLEND_THREADS / 2, 0, st>>>(p);
+            blend_backward_kernel2<S, true, DET><<<ctas, BLEND_THREADS / 2, 0, st>>>(p);
         else
-            blend_backward_kernel2<S, false, DET><<<p.g.tbx * p.g.tby, BLEND_THREADS / 2, 0, st>>>(p);
+            blend_backward_kernel2<S, false, DET><<<ctas, BLEND_THREADS / 2, 0, st>>>(p);
     } else {
-        blend_backward_kernel<S, DET><<<p.g.tbx * p.g.tby, BLEND_THREADS, 0, st>>>(p);
+        blend_backward_kernel<S, DET><<<ctas, BLEND_THREADS, 0, st>>>(p);
     }
     B200_LAUNCH_CHECK();
     return B200_OK;
@@ -585,7 +597,8 @@ static int run_blend_backward(int num_points, unsigned img_height, unsigned img_
                               const float *background, const float *final_Ts, const int32_t *final_idx,
                               const float *v_output, const float *v_output_alpha, float *v_xy, float *v_xy_abs,
                               float *v_pix_vels, float *v_conic, float *v_colors, float *v_opacity, bool outputs_are_zero,
-                              cudaStream_t st, const int32_t *tile_order = nullptr, float *slots = nullptr) {
+                              cudaStream_t st, const int32_t *tile_order = nullptr, float *slots = nullptr,
+                              int views = 1) {
     B200_REQUIRE(n_blur_samples > 0 && n_blur_samples <= B200_MAX_BLUR_SAMPLES, "unsupported blur size");
     B200_REQUIRE(num_points >= 1, "num_points must be >= 1");
     B200_REQUIRE(block_width > 1 && block_width <= 16, "block_width must be between 2 and 16");
@@ -613,6 +626,7 @@ static int run_blend_backward(int num_points, unsigned img_height, unsigned img_
     p.v_xy = v_xy; p.v_xy_abs = v_xy_abs; p.v_pix_vel = v_pix_vels; p.v_conic = v_conic; p.v_rgb = v_colors;
     p.v_opac = v_opacity;
     p.slots = slots;
+    p.views = views;
     return with_blur_samples(n_blur_samples, [&](auto s) {
         return slots ? launch_bwd<decltype(s)::value, true>(p, st) : launch_bwd<decltype(s)::value, false>(p, st);
     });
@@ -654,16 +668,15 @@ extern "C" size_t b200_blend_backward_deterministic_ws_bytes(int num_points, int
     return det_bwd_layout(num_points, num_entries, bwd_warps(block_width)).total;
 }
 
-extern "C" int b200_blend_backward_packed_deterministic(int num_points, int num_entries, unsigned img_height,
-                                                        unsigned img_width, unsigned block_width, unsigned n_blur_samples,
-                                                        const int32_t *gaussian_ids_sorted, const int32_t *tile_bins,
-                                                        const void *packed, float rolling_shutter_time,
-                                                        float exposure_time, const float *background,
-                                                        const float *final_Ts, const int32_t *final_idx,
-                                                        const float *v_output, const float *v_output_alpha,
-                                                        const int32_t *status, const int32_t *tile_order, void *ws,
-                                                        size_t ws_bytes, float *v_xy, float *v_xy_abs, float *v_pix_vels,
-                                                        float *v_conic, float *v_colors, float *v_opacity, void *stream) {
+static int run_blend_backward_deterministic(int views, int num_points, int num_entries, unsigned img_height,
+                                            unsigned img_width, unsigned block_width, unsigned n_blur_samples,
+                                            const int32_t *gaussian_ids_sorted, const int32_t *tile_bins,
+                                            const void *packed, float rolling_shutter_time, float exposure_time,
+                                            const float *background, const float *final_Ts, const int32_t *final_idx,
+                                            const float *v_output, const float *v_output_alpha, const int32_t *status,
+                                            const int32_t *tile_order, void *ws, size_t ws_bytes, float *v_xy,
+                                            float *v_xy_abs, float *v_pix_vels, float *v_conic, float *v_colors,
+                                            float *v_opacity, void *stream) {
     B200_REQUIRE(num_points >= 1, "num_points must be >= 1");
     B200_REQUIRE(num_entries >= 0, "num_entries must be >= 0");
     B200_REQUIRE(num_entries == 0 || gaussian_ids_sorted, "null gaussian_ids_sorted");
@@ -684,7 +697,7 @@ extern "C" int b200_blend_backward_packed_deterministic(int num_points, int num_
         int rc = run_blend_backward(num_points, img_height, img_width, block_width, n_blur_samples, gaussian_ids_sorted,
                                     tile_bins, packed, rolling_shutter_time, exposure_time, background, final_Ts,
                                     final_idx, v_output, v_output_alpha, v_xy, v_xy_abs, v_pix_vels, v_conic, v_colors,
-                                    v_opacity, true, st, tile_order, slots);
+                                    v_opacity, true, st, tile_order, slots, views);
         if (rc) return rc;
         uint32_t *keys_a = reinterpret_cast<uint32_t *>(base + L.keys_a);
         int32_t *pos_a = reinterpret_cast<int32_t *>(base + L.pos_a);
@@ -700,6 +713,68 @@ extern "C" int b200_blend_backward_packed_deterministic(int num_points, int num_
         num_points, warps, slots, pos_sorted, seg, v_colors, v_conic, v_xy, v_xy_abs, v_pix_vels, v_opacity);
     B200_LAUNCH_CHECK();
     return B200_OK;
+}
+
+extern "C" int b200_blend_backward_packed_deterministic(int num_points, int num_entries, unsigned img_height,
+                                                        unsigned img_width, unsigned block_width, unsigned n_blur_samples,
+                                                        const int32_t *gaussian_ids_sorted, const int32_t *tile_bins,
+                                                        const void *packed, float rolling_shutter_time,
+                                                        float exposure_time, const float *background,
+                                                        const float *final_Ts, const int32_t *final_idx,
+                                                        const float *v_output, const float *v_output_alpha,
+                                                        const int32_t *status, const int32_t *tile_order, void *ws,
+                                                        size_t ws_bytes, float *v_xy, float *v_xy_abs, float *v_pix_vels,
+                                                        float *v_conic, float *v_colors, float *v_opacity, void *stream) {
+    return run_blend_backward_deterministic(1, num_points, num_entries, img_height, img_width, block_width, n_blur_samples,
+                                            gaussian_ids_sorted, tile_bins, packed, rolling_shutter_time, exposure_time,
+                                            background, final_Ts, final_idx, v_output, v_output_alpha, status, tile_order,
+                                            ws, ws_bytes, v_xy, v_xy_abs, v_pix_vels, v_conic, v_colors, v_opacity, stream);
+}
+
+static int check_views_bwd(int num_views, unsigned img_height, unsigned img_width, unsigned block_width,
+                           const int32_t *tile_order) {
+    B200_REQUIRE(num_views >= 1, "num_views must be >= 1");
+    B200_REQUIRE(tile_order, "null per-view array");
+    B200_REQUIRE(block_width > 1 && block_width <= 16, "block_width must be between 2 and 16");
+    const long long tiles = (long long)((img_width + block_width - 1) / block_width) * ((img_height + block_width - 1) / block_width);
+    B200_REQUIRE((long long)num_views * tiles < 0x7fffffffll && (long long)num_views * img_height < 0x7fffffffll,
+                 "num_views * tiles exceeds int32");
+    return B200_OK;
+}
+
+extern "C" int b200_blend_backward_views(int num_views, int num_records, unsigned img_height, unsigned img_width,
+                                         unsigned block_width, unsigned n_blur_samples, const int32_t *gaussian_ids_sorted,
+                                         const int32_t *tile_bins, const void *packed, float rolling_shutter_time,
+                                         float exposure_time, const float *background, const float *final_Ts,
+                                         const int32_t *final_idx, const float *v_output, const float *v_output_alpha,
+                                         const int32_t *tile_order, float *v_xy, float *v_xy_abs, float *v_pix_vels,
+                                         float *v_conic, float *v_colors, float *v_opacity, int outputs_are_zero,
+                                         void *stream) {
+    int rc = check_views_bwd(num_views, img_height, img_width, block_width, tile_order);
+    if (rc) return rc;
+    return run_blend_backward(num_records, img_height, img_width, block_width, n_blur_samples, gaussian_ids_sorted,
+                              tile_bins, packed, rolling_shutter_time, exposure_time, background, final_Ts, final_idx,
+                              v_output, v_output_alpha, v_xy, v_xy_abs, v_pix_vels, v_conic, v_colors, v_opacity,
+                              outputs_are_zero != 0, as_stream(stream), tile_order, nullptr, num_views);
+}
+
+extern "C" int b200_blend_backward_views_deterministic(int num_views, int num_records, int num_entries,
+                                                       unsigned img_height, unsigned img_width, unsigned block_width,
+                                                       unsigned n_blur_samples, const int32_t *gaussian_ids_sorted,
+                                                       const int32_t *tile_bins, const void *packed,
+                                                       float rolling_shutter_time, float exposure_time,
+                                                       const float *background, const float *final_Ts,
+                                                       const int32_t *final_idx, const float *v_output,
+                                                       const float *v_output_alpha, const int32_t *tile_order, void *ws,
+                                                       size_t ws_bytes, float *v_xy, float *v_xy_abs, float *v_pix_vels,
+                                                       float *v_conic, float *v_colors, float *v_opacity, void *stream) {
+    int rc = check_views_bwd(num_views, img_height, img_width, block_width, tile_order);
+    if (rc) return rc;
+    return run_blend_backward_deterministic(num_views, num_records, num_entries, img_height, img_width, block_width,
+                                            n_blur_samples, gaussian_ids_sorted, tile_bins, packed, rolling_shutter_time,
+                                            exposure_time, background, final_Ts, final_idx, v_output, v_output_alpha,
+                                            nullptr, tile_order, ws, ws_bytes, v_xy, v_xy_abs, v_pix_vels, v_conic,
+                                            v_colors, v_opacity, stream);
 }
 
 extern "C" int b200_rasterize_backward(int num_points, unsigned img_height, unsigned img_width, unsigned block_width,

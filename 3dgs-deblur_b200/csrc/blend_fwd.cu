@@ -28,14 +28,25 @@ struct BlendFwdParams {
     float *final_Ts;          // (H,W,S)
     float *out_alpha;         // (H,W) or null: 1 - mean_s final_T, what rasterize.py:161-163 derives with two torch ops
     int32_t *final_idx;       // (H,W,S)
-    const int32_t *ref_isect;  // DEVICE int32 or null: the reference's num_intersects of this image, when the host never
-                               // learned it (capacity-mode binning); < 1 selects the reference's empty-render branch
+    const int32_t *ref_isect;  // DEVICE int32[views] or null: the reference's num_intersects of each image, when the host
+                               // never learned it (capacity-mode binning, view batches); < 1 selects the reference's
+                               // empty-render branch for that image
+    int views;                 // images blended by one launch: tile t of image v is tile v * tbx * tby + t of the lists,
+                               // its pixels are rows v * H .. v * H + H - 1 of the (views * H, W) outputs
 };
+
+// CTA -> (image, tile within the image)
+__device__ __forceinline__ void cta_tile(const int32_t *tile_order, const BlendGeom &g, int &view, int &tile) {
+    const int t = tile_order ? __ldg(tile_order + blockIdx.x) : (int)blockIdx.x;
+    const int per_view = g.tbx * g.tby;
+    view = t / per_view;
+    tile = t - view * per_view;
+}
 
 // What the reference returns when nothing intersects a tile (rasterize.py:136-144): the background colour and all-zero
 // final_Ts / final_idx, hence alpha = 1.  Only reachable in the capacity mode, where the count lives on the device.
 template <int S>
-__device__ __forceinline__ void write_empty_render(const BlendFwdParams &p, bool inside, int i, int j) {
+__device__ __forceinline__ void write_empty_render(const BlendFwdParams &p, bool inside, int i, int j) {  // i: row of all views
     if (!inside) return;
     const size_t pix = (size_t)i * p.g.W + j;
 #pragma unroll
@@ -52,7 +63,8 @@ __global__ void __launch_bounds__(BLEND_THREADS, 1) blend_forward_kernel(const B
     __shared__ __align__(8) uint64_t s_bar[BLEND_STAGES];
 
     const int tid = threadIdx.x, lane = tid & 31;
-    const int tile = p.tile_order ? __ldg(p.tile_order + blockIdx.x) : (int)blockIdx.x;
+    int view, tile;
+    cta_tile(p.tile_order, p.g, view, tile);
     const int tile_x = tile % p.g.tbx, tile_y = tile / p.g.tbx;
     int lx, ly;
     bool has_pixel;
@@ -61,8 +73,8 @@ __global__ void __launch_bounds__(BLEND_THREADS, 1) blend_forward_kernel(const B
     const bool inside = has_pixel && pi < p.g.H && pj < p.g.W;
     const float px = (float)pj + 0.5f, py = (float)pi + 0.5f;
     const float roll = (float)((double)p.g.rs_time * ((double)(py / (float)p.g.H) - 0.5));  // forward.cu:360
-    if (p.ref_isect && __ldg(p.ref_isect) < 1) {  // block-uniform
-        write_empty_render<S>(p, inside, pi, pj);
+    if (p.ref_isect && __ldg(p.ref_isect + view) < 1) {  // block-uniform
+        write_empty_render<S>(p, inside, view * p.g.H + pi, pj);
         return;
     }
     float blur[S];  // blur_rel of forward.cu:363 without the roll part; tau = blur[s] + roll
@@ -71,7 +83,7 @@ __global__ void __launch_bounds__(BLEND_THREADS, 1) blend_forward_kernel(const B
 
     const WarpWindow win = warp_window<1>({inside}, {px}, {py}, {roll});
 
-    const int2 range = p.tile_bins[tile];
+    const int2 range = p.tile_bins[view * (p.g.tbx * p.g.tby) + tile];
     const int total = range.y - range.x;
     const int nb = (total + BLEND_BATCH - 1) / BLEND_BATCH;
 
@@ -162,7 +174,7 @@ __global__ void __launch_bounds__(BLEND_THREADS, 1) blend_forward_kernel(const B
 
     const float bg0 = __ldg(p.background), bg1 = __ldg(p.background + 1), bg2 = __ldg(p.background + 2);
     if (!inside) return;
-    const size_t pix = (size_t)pi * p.g.W + pj;
+    const size_t pix = (size_t)(view * p.g.H + pi) * p.g.W + pj;
     float meanT = 0.f, sumT = 0.f;
 #pragma unroll
     for (int s = 0; s < S; ++s) {
@@ -193,7 +205,8 @@ __global__ void __launch_bounds__(128, FWD_MIN_CTAS) blend_forward_kernel2(const
     __shared__ __align__(8) uint64_t s_bar[BLEND_STAGES];
 
     const int tid = threadIdx.x, lane = tid & 31;
-    const int tile = p.tile_order ? __ldg(p.tile_order + blockIdx.x) : (int)blockIdx.x;
+    int view, tile;
+    cta_tile(p.tile_order, p.g, view, tile);
     const int tile_x = tile % p.g.tbx, tile_y = tile / p.g.tbx;
     bool inside[2];
     float px[2], py[2], roll[2];
@@ -206,8 +219,9 @@ __global__ void __launch_bounds__(128, FWD_MIN_CTAS) blend_forward_kernel2(const
         inside[q] = pi[q] < p.g.H && pj[q] < p.g.W;
         px[q] = (float)pj[q] + 0.5f; py[q] = (float)pi[q] + 0.5f;
         roll[q] = (float)((double)p.g.rs_time * ((double)(py[q] / (float)p.g.H) - 0.5));  // forward.cu:360
+        pi[q] += view * p.g.H;  // from here on: the row in the (views * H, W) outputs
     }
-    if (p.ref_isect && __ldg(p.ref_isect) < 1) {  // block-uniform
+    if (p.ref_isect && __ldg(p.ref_isect + view) < 1) {  // block-uniform
 #pragma unroll
         for (int q = 0; q < 2; ++q) write_empty_render<S>(p, inside[q], pi[q], pj[q]);
         return;
@@ -218,7 +232,7 @@ __global__ void __launch_bounds__(128, FWD_MIN_CTAS) blend_forward_kernel2(const
     const WarpWindow win = warp_window<2>(inside, px, py, roll);
     const f2 PX = f2_make(px[0], px[1]), PY = f2_make(py[0], py[1]), ROLL = f2_make(roll[0], roll[1]);
 
-    const int2 range = p.tile_bins[tile];
+    const int2 range = p.tile_bins[view * (p.g.tbx * p.g.tby) + tile];
     const int total = range.y - range.x;
     const int nb = (total + BLEND_BATCH - 1) / BLEND_BATCH;
 
@@ -360,10 +374,11 @@ __global__ void __launch_bounds__(128, FWD_MIN_CTAS) blend_forward_kernel2(const
 template <int S>
 static int launch_fwd(const BlendFwdParams &p, cudaStream_t st) {
     // two pixels per lane when the tile is the full 16x16 (the only size Splatfacto uses, splatfacto.py:815)
+    const int ctas = p.views * p.g.tbx * p.g.tby;
     if (p.g.bw == 16 && !blend_force_one_pixel(false))
-        blend_forward_kernel2<S><<<p.g.tbx * p.g.tby, BLEND_THREADS / 2, 0, st>>>(p);
+        blend_forward_kernel2<S><<<ctas, BLEND_THREADS / 2, 0, st>>>(p);
     else
-        blend_forward_kernel<S><<<p.g.tbx * p.g.tby, BLEND_THREADS, 0, st>>>(p);
+        blend_forward_kernel<S><<<ctas, BLEND_THREADS, 0, st>>>(p);
     B200_LAUNCH_CHECK();
     return B200_OK;
 }
@@ -436,7 +451,7 @@ static int run_blend_forward(unsigned img_height, unsigned img_width, unsigned b
                              const int32_t *gaussian_ids_sorted, const int32_t *tile_bins, const void *packed,
                              float rolling_shutter_time, float exposure_time, const float *background, float *out_img,
                              float *final_Ts, int32_t *final_idx, float *out_alpha, cudaStream_t st,
-                             const int32_t *ref_isect = nullptr, const int32_t *tile_order = nullptr) {
+                             const int32_t *ref_isect = nullptr, const int32_t *tile_order = nullptr, int views = 1) {
     B200_REQUIRE(n_blur_samples > 0 && n_blur_samples <= B200_MAX_BLUR_SAMPLES, "unsupported blur size");  // bindings.cu:450-452
     B200_REQUIRE(block_width > 1 && block_width <= 16, "block_width must be between 2 and 16");
     B200_REQUIRE(img_height > 0 && img_width > 0, "image size must be positive");
@@ -452,6 +467,7 @@ static int run_blend_forward(unsigned img_height, unsigned img_width, unsigned b
     p.background = background;
     p.out_img = out_img; p.final_Ts = final_Ts; p.final_idx = final_idx; p.out_alpha = out_alpha;
     p.ref_isect = ref_isect;
+    p.views = views;
     return with_blur_samples(n_blur_samples, [&](auto s) { return launch_fwd<decltype(s)::value>(p, st); });
 }
 
@@ -510,6 +526,25 @@ extern "C" int b200_blend_forward_packed_status(unsigned img_height, unsigned im
 
 // b200_blend_forward_packed / _status with the CTAs launched in `tile_order` (b200_blend_tile_order of the same
 // tile_bins); `status` may be null.  The order changes no output bit: every tile is blended on its own.
+// num_views images at once (lists of b200_bin_cull_emit_views); view_isect: DEVICE int32[num_views] from
+// b200_bin_cull_count_views, < 1 takes the empty-render branch for that view.
+extern "C" int b200_blend_forward_views(int num_views, unsigned img_height, unsigned img_width, unsigned block_width,
+                                        unsigned n_blur_samples, const int32_t *gaussian_ids_sorted,
+                                        const int32_t *tile_bins, const void *packed, float rolling_shutter_time,
+                                        float exposure_time, const float *background, const int32_t *view_isect,
+                                        const int32_t *tile_order, float *out_img, float *final_Ts, int32_t *final_idx,
+                                        float *out_alpha, void *stream) {
+    B200_REQUIRE(num_views >= 1, "num_views must be >= 1");
+    B200_REQUIRE(view_isect && tile_order, "null per-view array");
+    B200_REQUIRE(block_width > 1 && block_width <= 16, "block_width must be between 2 and 16");
+    const long long tiles = (long long)((img_width + block_width - 1) / block_width) * ((img_height + block_width - 1) / block_width);
+    B200_REQUIRE((long long)num_views * tiles < 0x7fffffffll && (long long)num_views * img_height < 0x7fffffffll,
+                 "num_views * tiles exceeds int32");
+    return run_blend_forward(img_height, img_width, block_width, n_blur_samples, gaussian_ids_sorted, tile_bins, packed,
+                             rolling_shutter_time, exposure_time, background, out_img, final_Ts, final_idx, out_alpha,
+                             as_stream(stream), view_isect, tile_order, num_views);
+}
+
 extern "C" int b200_blend_forward_packed_ordered(unsigned img_height, unsigned img_width, unsigned block_width,
                                                  unsigned n_blur_samples, const int32_t *gaussian_ids_sorted,
                                                  const int32_t *tile_bins, const void *packed, float rolling_shutter_time,

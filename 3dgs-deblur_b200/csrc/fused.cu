@@ -23,7 +23,23 @@ struct FusedParams {
     const float *log_scales, *quats_raw, *opacity_logit, *sh_dc, *sh_rest, *cam_pos;
     int K, deg_use;
     bool quats_al;          // quats_raw is 16-byte aligned (vector loads); otherwise scalar loads
+    // View batch: camera v's viewmat (12 floats), cam_pos, velocities (3 each) sit at v times their size past the
+    // pointers above, and intr (when not null) holds fx, fy, cx, cy of every view; Gaussian g of view v is record v * n + g.
+    int views;
+    const float *intr;
 };
+
+// The camera of view v in f (v = 0 and no intr: f itself)
+__device__ __forceinline__ void select_view(FusedParams &f, int v) {
+    f.proj.viewmat += 12 * (size_t)v;
+    if (f.cam_pos) f.cam_pos += 3 * (size_t)v;
+    if (f.proj.lin_vel) f.proj.lin_vel += 3 * (size_t)v;
+    if (f.proj.ang_vel) f.proj.ang_vel += 3 * (size_t)v;
+    if (f.intr) {
+        const float4 k = __ldg(reinterpret_cast<const float4 *>(f.intr) + v);
+        f.proj.fx = k.x; f.proj.fy = k.y; f.proj.cx = k.z; f.proj.cy = k.w;
+    }
+}
 
 __device__ __forceinline__ float4 load_quat(const FusedParams &f, int i) {
     if (f.quats_al) return reinterpret_cast<const float4 *>(f.quats_raw)[i];
@@ -57,6 +73,7 @@ __device__ __forceinline__ void sh_colour(const FusedParams &f, int i, const flo
 
 // DEG_USE < 0: geometry only -- the record's colour is left 0 for fused_colors_kernel to fill in later (a trainer that
 // projects and bins the next image while the SH block of the previous step is still being exchanged / updated).
+// Grid (ceil(n / FUSED_THREADS), views): blockIdx.y is the view.
 template <int DEG_USE>
 __global__ void __launch_bounds__(FUSED_THREADS) fused_forward_kernel(FusedParams f, PackedGaussian *__restrict__ rec,
                                                                       float *__restrict__ depths,
@@ -65,24 +82,27 @@ __global__ void __launch_bounds__(FUSED_THREADS) fused_forward_kernel(FusedParam
     constexpr int KU = DEG_USE < 0 ? 1 : (DEG_USE + 1) * (DEG_USE + 1);
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= f.proj.n) return;
+    const int v = blockIdx.y;
+    select_view(f, v);
+    const int ri = v * f.proj.n + i;  // record index (< 2^31: checked by the entry point)
     const float *m = f.proj.means + 3 * (size_t)i, *ls = f.log_scales + 3 * (size_t)i;
     const float4 q = load_quat(f, i);
     const float qn = 1.f / sqrtf(q.x * q.x + q.y * q.y + q.z * q.z + q.w * q.w);
     ProjGaussIn in{m[0], m[1], m[2], expf(ls[0]), expf(ls[1]), expf(ls[2]), q.x * qn, q.y * qn, q.z * qn, q.w * qn};
     ProjGaussOut r;
     project_forward_one(f.proj, in, r);
-    depths[i] = r.depth; radii[i] = r.radius_i; tiles_hit[i] = r.tiles;
+    depths[ri] = r.depth; radii[ri] = r.radius_i; tiles_hit[ri] = r.tiles;
     PackedGaussian g;
     if (r.tiles > 0) {
         float c0 = -0.5f, c1 = -0.5f, c2 = -0.5f;
         if constexpr (DEG_USE >= 0) sh_colour<DEG_USE>(f, i, m, c0, c1, c2);
         const float opac = sigmoidf_(f.opacity_logit[i]) * r.comp;  // splatfacto.py:853-854 ("antialiased")
-        g = make_record(i, r.xy[0], r.xy[1], r.vel[0], r.vel[1], r.conic[0], r.conic[1], r.conic[2], opac,
+        g = make_record(ri, r.xy[0], r.xy[1], r.vel[0], r.vel[1], r.conic[0], r.conic[1], r.conic[2], opac,
                         clamp_colour(c0 + 0.5f), clamp_colour(c1 + 0.5f), clamp_colour(c2 + 0.5f));  // :846
     } else {
-        g = make_record(i, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f);  // hx = -1: never blended
+        g = make_record(ri, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f);  // hx = -1: never blended
     }
-    store_record(rec + i, g);
+    store_record(rec + ri, g);
 }
 
 // The colour half of fused_forward_kernel for records built geometry-only: clamp(SH colour + 0.5, 0) of every Gaussian
@@ -116,80 +136,130 @@ __device__ __forceinline__ void store_rows(float *dst, const float *s, int row, 
     }
 }
 
-// DET: the camera partials of the block are stored to io.cam_partials instead of added to the outputs (deterministic mode)
-template <int DEG_USE, bool DET>
-__global__ void __launch_bounds__(FUSED_THREADS) fused_backward_kernel(FusedParams f, FusedBwdIO io) {
+// a = x for the first view, a + x (rounded on its own: never contracted into an FMA) for the others -- the sum over
+// views in view order, bit for bit what adding the single-view gradients one after the other gives
+__device__ __forceinline__ void add_view(float &a, float x, bool first) { a = first ? x : __fadd_rn(a, x); }
+
+// One thread per Gaussian; views in order (f.views, record v * n + g of view v).  Every view's VJP is the single-view
+// one, the raw-parameter gradients are summed over the views in registers (the sh_rest rows in shared memory) and each
+// row is written once.  The camera gradients are per view: io.g_lin / g_ang / g_viewmat + 3 v / 3 v / 12 v.
+// DET: the camera partials of the block are stored to io.cam_partials (18 floats per (view, block)) instead of added to
+// the outputs (deterministic mode).  VIEWS = false: one view (f0.views == 1), the loop and the view sums compile away.
+template <int DEG_USE, bool DET, bool VIEWS>
+__global__ void __launch_bounds__(FUSED_THREADS) fused_backward_kernel(const FusedParams f0, FusedBwdIO io) {
     constexpr int KU = (DEG_USE + 1) * (DEG_USE + 1);
     extern __shared__ __align__(16) float s_rows[];  // [FUSED_THREADS][pitch] gradient rows of sh_rest
     __shared__ float s_red[FUSED_THREADS / 32][18];
-    const int rest_row = 3 * (f.K - 1);
+    const int rest_row = 3 * (f0.K - 1);
     const int pitch = (rest_row & 1) ? rest_row : rest_row + 1;
     const int t = threadIdx.x;
     const int base = blockIdx.x * FUSED_THREADS;
-    const int count = min(FUSED_THREADS, f.proj.n - base);
+    const int count = min(FUSED_THREADS, f0.proj.n - base);
     const int i = base + t;
     const bool want_cam = io.g_lin || io.g_ang || io.g_viewmat;
 
-    ProjGaussGrad gr;
-#pragma unroll
-    for (int k = 0; k < 18; ++k) gr.red[k] = 0.f;
-#pragma unroll
-    for (int k = 0; k < 6; ++k) gr.v_c3[k] = 0.f;
-    gr.v_mean[0] = gr.v_mean[1] = gr.v_mean[2] = 0.f; gr.v_scale[0] = gr.v_scale[1] = gr.v_scale[2] = 0.f;
-    gr.v_quat[0] = gr.v_quat[1] = gr.v_quat[2] = gr.v_quat[3] = 0.f; gr.vc2[0] = gr.vc2[1] = gr.vc2[2] = 0.f;
-    float g_ls[3] = {0.f, 0.f, 0.f}, g_q[4] = {0.f, 0.f, 0.f, 0.f}, g_op = 0.f, g_dc[3] = {0.f, 0.f, 0.f};
+    float g_mean[3] = {0.f, 0.f, 0.f}, g_ls[3] = {0.f, 0.f, 0.f}, g_q[4] = {0.f, 0.f, 0.f, 0.f}, g_op = 0.f,
+          g_dc[3] = {0.f, 0.f, 0.f};
     float *my_rows = s_rows + t * pitch;
-    bool active = false;
-    if (t < count) {
-        active = io.radii[i] > 0;
-        if (!active)
-            for (int k = 0; k < rest_row; ++k) my_rows[k] = 0.f;
-    }
-    if (active) {
-        const float *m = f.proj.means + 3 * (size_t)i, *ls = f.log_scales + 3 * (size_t)i;
-        const float4 q = load_quat(f, i);
-        const float qn = 1.f / sqrtf(q.x * q.x + q.y * q.y + q.z * q.z + q.w * q.w);
-        ProjGaussIn in{m[0], m[1], m[2], expf(ls[0]), expf(ls[1]), expf(ls[2]), q.x * qn, q.y * qn, q.z * qn, q.w * qn};
-        ProjGaussOut r;
-        project_forward_one(f.proj, in, r);  // recompute instead of saving 40 B per Gaussian
-        const float4 C = *reinterpret_cast<const float4 *>(&io.rec[i].r);  // clamped colour of the forward
-        // colour: clamp gate (see clamp_colour), then basis outer product (sh.cuh:467-498)
-        const float v0 = !signbit(C.x) ? io.v_colors[3 * (size_t)i] : 0.f,
-                    v1 = !signbit(C.y) ? io.v_colors[3 * (size_t)i + 1] : 0.f,
-                    v2 = !signbit(C.z) ? io.v_colors[3 * (size_t)i + 2] : 0.f;
-        float B[KU];
-        sh_basis<B200_SH_FAST>(DEG_USE, m[0] - __ldg(f.cam_pos), m[1] - __ldg(f.cam_pos + 1), m[2] - __ldg(f.cam_pos + 2), B);
-        g_dc[0] = B[0] * v0; g_dc[1] = B[0] * v1; g_dc[2] = B[0] * v2;
+    const int views = VIEWS ? f0.views : 1;
+    for (int v = 0; v < views; ++v) {
+        FusedParams f = f0;
+        if (VIEWS) select_view(f, v);
+        const bool first = !VIEWS || v == 0;
+        const size_t ri = (size_t)v * f0.proj.n + i;  // record of Gaussian i in view v
+        ProjGaussGrad gr;
 #pragma unroll
-        for (int k = 1; k < KU; ++k) {
-            my_rows[3 * (k - 1)] = B[k] * v0; my_rows[3 * (k - 1) + 1] = B[k] * v1; my_rows[3 * (k - 1) + 2] = B[k] * v2;
+        for (int k = 0; k < 18; ++k) gr.red[k] = 0.f;
+#pragma unroll
+        for (int k = 0; k < 6; ++k) gr.v_c3[k] = 0.f;
+        gr.v_mean[0] = gr.v_mean[1] = gr.v_mean[2] = 0.f; gr.v_scale[0] = gr.v_scale[1] = gr.v_scale[2] = 0.f;
+        gr.v_quat[0] = gr.v_quat[1] = gr.v_quat[2] = gr.v_quat[3] = 0.f; gr.vc2[0] = gr.vc2[1] = gr.vc2[2] = 0.f;
+        float l_ls[3] = {0.f, 0.f, 0.f}, l_q[4] = {0.f, 0.f, 0.f, 0.f}, l_op = 0.f, l_dc[3] = {0.f, 0.f, 0.f};
+        bool active = false;
+        if (t < count) {
+            active = io.radii[ri] > 0;
+            if (!active)
+                for (int k = 0; k < rest_row; ++k) add_view(my_rows[k], 0.f, first);
         }
-        for (int k = 3 * (KU - 1); k < rest_row; ++k) my_rows[k] = 0.f;
-        // opacity = sigmoid(logit) * comp
-        const float sg = sigmoidf_(f.opacity_logit[i]);
-        const float vo = io.v_opacity[i];
-        g_op = vo * r.comp * sg * (1.f - sg);
-        // projection VJP
-        ProjGaussSaved sv;
+        if (active) {
+            const float *m = f.proj.means + 3 * (size_t)i, *ls = f.log_scales + 3 * (size_t)i;
+            const float4 q = load_quat(f, i);
+            const float qn = 1.f / sqrtf(q.x * q.x + q.y * q.y + q.z * q.z + q.w * q.w);
+            ProjGaussIn in{m[0], m[1], m[2], expf(ls[0]), expf(ls[1]), expf(ls[2]), q.x * qn, q.y * qn, q.z * qn, q.w * qn};
+            ProjGaussOut r;
+            project_forward_one(f.proj, in, r);  // recompute instead of saving 40 B per Gaussian
+            const float4 C = *reinterpret_cast<const float4 *>(&io.rec[ri].r);  // clamped colour of the forward
+            // colour: clamp gate (see clamp_colour), then basis outer product (sh.cuh:467-498)
+            const float v0 = !signbit(C.x) ? io.v_colors[3 * ri] : 0.f,
+                        v1 = !signbit(C.y) ? io.v_colors[3 * ri + 1] : 0.f,
+                        v2 = !signbit(C.z) ? io.v_colors[3 * ri + 2] : 0.f;
+            float B[KU];
+            sh_basis<B200_SH_FAST>(DEG_USE, m[0] - __ldg(f.cam_pos), m[1] - __ldg(f.cam_pos + 1), m[2] - __ldg(f.cam_pos + 2), B);
+            l_dc[0] = B[0] * v0; l_dc[1] = B[0] * v1; l_dc[2] = B[0] * v2;
 #pragma unroll
-        for (int k = 0; k < 6; ++k) sv.cov3d[k] = r.cov3d[k];
-        sv.conic[0] = r.conic[0]; sv.conic[1] = r.conic[1]; sv.conic[2] = r.conic[2];
-        sv.comp = r.comp;
-        ProjGaussCot ct;
-        const float2 gxy = reinterpret_cast<const float2 *>(io.v_xy)[i], gpv = reinterpret_cast<const float2 *>(io.v_pix_vel)[i];
-        ct.v_xy[0] = gxy.x; ct.v_xy[1] = gxy.y; ct.v_pix_vel[0] = gpv.x; ct.v_pix_vel[1] = gpv.y;
-        ct.v_depth = 0.f;
-        ct.v_conic[0] = io.v_conic[3 * (size_t)i]; ct.v_conic[1] = io.v_conic[3 * (size_t)i + 1]; ct.v_conic[2] = io.v_conic[3 * (size_t)i + 2];
-        ct.v_comp = vo * sg;
-        project_backward_one<true>(f.proj, want_cam, io.g_viewmat != nullptr, in, sv, ct, gr);
-        // exp and normalisation chains
-        g_ls[0] = gr.v_scale[0] * in.s0; g_ls[1] = gr.v_scale[1] * in.s1; g_ls[2] = gr.v_scale[2] * in.s2;
-        const float dotq = in.qw * gr.v_quat[0] + in.qx * gr.v_quat[1] + in.qy * gr.v_quat[2] + in.qz * gr.v_quat[3];
-        g_q[0] = (gr.v_quat[0] - in.qw * dotq) * qn; g_q[1] = (gr.v_quat[1] - in.qx * dotq) * qn;
-        g_q[2] = (gr.v_quat[2] - in.qy * dotq) * qn; g_q[3] = (gr.v_quat[3] - in.qz * dotq) * qn;
+            for (int k = 1; k < KU; ++k) {
+                add_view(my_rows[3 * (k - 1)], B[k] * v0, first);
+                add_view(my_rows[3 * (k - 1) + 1], B[k] * v1, first);
+                add_view(my_rows[3 * (k - 1) + 2], B[k] * v2, first);
+            }
+            for (int k = 3 * (KU - 1); k < rest_row; ++k) add_view(my_rows[k], 0.f, first);
+            // opacity = sigmoid(logit) * comp
+            const float sg = sigmoidf_(f.opacity_logit[i]);
+            const float vo = io.v_opacity[ri];
+            l_op = vo * r.comp * sg * (1.f - sg);
+            // projection VJP
+            ProjGaussSaved sv;
+#pragma unroll
+            for (int k = 0; k < 6; ++k) sv.cov3d[k] = r.cov3d[k];
+            sv.conic[0] = r.conic[0]; sv.conic[1] = r.conic[1]; sv.conic[2] = r.conic[2];
+            sv.comp = r.comp;
+            ProjGaussCot ct;
+            const float2 gxy = reinterpret_cast<const float2 *>(io.v_xy)[ri], gpv = reinterpret_cast<const float2 *>(io.v_pix_vel)[ri];
+            ct.v_xy[0] = gxy.x; ct.v_xy[1] = gxy.y; ct.v_pix_vel[0] = gpv.x; ct.v_pix_vel[1] = gpv.y;
+            ct.v_depth = 0.f;
+            ct.v_conic[0] = io.v_conic[3 * ri]; ct.v_conic[1] = io.v_conic[3 * ri + 1]; ct.v_conic[2] = io.v_conic[3 * ri + 2];
+            ct.v_comp = vo * sg;
+            project_backward_one<true>(f.proj, want_cam, io.g_viewmat != nullptr, in, sv, ct, gr);
+            // exp and normalisation chains
+            l_ls[0] = gr.v_scale[0] * in.s0; l_ls[1] = gr.v_scale[1] * in.s1; l_ls[2] = gr.v_scale[2] * in.s2;
+            const float dotq = in.qw * gr.v_quat[0] + in.qx * gr.v_quat[1] + in.qy * gr.v_quat[2] + in.qz * gr.v_quat[3];
+            l_q[0] = (gr.v_quat[0] - in.qw * dotq) * qn; l_q[1] = (gr.v_quat[1] - in.qx * dotq) * qn;
+            l_q[2] = (gr.v_quat[2] - in.qy * dotq) * qn; l_q[3] = (gr.v_quat[3] - in.qz * dotq) * qn;
+        }
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+            add_view(g_mean[k], gr.v_mean[k], first); add_view(g_ls[k], l_ls[k], first); add_view(g_dc[k], l_dc[k], first);
+        }
+#pragma unroll
+        for (int k = 0; k < 4; ++k) add_view(g_q[k], l_q[k], first);
+        add_view(g_op, l_op, first);
+
+        if (want_cam) {
+            const int lane = t & 31, warp = t >> 5;
+#pragma unroll
+            for (int k = 0; k < 18; ++k) {
+                const float s = warp_sum(gr.red[k]);
+                if (lane == 0) s_red[warp][k] = s;
+            }
+            __syncthreads();
+            if (t < 18) {
+                float s = 0.f;
+#pragma unroll
+                for (int w = 0; w < FUSED_THREADS / 32; ++w) s += s_red[w][t];
+                if constexpr (DET) {
+                    io.cam_partials[18 * ((size_t)v * gridDim.x + blockIdx.x) + t] = s;
+                } else {
+                    float *dst = t < 3 ? (io.g_lin ? io.g_lin + 3 * (size_t)v + t : nullptr)
+                               : t < 6 ? (io.g_ang ? io.g_ang + 3 * (size_t)v + (t - 3) : nullptr)
+                                       : (io.g_viewmat ? io.g_viewmat + 12 * (size_t)v + (t - 6) : nullptr);
+                    if (dst && s != 0.f) atomicAdd(dst, s);
+                }
+            }
+            __syncthreads();  // s_red is refilled by the next view
+        }
     }
     if (t < count) {
-        io.g_means[3 * (size_t)i] = gr.v_mean[0]; io.g_means[3 * (size_t)i + 1] = gr.v_mean[1]; io.g_means[3 * (size_t)i + 2] = gr.v_mean[2];
+        io.g_means[3 * (size_t)i] = g_mean[0]; io.g_means[3 * (size_t)i + 1] = g_mean[1]; io.g_means[3 * (size_t)i + 2] = g_mean[2];
         io.g_log_scales[3 * (size_t)i] = g_ls[0]; io.g_log_scales[3 * (size_t)i + 1] = g_ls[1]; io.g_log_scales[3 * (size_t)i + 2] = g_ls[2];
         if (io.gq_al) {
             reinterpret_cast<float4 *>(io.g_quats)[i] = make_float4(g_q[0], g_q[1], g_q[2], g_q[3]);
@@ -202,29 +272,6 @@ __global__ void __launch_bounds__(FUSED_THREADS) fused_backward_kernel(FusedPara
     }
     __syncthreads();
     store_rows(io.g_sh_rest + (size_t)base * rest_row, s_rows, rest_row, pitch, count);
-
-    if (want_cam) {
-        const int lane = t & 31, warp = t >> 5;
-#pragma unroll
-        for (int k = 0; k < 18; ++k) {
-            const float s = warp_sum(gr.red[k]);
-            if (lane == 0) s_red[warp][k] = s;
-        }
-        __syncthreads();
-        if (t < 18) {
-            float s = 0.f;
-#pragma unroll
-            for (int w = 0; w < FUSED_THREADS / 32; ++w) s += s_red[w][t];
-            if constexpr (DET) {
-                io.cam_partials[18 * (size_t)blockIdx.x + t] = s;
-            } else {
-                float *dst = t < 3 ? (io.g_lin ? io.g_lin + t : nullptr)
-                           : t < 6 ? (io.g_ang ? io.g_ang + (t - 3) : nullptr)
-                                   : (io.g_viewmat ? io.g_viewmat + (t - 6) : nullptr);
-                if (dst && s != 0.f) atomicAdd(dst, s);
-            }
-        }
-    }
 }
 
 static int fill_fused(FusedParams &f, int n, const float *means, const float *log_scales, const float *quats,
@@ -245,12 +292,43 @@ static int fill_fused(FusedParams &f, int n, const float *means, const float *lo
     f.proj = ProjCommon{n, means, nullptr, nullptr, lin_vel, ang_vel, viewmat, 1.0f, rs, exposure, fx, fy, cx, cy, (int)H, (int)W, (int)bw, clip};
     f.log_scales = log_scales; f.quats_raw = quats; f.opacity_logit = opacity_logit; f.sh_dc = sh_dc; f.sh_rest = sh_rest;
     f.cam_pos = cam_pos; f.K = sh_bases; f.deg_use = degrees_to_use; f.quats_al = aligned16(quats);
+    f.views = 1; f.intr = nullptr;
+    return B200_OK;
+}
+
+// The view-batched entry points: B >= 1 views, every per-view array present, B * N records addressable with int32
+// (record ids and list entries are int32), and B within the grid's y extent.
+static int check_views(int views, int n, const float *viewmats, const float *cam_pos, const float *lin_vel,
+                       const float *ang_vel, const float *intr) {
+    B200_REQUIRE(views >= 1, "num_views must be >= 1");
+    B200_REQUIRE(views <= 65535, "num_views must be <= 65535");
+    B200_REQUIRE(n >= 1, "num_points must be >= 1");
+    B200_REQUIRE((long long)views * n <= 0x7fffffffll, "num_views * num_points exceeds int32");
+    B200_REQUIRE(viewmats && cam_pos && lin_vel && ang_vel && intr, "null per-view array");
+    B200_REQUIRE(aligned16(intr), "intrinsics must be 16-byte aligned");
     return B200_OK;
 }
 
 }  // namespace b200
 
 using namespace b200;
+
+static int launch_fused_forward(const FusedParams &f, void *packed, float *depths, int32_t *radii, int32_t *num_tiles_hit,
+                                void *stream) {
+    B200_REQUIRE(packed && aligned16(packed) && depths && radii && num_tiles_hit, "null / misaligned output pointer");
+    const dim3 grid(ceil_div(f.proj.n, FUSED_THREADS), f.views);
+    cudaStream_t st = as_stream(stream);
+    PackedGaussian *rec = reinterpret_cast<PackedGaussian *>(packed);
+    switch (f.deg_use) {
+        case 0: fused_forward_kernel<0><<<grid, FUSED_THREADS, 0, st>>>(f, rec, depths, radii, num_tiles_hit); break;
+        case 1: fused_forward_kernel<1><<<grid, FUSED_THREADS, 0, st>>>(f, rec, depths, radii, num_tiles_hit); break;
+        case 2: fused_forward_kernel<2><<<grid, FUSED_THREADS, 0, st>>>(f, rec, depths, radii, num_tiles_hit); break;
+        case 3: fused_forward_kernel<3><<<grid, FUSED_THREADS, 0, st>>>(f, rec, depths, radii, num_tiles_hit); break;
+        default: fused_forward_kernel<4><<<grid, FUSED_THREADS, 0, st>>>(f, rec, depths, radii, num_tiles_hit); break;
+    }
+    B200_LAUNCH_CHECK();
+    return B200_OK;
+}
 
 extern "C" int b200_fused_preprocess_forward(int num_points, const float *means, const float *log_scales,
                                              const float *quats, const float *opacity_logit, const float *sh_dc,
@@ -265,19 +343,27 @@ extern "C" int b200_fused_preprocess_forward(int num_points, const float *means,
                         viewmat, cam_pos, lin_vel, ang_vel, rolling_shutter_time, exposure_time, fx, fy, cx, cy, img_height,
                         img_width, block_width, clip_thresh);
     if (rc) return rc;
-    B200_REQUIRE(packed && aligned16(packed) && depths && radii && num_tiles_hit, "null / misaligned output pointer");
-    const int blocks = ceil_div(num_points, FUSED_THREADS);
-    cudaStream_t st = as_stream(stream);
-    PackedGaussian *rec = reinterpret_cast<PackedGaussian *>(packed);
-    switch (degrees_to_use) {
-        case 0: fused_forward_kernel<0><<<blocks, FUSED_THREADS, 0, st>>>(f, rec, depths, radii, num_tiles_hit); break;
-        case 1: fused_forward_kernel<1><<<blocks, FUSED_THREADS, 0, st>>>(f, rec, depths, radii, num_tiles_hit); break;
-        case 2: fused_forward_kernel<2><<<blocks, FUSED_THREADS, 0, st>>>(f, rec, depths, radii, num_tiles_hit); break;
-        case 3: fused_forward_kernel<3><<<blocks, FUSED_THREADS, 0, st>>>(f, rec, depths, radii, num_tiles_hit); break;
-        default: fused_forward_kernel<4><<<blocks, FUSED_THREADS, 0, st>>>(f, rec, depths, radii, num_tiles_hit); break;
-    }
-    B200_LAUNCH_CHECK();
-    return B200_OK;
+    return launch_fused_forward(f, packed, depths, radii, num_tiles_hit, stream);
+}
+
+extern "C" int b200_fused_preprocess_forward_views(int num_views, int num_points, const float *means,
+                                                   const float *log_scales, const float *quats,
+                                                   const float *opacity_logit, const float *sh_dc, const float *sh_rest,
+                                                   int sh_bases, int degrees_to_use, const float *viewmats,
+                                                   const float *cam_pos, const float *lin_vel, const float *ang_vel,
+                                                   const float *intrinsics, float rolling_shutter_time,
+                                                   float exposure_time, unsigned img_height, unsigned img_width,
+                                                   unsigned block_width, float clip_thresh, void *packed, float *depths,
+                                                   int32_t *radii, int32_t *num_tiles_hit, void *stream) {
+    int rc = check_views(num_views, num_points, viewmats, cam_pos, lin_vel, ang_vel, intrinsics);
+    if (rc) return rc;
+    FusedParams f;
+    rc = fill_fused(f, num_points, means, log_scales, quats, opacity_logit, sh_dc, sh_rest, sh_bases, degrees_to_use,
+                    viewmats, cam_pos, lin_vel, ang_vel, rolling_shutter_time, exposure_time, 1.f, 1.f, 0.f, 0.f, img_height,
+                    img_width, block_width, clip_thresh);
+    if (rc) return rc;
+    f.views = num_views; f.intr = intrinsics;
+    return launch_fused_forward(f, packed, depths, radii, num_tiles_hit, stream);
 }
 
 extern "C" int b200_fused_geometry_forward(int num_points, const float *means, const float *log_scales, const float *quats,
@@ -323,14 +409,15 @@ extern "C" int b200_fused_colors_forward(int num_points, const float *means, con
     return B200_OK;
 }
 
-// cam_ws != null: deterministic camera sums (b200_fused_preprocess_backward_deterministic)
-static int run_fused_backward(int num_points, const float *means, const float *log_scales, const float *quats,
+// cam_ws != null: deterministic camera sums (b200_fused_preprocess_backward_deterministic).  views / intr: the view batch
+// (1 / null for one camera with the scalar intrinsics).
+static int run_fused_backward(int views, int num_points, const float *means, const float *log_scales, const float *quats,
                               const float *opacity_logit, const float *sh_dc, const float *sh_rest, int sh_bases,
                               int degrees_to_use, const float *viewmat, const float *cam_pos, const float *lin_vel,
-                              const float *ang_vel, float rolling_shutter_time, float exposure_time, float fx, float fy,
-                              float cx, float cy, unsigned img_height, unsigned img_width, unsigned block_width,
-                              float clip_thresh, const void *packed, const int32_t *radii, const float *v_xy,
-                              const float *v_pix_vel, const float *v_conic, const float *v_colors,
+                              const float *ang_vel, const float *intr, float rolling_shutter_time, float exposure_time,
+                              float fx, float fy, float cx, float cy, unsigned img_height, unsigned img_width,
+                              unsigned block_width, float clip_thresh, const void *packed, const int32_t *radii,
+                              const float *v_xy, const float *v_pix_vel, const float *v_conic, const float *v_colors,
                               const float *v_opacity, float *g_means, float *g_log_scales, float *g_quats,
                               float *g_opacity_logit, float *g_sh_dc, float *g_sh_rest, float *g_lin_vel,
                               float *g_ang_vel, float *g_viewmat, float *cam_ws, cudaStream_t st) {
@@ -339,15 +426,16 @@ static int run_fused_backward(int num_points, const float *means, const float *l
                         viewmat, cam_pos, lin_vel, ang_vel, rolling_shutter_time, exposure_time, fx, fy, cx, cy, img_height,
                         img_width, block_width, clip_thresh);
     if (rc) return rc;
+    f.views = views; f.intr = intr;
     B200_REQUIRE(packed && radii && v_xy && v_pix_vel && v_conic && v_colors && v_opacity, "null input pointer");
     B200_REQUIRE(g_means && g_log_scales && g_quats && g_opacity_logit && g_sh_dc && (sh_bases == 1 || g_sh_rest),
                  "null gradient pointer");
     // deterministic camera sums: the blocks store partials and cam_partials_sum_kernel overwrites the outputs
     const bool det = cam_ws && (g_lin_vel || g_ang_vel || g_viewmat);
     if (!det) {
-        if (g_lin_vel) B200_CUDA(cudaMemsetAsync(g_lin_vel, 0, 3 * sizeof(float), st));
-        if (g_ang_vel) B200_CUDA(cudaMemsetAsync(g_ang_vel, 0, 3 * sizeof(float), st));
-        if (g_viewmat) B200_CUDA(cudaMemsetAsync(g_viewmat, 0, 12 * sizeof(float), st));
+        if (g_lin_vel) B200_CUDA(cudaMemsetAsync(g_lin_vel, 0, 3 * sizeof(float) * (size_t)views, st));
+        if (g_ang_vel) B200_CUDA(cudaMemsetAsync(g_ang_vel, 0, 3 * sizeof(float) * (size_t)views, st));
+        if (g_viewmat) B200_CUDA(cudaMemsetAsync(g_viewmat, 0, 12 * sizeof(float) * (size_t)views, st));
     }
     FusedBwdIO io{reinterpret_cast<const PackedGaussian *>(packed), radii, v_xy, v_pix_vel, v_conic, v_colors, v_opacity,
                   g_means, g_log_scales, g_quats, g_opacity_logit, g_sh_dc, g_sh_rest, g_lin_vel, g_ang_vel, g_viewmat,
@@ -356,24 +444,24 @@ static int run_fused_backward(int num_points, const float *means, const float *l
     const int pitch = (rest_row & 1) ? rest_row : rest_row + 1;
     const size_t smem = sizeof(float) * FUSED_THREADS * (size_t)(pitch > 0 ? pitch : 1);
     const int blocks = ceil_div(num_points, FUSED_THREADS);
+    auto launch = [&](auto det_c, auto views_c) {
+        constexpr bool D = decltype(det_c)::value, V = decltype(views_c)::value;
+        switch (degrees_to_use) {
+            case 0: fused_backward_kernel<0, D, V><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
+            case 1: fused_backward_kernel<1, D, V><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
+            case 2: fused_backward_kernel<2, D, V><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
+            case 3: fused_backward_kernel<3, D, V><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
+            default: fused_backward_kernel<4, D, V><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
+        }
+    };
+    using T_ = std::true_type;
+    using F_ = std::false_type;
     if (det) {
-        switch (degrees_to_use) {
-            case 0: fused_backward_kernel<0, true><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
-            case 1: fused_backward_kernel<1, true><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
-            case 2: fused_backward_kernel<2, true><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
-            case 3: fused_backward_kernel<3, true><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
-            default: fused_backward_kernel<4, true><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
-        }
+        if (intr) launch(T_{}, T_{}); else launch(T_{}, F_{});
         B200_LAUNCH_CHECK();
-        cam_partials_sum_kernel<<<1, 32, 0, st>>>(blocks, cam_ws, g_lin_vel, g_ang_vel, g_viewmat);
+        cam_partials_sum_kernel<<<views, 32, 0, st>>>(blocks, cam_ws, g_lin_vel, g_ang_vel, g_viewmat);
     } else {
-        switch (degrees_to_use) {
-            case 0: fused_backward_kernel<0, false><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
-            case 1: fused_backward_kernel<1, false><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
-            case 2: fused_backward_kernel<2, false><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
-            case 3: fused_backward_kernel<3, false><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
-            default: fused_backward_kernel<4, false><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
-        }
+        if (intr) launch(F_{}, T_{}); else launch(F_{}, F_{});
     }
     B200_LAUNCH_CHECK();
     return B200_OK;
@@ -391,11 +479,12 @@ extern "C" int b200_fused_preprocess_backward(int num_points, const float *means
                                               const float *v_opacity, float *g_means, float *g_log_scales,
                                               float *g_quats, float *g_opacity_logit, float *g_sh_dc, float *g_sh_rest,
                                               float *g_lin_vel, float *g_ang_vel, float *g_viewmat, void *stream) {
-    return run_fused_backward(num_points, means, log_scales, quats, opacity_logit, sh_dc, sh_rest, sh_bases,
-                              degrees_to_use, viewmat, cam_pos, lin_vel, ang_vel, rolling_shutter_time, exposure_time, fx,
-                              fy, cx, cy, img_height, img_width, block_width, clip_thresh, packed, radii, v_xy, v_pix_vel,
-                              v_conic, v_colors, v_opacity, g_means, g_log_scales, g_quats, g_opacity_logit, g_sh_dc,
-                              g_sh_rest, g_lin_vel, g_ang_vel, g_viewmat, nullptr, as_stream(stream));
+    return run_fused_backward(1, num_points, means, log_scales, quats, opacity_logit, sh_dc, sh_rest, sh_bases,
+                              degrees_to_use, viewmat, cam_pos, lin_vel, ang_vel, nullptr, rolling_shutter_time,
+                              exposure_time, fx, fy, cx, cy, img_height, img_width, block_width, clip_thresh, packed, radii,
+                              v_xy, v_pix_vel, v_conic, v_colors, v_opacity, g_means, g_log_scales, g_quats,
+                              g_opacity_logit, g_sh_dc, g_sh_rest, g_lin_vel, g_ang_vel, g_viewmat, nullptr,
+                              as_stream(stream));
 }
 
 extern "C" size_t b200_fused_preprocess_backward_ws_bytes(int num_points) {
@@ -416,9 +505,56 @@ extern "C" int b200_fused_preprocess_backward_deterministic(
     const size_t need = b200_fused_preprocess_backward_ws_bytes(num_points);
     B200_REQUIRE(ws_bytes >= need, "ws too small: %zu bytes, b200_fused_preprocess_backward_ws_bytes gives %zu",
                  ws_bytes, need);
-    return run_fused_backward(num_points, means, log_scales, quats, opacity_logit, sh_dc, sh_rest, sh_bases,
-                              degrees_to_use, viewmat, cam_pos, lin_vel, ang_vel, rolling_shutter_time, exposure_time, fx,
-                              fy, cx, cy, img_height, img_width, block_width, clip_thresh, packed, radii, v_xy, v_pix_vel,
-                              v_conic, v_colors, v_opacity, g_means, g_log_scales, g_quats, g_opacity_logit, g_sh_dc,
-                              g_sh_rest, g_lin_vel, g_ang_vel, g_viewmat, static_cast<float *>(ws), as_stream(stream));
+    return run_fused_backward(1, num_points, means, log_scales, quats, opacity_logit, sh_dc, sh_rest, sh_bases,
+                              degrees_to_use, viewmat, cam_pos, lin_vel, ang_vel, nullptr, rolling_shutter_time,
+                              exposure_time, fx, fy, cx, cy, img_height, img_width, block_width, clip_thresh, packed, radii,
+                              v_xy, v_pix_vel, v_conic, v_colors, v_opacity, g_means, g_log_scales, g_quats,
+                              g_opacity_logit, g_sh_dc, g_sh_rest, g_lin_vel, g_ang_vel, g_viewmat,
+                              static_cast<float *>(ws), as_stream(stream));
+}
+
+extern "C" int b200_fused_preprocess_backward_views(
+    int num_views, int num_points, const float *means, const float *log_scales, const float *quats,
+    const float *opacity_logit, const float *sh_dc, const float *sh_rest, int sh_bases, int degrees_to_use,
+    const float *viewmats, const float *cam_pos, const float *lin_vel, const float *ang_vel, const float *intrinsics,
+    float rolling_shutter_time, float exposure_time, unsigned img_height, unsigned img_width, unsigned block_width,
+    float clip_thresh, const void *packed, const int32_t *radii, const float *v_xy, const float *v_pix_vel,
+    const float *v_conic, const float *v_colors, const float *v_opacity, float *g_means, float *g_log_scales,
+    float *g_quats, float *g_opacity_logit, float *g_sh_dc, float *g_sh_rest, float *g_lin_vel, float *g_ang_vel,
+    float *g_viewmat, void *stream) {
+    int rc = check_views(num_views, num_points, viewmats, cam_pos, lin_vel, ang_vel, intrinsics);
+    if (rc) return rc;
+    return run_fused_backward(num_views, num_points, means, log_scales, quats, opacity_logit, sh_dc, sh_rest, sh_bases,
+                              degrees_to_use, viewmats, cam_pos, lin_vel, ang_vel, intrinsics, rolling_shutter_time,
+                              exposure_time, 1.f, 1.f, 0.f, 0.f, img_height, img_width, block_width, clip_thresh, packed,
+                              radii, v_xy, v_pix_vel, v_conic, v_colors, v_opacity, g_means, g_log_scales, g_quats,
+                              g_opacity_logit, g_sh_dc, g_sh_rest, g_lin_vel, g_ang_vel, g_viewmat, nullptr,
+                              as_stream(stream));
+}
+
+extern "C" size_t b200_fused_preprocess_backward_views_ws_bytes(int num_views, int num_points) {
+    return num_views < 1 ? 0 : (size_t)num_views * b200_fused_preprocess_backward_ws_bytes(num_points);
+}
+
+extern "C" int b200_fused_preprocess_backward_views_deterministic(
+    int num_views, int num_points, const float *means, const float *log_scales, const float *quats,
+    const float *opacity_logit, const float *sh_dc, const float *sh_rest, int sh_bases, int degrees_to_use,
+    const float *viewmats, const float *cam_pos, const float *lin_vel, const float *ang_vel, const float *intrinsics,
+    float rolling_shutter_time, float exposure_time, unsigned img_height, unsigned img_width, unsigned block_width,
+    float clip_thresh, const void *packed, const int32_t *radii, const float *v_xy, const float *v_pix_vel,
+    const float *v_conic, const float *v_colors, const float *v_opacity, float *g_means, float *g_log_scales,
+    float *g_quats, float *g_opacity_logit, float *g_sh_dc, float *g_sh_rest, float *g_lin_vel, float *g_ang_vel,
+    float *g_viewmat, void *ws, size_t ws_bytes, void *stream) {
+    int rc = check_views(num_views, num_points, viewmats, cam_pos, lin_vel, ang_vel, intrinsics);
+    if (rc) return rc;
+    B200_REQUIRE(ws && aligned16(ws), "ws must be a 16-byte aligned workspace");
+    const size_t need = b200_fused_preprocess_backward_views_ws_bytes(num_views, num_points);
+    B200_REQUIRE(ws_bytes >= need, "ws too small: %zu bytes, b200_fused_preprocess_backward_views_ws_bytes gives %zu",
+                 ws_bytes, need);
+    return run_fused_backward(num_views, num_points, means, log_scales, quats, opacity_logit, sh_dc, sh_rest, sh_bases,
+                              degrees_to_use, viewmats, cam_pos, lin_vel, ang_vel, intrinsics, rolling_shutter_time,
+                              exposure_time, 1.f, 1.f, 0.f, 0.f, img_height, img_width, block_width, clip_thresh, packed,
+                              radii, v_xy, v_pix_vel, v_conic, v_colors, v_opacity, g_means, g_log_scales, g_quats,
+                              g_opacity_logit, g_sh_dc, g_sh_rest, g_lin_vel, g_ang_vel, g_viewmat,
+                              static_cast<float *>(ws), as_stream(stream));
 }

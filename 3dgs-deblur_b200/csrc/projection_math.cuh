@@ -317,17 +317,20 @@ __device__ __forceinline__ void project_backward_one(const ProjCommon &p, bool w
 }
 
 // Deterministic mode of the camera gradients: block b of a projection / fused backward stores its 18 partial sums
-// (lin_vel 3, ang_vel 3, viewmat 12) at partials[18 b + c] instead of adding them to the outputs; this kernel (one warp)
-// sums each component in block order and OVERWRITES the non-null outputs.
+// (lin_vel 3, ang_vel 3, viewmat 12) at partials[18 b + c] instead of adding them to the outputs; this kernel (one warp
+// per view, grid = views; view v's partials follow those of view v - 1) sums each component in block order and
+// OVERWRITES the non-null outputs (v_lin / v_ang + 3 v, v_viewmat + 12 v).
 static __global__ void __launch_bounds__(32) cam_partials_sum_kernel(int blocks, const float *__restrict__ partials,
                                                                      float *v_lin, float *v_ang, float *v_viewmat) {
     const int c = threadIdx.x;
     if (c >= 18) return;
+    const size_t v = blockIdx.x;
+    partials += 18 * (size_t)blocks * v;
     float s = 0.f;
     for (int b = 0; b < blocks; ++b) s += partials[18 * (size_t)b + c];
-    float *dst = c < 3 ? (v_lin ? v_lin + c : nullptr)
-               : c < 6 ? (v_ang ? v_ang + (c - 3) : nullptr)
-                       : (v_viewmat ? v_viewmat + (c - 6) : nullptr);
+    float *dst = c < 3 ? (v_lin ? v_lin + 3 * v + c : nullptr)
+               : c < 6 ? (v_ang ? v_ang + 3 * v + (c - 3) : nullptr)
+                       : (v_viewmat ? v_viewmat + 12 * v + (c - 6) : nullptr);
     if (dst) *dst = s;
 }
 

@@ -87,6 +87,23 @@ SIGNATURES = {
     "b200_fused_preprocess_backward_deterministic": (_i, [_i, _p, _p, _p, _p, _p, _p, _i, _i, _p, _p, _p, _p, _f, _f, _f, _f,
                                                           _f, _f, _u, _u, _u, _f, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p,
                                                           _p, _p, _p, _p, _p, _p, _p, _sz, _p]),
+    "b200_fused_preprocess_forward_views": (_i, [_i, _i, _p, _p, _p, _p, _p, _p, _i, _i, _p, _p, _p, _p, _p, _f, _f, _u, _u, _u,
+                                                 _f, _p, _p, _p, _p, _p]),
+    "b200_fused_preprocess_backward_views": (_i, [_i, _i, _p, _p, _p, _p, _p, _p, _i, _i, _p, _p, _p, _p, _p, _f, _f, _u, _u,
+                                                  _u, _f, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p,
+                                                  _p]),
+    "b200_fused_preprocess_backward_views_ws_bytes": (_sz, [_i, _i]),
+    "b200_fused_preprocess_backward_views_deterministic": (_i, [_i, _i, _p, _p, _p, _p, _p, _p, _i, _i, _p, _p, _p, _p, _p,
+                                                                _f, _f, _u, _u, _u, _f, _p, _p, _p, _p, _p, _p, _p, _p,
+                                                                _p, _p, _p, _p, _p, _p, _p, _p, _p, _sz, _p]),
+    "b200_bin_cull_views_ws_bytes": (_sz, [_i, _i]),
+    "b200_bin_cull_count_views": (_i, [_i, _i, _p, _p, _p, _p, _u, _u, _u, _u, _f, _f, _p, _sz, _p, _p, _p, _p]),
+    "b200_bin_cull_emit_views": (_i, [_i, _i, _i, _p, _p, _p, _u, _u, _u, _u, _f, _f, _p, _p, _sz, _p, _p, _p]),
+    "b200_blend_forward_views": (_i, [_i, _u, _u, _u, _u, _p, _p, _p, _f, _f, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "b200_blend_backward_views": (_i, [_i, _i, _u, _u, _u, _u, _p, _p, _p, _f, _f, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p,
+                                       _p, _p, _i, _p]),
+    "b200_blend_backward_views_deterministic": (_i, [_i, _i, _i, _u, _u, _u, _u, _p, _p, _p, _f, _f, _p, _p, _p, _p, _p,
+                                                     _p, _p, _sz, _p, _p, _p, _p, _p, _p, _p]),
     "b200_nd_rasterize_forward": (_i, [_i, _u, _u, _u, _u, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
     "b200_nd_rasterize_backward": (_i, [_i, _u, _u, _u, _u, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p,
                                         _p, _p, _p, _p, _p, _p]),

@@ -414,12 +414,126 @@ def fused_preprocess_backward(device, *args):
         check(lib.b200_fused_preprocess_backward(*args, stream()))
 
 
-def _tile_order(tile_bins, H, W, bw):
-    """Scratch int32[num_tiles] holding the blend's CTA -> tile order (longest list first), computed on the device."""
-    tiles = ((W + bw - 1) // bw) * ((H + bw - 1) // bw)
+def _tile_order(tile_bins, H, W, bw, views=1):
+    """Scratch int32[num_tiles] holding the blend's CTA -> tile order (longest list first), computed on the device.
+    views > 1: the (view, tile) order over the views * num_tiles bins of a view batch."""
+    tiles = views * ((W + bw - 1) // bw) * ((H + bw - 1) // bw)
     order = torch.empty((tiles,), dtype=torch.int32, device=tile_bins.device)
     check(_lib.load().b200_blend_tile_order(tiles, ptr(tile_bins), ptr(order), stream()))
     return order
+
+
+# ---- view batches (include/b200splat.h "view batches"): record v * N + g is Gaussian g seen by camera v ----------------
+
+def bin_cull_views(views, packed, depths, radii, num_tiles_hit, img_height, img_width, block_width, n_blur_samples,
+                   rolling_shutter_time, exposure_time):
+    """Extension: culled binning of a batch of `views` images over views * N records -> (view_isect (views,) int32 on the
+    device: every view's reference num_intersects, gaussian_ids_sorted (M,), tile_bins (views * tiles, 2)).  One host sync
+    for the whole batch."""
+    require_cuda(packed, depths, radii, num_tiles_hit)
+    dev = depths.device
+    B = int(views)
+    n = depths.numel() // B
+    H, W, bw, S = int(img_height), int(img_width), int(block_width), int(n_blur_samples)
+    rs, ex = float(rolling_shutter_time), float(exposure_time)
+    with on_device(dev):
+        lib = _lib.load()
+        ws_bytes = lib.b200_bin_cull_views_ws_bytes(B, n)
+        if ws_bytes == 0:
+            raise ValueError(f"bin_cull_views: {B} views x {n} Gaussians exceed the int32 record ids")
+        ws_g = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
+        view_isect = torch.empty((B,), dtype=torch.int32, device=dev)
+        bins = torch.empty((B * ((W + bw - 1) // bw) * ((H + bw - 1) // bw), 2), dtype=torch.int32, device=dev)
+        host_ptr, host = _lib.host_scratch_np(dev)
+        flag = _lib.take_pending_flag(dev)
+        check(lib.b200_bin_cull_count_views(B, n, ptr(packed), ptr(_f32(depths)), ptr(radii), ptr(num_tiles_hit), H, W,
+                                            bw, S, rs, ex, ptr(ws_g), ws_bytes, host_ptr, ptr(view_isect), ptr(flag),
+                                            stream()))
+        torch.cuda.current_stream().synchronize()  # the one host sync of the batch
+        if host[4]:
+            _lib.raise_if_flagged(host[4])
+        if B > 1 and host[6]:
+            raise ValueError("render_gaussians_batch: the batch's list entries exceed int32; render fewer views per call")
+        m = int(host[3])
+        ids = torch.empty((m,), dtype=torch.int32, device=dev)
+        e_bytes = lib.b200_bin_cull_emit_ws_bytes(m)
+        ws_e = torch.empty((e_bytes,), dtype=torch.uint8, device=dev)
+        check(lib.b200_bin_cull_emit_views(B, n, m, ptr(packed), ptr(radii), ptr(num_tiles_hit), H, W, bw, S, rs, ex,
+                                           ptr(ws_g), ptr(ws_e), e_bytes, ptr(ids), ptr(bins), stream()))
+    return view_isect, ids, bins
+
+
+def blend_forward_views(views, img_height, img_width, block_width, n_blur_samples, gaussian_ids_sorted, tile_bins, packed,
+                        rolling_shutter_time, exposure_time, background, view_isect, want_alpha=True):
+    """Extension: blend forward of a view batch -> (out_img (B,H,W,3), final_Ts (B,H,W,S), final_idx (B,H,W,S)[, alpha
+    (B,H,W)]); a view whose view_isect is < 1 gets the reference's empty render."""
+    require_cuda(gaussian_ids_sorted, tile_bins, packed, background, view_isect)
+    dev = packed.device
+    B, H, W, bw, S = int(views), int(img_height), int(img_width), int(block_width), int(n_blur_samples)
+    with on_device(dev):
+        out_img = torch.empty((B, H, W, 3), dtype=torch.float32, device=dev)
+        final_Ts = torch.empty((B, H, W, S), dtype=torch.float32, device=dev)
+        final_idx = torch.empty((B, H, W, S), dtype=torch.int32, device=dev)
+        alpha = torch.empty((B, H, W), dtype=torch.float32, device=dev) if want_alpha else None
+        order = _tile_order(tile_bins, H, W, bw, B)
+        check(_lib.load().b200_blend_forward_views(
+            B, H, W, bw, S, ptr(gaussian_ids_sorted), ptr(tile_bins), ptr(packed), float(rolling_shutter_time),
+            float(exposure_time), ptr(_f32(background)), ptr(view_isect), ptr(order), ptr(out_img), ptr(final_Ts),
+            ptr(final_idx), ptr(alpha), stream()))
+    if want_alpha:
+        return out_img, final_Ts, final_idx, alpha
+    return out_img, final_Ts, final_idx
+
+
+def blend_backward_views(views, num_records, img_height, img_width, block_width, n_blur_samples, gaussian_ids_sorted,
+                         tile_bins, packed, rolling_shutter_time, exposure_time, background, final_Ts, final_idx, v_output,
+                         v_output_alpha):
+    """Extension: blend backward of a view batch -> per-record (views * N rows) (v_xy, v_xy_abs, v_pix_vels, v_conic,
+    v_colors, v_opacity); deterministic under torch.use_deterministic_algorithms(True) like blend_backward_packed."""
+    require_cuda(gaussian_ids_sorted, tile_bins, packed, background, final_Ts, final_idx)
+    dev = packed.device
+    B, n, H, W, bw, S = int(views), int(num_records), int(img_height), int(img_width), int(block_width), int(n_blur_samples)
+    rs, ex = float(rolling_shutter_time), float(exposure_time)
+    lib = _lib.load()
+    with on_device(dev):
+        f32 = dict(dtype=torch.float32, device=dev)
+        v_output = _f32(v_output).contiguous()
+        v_output_alpha = _f32(v_output_alpha).contiguous() if v_output_alpha is not None else None
+        order = _tile_order(tile_bins, H, W, bw, B)
+        if deterministic():
+            m = gaussian_ids_sorted.numel()
+            nbytes = lib.b200_blend_backward_deterministic_ws_bytes(n, m, bw)
+            ws = _lib.workspace(nbytes, dev)
+            outs = (torch.empty((n, 2), **f32), torch.empty((n, 2), **f32), torch.empty((n, 2), **f32),
+                    torch.empty((n, 3), **f32), torch.empty((n, 3), **f32), torch.empty((n, 1), **f32))
+            check(lib.b200_blend_backward_views_deterministic(
+                B, n, m, H, W, bw, S, ptr(gaussian_ids_sorted), ptr(tile_bins), ptr(packed), rs, ex, ptr(_f32(background)),
+                ptr(_f32(final_Ts)), ptr(final_idx), ptr(v_output), ptr(v_output_alpha), ptr(order), ptr(ws), nbytes,
+                *[ptr(t) for t in outs], stream()))
+            return outs
+        pitch = (n + 15) & ~15  # one zero-filled allocation, as in blend_backward_packed
+        acc = torch.zeros(13 * pitch, **f32)
+        v_xy, v_xy_abs, v_pix = (acc[k * 2 * pitch:k * 2 * pitch + 2 * n].view(n, 2) for k in range(3))
+        v_conic, v_colors = (acc[6 * pitch + k * 3 * pitch:6 * pitch + k * 3 * pitch + 3 * n].view(n, 3) for k in range(2))
+        v_opacity = acc[12 * pitch:12 * pitch + n].view(n, 1)
+        check(lib.b200_blend_backward_views(
+            B, n, H, W, bw, S, ptr(gaussian_ids_sorted), ptr(tile_bins), ptr(packed), rs, ex, ptr(_f32(background)),
+            ptr(_f32(final_Ts)), ptr(final_idx), ptr(v_output), ptr(v_output_alpha), ptr(order), ptr(v_xy), ptr(v_xy_abs),
+            ptr(v_pix), ptr(v_conic), ptr(v_colors), ptr(v_opacity), 1, stream()))
+    return v_xy, v_xy_abs, v_pix, v_conic, v_colors, v_opacity
+
+
+def fused_preprocess_backward_views(device, *args):
+    """b200_fused_preprocess_backward_views with `args` as in include/b200splat.h up to the stream; camera sums in block
+    order under torch.use_deterministic_algorithms(True)."""
+    lib = _lib.load()
+    views, n, g_cam = int(args[0]), int(args[1]), args[-3:]
+    if deterministic() and any(p is not None for p in g_cam):
+        nbytes = lib.b200_fused_preprocess_backward_views_ws_bytes(views, n)
+        ws = _lib.workspace(nbytes, device)
+        check(lib.b200_fused_preprocess_backward_views_deterministic(*args, ptr(ws), nbytes, stream()))
+    else:
+        check(lib.b200_fused_preprocess_backward_views(*args, stream()))
 
 
 def _geom(tile_bounds, block, img_size):

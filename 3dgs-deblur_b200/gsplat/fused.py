@@ -8,6 +8,7 @@ binning, the blend, and in backward one fused post-processing kernel.  It needs 
 `gsplat.project_gaussians / spherical_harmonics / rasterize_gaussians` stay the drop-in surface.
 
 Outputs are the same as chaining the three drop-in operators the way Splatfacto does (tests/test_gpu_fused.py).
+`render_gaussians_batch` renders B cameras of the scene in one call (view v = the single-view render of camera v).
 """
 from typing import Dict, Optional
 
@@ -171,3 +172,166 @@ class _FusedRender(Function):
             else:
                 v_bg = torch.matmul(v_rgb.float().reshape(-1, 3).t(), Ts.mean(dim=-1).float().reshape(-1, 1)).squeeze()
         return (*ret, v_viewmat, None, v_lin, v_ang, v_bg, None, None, None)
+
+
+_INT32_MAX = 2**31 - 1
+
+
+def render_gaussians_batch(means: Tensor, log_scales: Tensor, quats: Tensor, opacity_logit: Tensor, sh_dc: Tensor,
+                           sh_rest: Tensor, viewmats: Tensor, cam_pos: Tensor, linear_velocity: Optional[Tensor],
+                           angular_velocity: Optional[Tensor], fx, fy, cx, cy, img_height: int, img_width: int,
+                           block_width: int, background: Tensor, rolling_shutter_time: float = 0.0,
+                           exposure_time: float = 0.0, blur_samples: int = 1, sh_degree_to_use: int = 3,
+                           clip_thresh: float = 0.01, return_depth: bool = False):
+    """`render_gaussians` for B cameras of one scene in one call: one fused pre-processing launch over B * N records,
+    one culled binning with one host sync, one blend grid over the B * T tiles (longest lists first across all views).
+
+    viewmats (B,3,4) or (B,4,4); cam_pos (B,3); linear / angular velocity (B,3) each or None (zero); fx, fy, cx, cy each a
+    float shared by the views or a (B,) tensor.  Image size, block width, blur samples, shutter timing, SH degree, clip
+    and background (3,) are shared by the batch.
+
+    Returns (rgb (B,H,W,3), alpha (B,H,W), info): info["radii"] (B,N) int32; after backward info["absgrad"] (B,N,2)
+    (per view: feed Densifier.accumulate once per view); with return_depth info["depth"] (B,H,W,1).
+
+    View v is the single-view render of camera v: rgb[v], alpha[v], radii[v] and depth[v] are bit-identical to
+    render_gaussians with camera v's arguments (a view with nothing to intersect takes the empty-render branch on its
+    own; the alpha-0 depth fill is that view's own maximum).  The raw-parameter and background gradients are the sums
+    of the single-view ones over the views, the view-matrix and velocity gradients are per view; under
+    torch.use_deterministic_algorithms(True) every gradient equals the single-view gradients added in view order, bit
+    for bit."""
+    if viewmats.dim() != 3 or tuple(viewmats.shape[1:]) not in ((3, 4), (4, 4)):
+        raise ValueError(f"render_gaussians_batch: viewmats must be (B,3,4) or (B,4,4), got {tuple(viewmats.shape)}")
+    B, n = int(viewmats.shape[0]), int(means.shape[0])
+    if B < 1:
+        raise ValueError("render_gaussians_batch: at least one view is needed")
+    for name, t in (("cam_pos", cam_pos), ("linear_velocity", linear_velocity), ("angular_velocity", angular_velocity)):
+        if t is not None and tuple(t.shape) != (B, 3):
+            raise ValueError(f"render_gaussians_batch: {name} must be ({B}, 3) for {B} views, got {tuple(t.shape)}")
+    for name, k in (("fx", fx), ("fy", fy), ("cx", cx), ("cy", cy)):
+        if torch.is_tensor(k) and tuple(k.shape) != (B,):
+            raise ValueError(f"render_gaussians_batch: {name} must be a float or a ({B},) tensor, got {tuple(k.shape)}")
+    if B * n > _INT32_MAX:
+        raise ValueError(f"render_gaussians_batch: {B} views x {n} Gaussians exceed the int32 record ids")
+    H, W, bw, S = int(img_height), int(img_width), int(block_width), int(blur_samples)
+    if not (0 < S <= 10):
+        raise RuntimeError("unsupported blur size")
+    tiles = ((W + bw - 1) // bw) * ((H + bw - 1) // bw) if bw > 0 else 0
+    if B * tiles > _INT32_MAX - 1 or B * H > _INT32_MAX - 1:
+        raise ValueError("render_gaussians_batch: the batch's tiles exceed int32")
+    _lib.require_cuda(*(t.contiguous() for t in (means, log_scales, quats, opacity_logit, sh_dc, sh_rest, viewmats, cam_pos,
+                                                  background)))
+    dev = means.device
+    lin = linear_velocity if linear_velocity is not None else torch.zeros(B, 3, device=dev)
+    ang = angular_velocity if angular_velocity is not None else torch.zeros(B, 3, device=dev)
+    intr = torch.stack([k.detach().to(device=dev, dtype=torch.float32).reshape(B) if torch.is_tensor(k)
+                        else torch.full((B,), float(k), dtype=torch.float32, device=dev)
+                        for k in (fx, fy, cx, cy)], dim=1).contiguous()
+    info: Dict[str, Tensor] = {}
+    rgb, alpha = _FusedRenderBatch.apply(means, log_scales, quats, opacity_logit, sh_dc, sh_rest, viewmats, cam_pos, lin,
+                                         ang, background, intr,
+                                         (H, W, bw, float(rolling_shutter_time), float(exposure_time), S,
+                                          int(sh_degree_to_use), float(clip_thresh)), info)
+    lists = info.pop("_lists")
+    if return_depth:
+        info["depth"] = _depth_pass_views(lists, alpha, B, H, W, bw, S, float(rolling_shutter_time), float(exposure_time))
+    return rgb, alpha, info
+
+
+def _depth_pass_views(lists, alpha, B, H, W, bw, S, rs, ex):
+    """`_depth_pass` over a view batch: the same static depth blend and lists reuse rule, each view filled with its own
+    maximum where its alpha is 0."""
+    packed, depths, radii, nth, ids, bins, view_isect = lists
+    dev = depths.device
+    with torch.no_grad(), _lib.on_device(dev):
+        rec = _C.set_record_colors(packed.clone(), depths[:, None].expand(-1, 3).contiguous())
+        if not (rs == 0 and (ex == 0 or S % 2 == 1)):  # see _depth_pass
+            view_isect, ids, bins = _C.bin_cull_views(B, rec, depths, radii, nth, H, W, bw, 1, 0.0, 0.0)
+        img, _, _ = _C.blend_forward_views(B, H, W, bw, 1, ids, bins, rec, 0.0, 0.0, torch.zeros(3, device=dev), view_isect,
+                                           want_alpha=False)
+        depth_im = img[..., 0:1]
+        a = alpha.detach()[..., None]
+        return torch.where(a > 0, depth_im / a, depth_im.amax(dim=(1, 2, 3), keepdim=True))
+
+
+class _FusedRenderBatch(Function):
+    @staticmethod
+    def forward(ctx, means, log_scales, quats, opacity_logit, sh_dc, sh_rest, viewmats, cam_pos, lin, ang, background,
+                intr, cfg, info):
+        H, W, bw, rs, ex, S, deg, clip = cfg
+        dev = means.device
+        lib = _lib.load()
+        B, n = viewmats.shape[0], means.shape[0]
+        K = sh_rest.shape[1] + 1
+        tens = [t.contiguous() for t in (means, log_scales, quats, opacity_logit, sh_dc, sh_rest, cam_pos)]
+        means, log_scales, quats, opacity_logit, sh_dc, sh_rest, cam_pos = tens
+        vm = viewmats.detach()[:, :3, :4].contiguous()
+        # velocities may live on the host, like render_gaussians': the kernels take device arrays
+        lin_d = lin.detach().to(device=dev, dtype=torch.float32).reshape(B, 3).contiguous()
+        ang_d = ang.detach().to(device=dev, dtype=torch.float32).reshape(B, 3).contiguous()
+        with _lib.on_device(dev):
+            packed = torch.empty((B * n * lib.b200_packed_record_bytes(),), dtype=torch.uint8, device=dev)
+            depths = torch.empty((B * n,), dtype=torch.float32, device=dev)
+            radii = torch.empty((B * n,), dtype=torch.int32, device=dev)
+            nth = torch.empty((B * n,), dtype=torch.int32, device=dev)
+            check(lib.b200_fused_preprocess_forward_views(
+                B, n, ptr(means), ptr(log_scales), ptr(quats), ptr(opacity_logit), ptr(sh_dc), ptr(sh_rest), K, deg,
+                ptr(vm), ptr(cam_pos), ptr(lin_d), ptr(ang_d), ptr(intr), rs, ex, H, W, bw, clip, ptr(packed),
+                ptr(depths), ptr(radii), ptr(nth), stream()))
+            view_isect, ids, bins = _C.bin_cull_views(B, packed, depths, radii, nth, H, W, bw, S, rs, ex)
+            bg = background.contiguous()
+            rgb, Ts, fi, alpha = _C.blend_forward_views(B, H, W, bw, S, ids, bins, packed, rs, ex, bg, view_isect)
+        ctx.cfg, ctx.K, ctx.B = cfg, K, B
+        ctx.info = info
+        ctx.vel_shapes = (lin.shape, ang.shape)
+        ctx.vel_devs = (lin.device, ang.device)
+        ctx.save_for_backward(means, log_scales, quats, opacity_logit, sh_dc, sh_rest, viewmats, vm, cam_pos, lin_d, ang_d,
+                              intr, bg, packed, radii, ids, bins, Ts, fi)
+        info["radii"] = radii.view(B, n)
+        info["_lists"] = (packed, depths, radii, nth, ids, bins, view_isect)  # for the optional depth pass
+        ctx.mark_non_differentiable(radii)
+        ctx.set_materialize_grads(False)
+        return rgb, alpha
+
+    @staticmethod
+    def backward(ctx, v_rgb, v_alpha):
+        (means, log_scales, quats, opacity_logit, sh_dc, sh_rest, viewmats, vm, cam_pos, lin_d, ang_d, intr, bg, packed,
+         radii, ids, bins, Ts, fi) = ctx.saved_tensors
+        H, W, bw, rs, ex, S, deg, clip = ctx.cfg
+        dev = means.device
+        B, n, K = ctx.B, means.shape[0], ctx.K
+        f32 = dict(dtype=torch.float32, device=dev)
+        if v_rgb is None:
+            v_rgb = torch.zeros(B, H, W, 3, **f32)
+        with _lib.on_device(dev):
+            v_xy, v_abs, v_pix, v_conic, v_col, v_op = _C.blend_backward_views(
+                B, B * n, H, W, bw, S, ids, bins, packed, rs, ex, bg, Ts, fi, v_rgb.contiguous(), v_alpha)
+            ctx.info["absgrad"] = v_abs.view(B, n, 2)
+            raw = (means, log_scales, quats, opacity_logit, sh_dc, sh_rest)
+            out = [torch.empty_like(t) for t in raw]
+            want_vel = ctx.needs_input_grad[8] or ctx.needs_input_grad[9]
+            want_vm = ctx.needs_input_grad[6]
+            g_lin = torch.empty(B, 3, **f32) if want_vel else None
+            g_ang = torch.empty(B, 3, **f32) if want_vel else None
+            g_vm = torch.empty(B, 3, 4, **f32) if want_vm else None
+            _C.fused_preprocess_backward_views(
+                dev, B, n, ptr(means), ptr(log_scales), ptr(quats), ptr(opacity_logit), ptr(sh_dc), ptr(sh_rest), K, deg,
+                ptr(vm), ptr(cam_pos), ptr(lin_d), ptr(ang_d), ptr(intr), rs, ex, H, W, bw, clip, ptr(packed), ptr(radii),
+                ptr(v_xy), ptr(v_pix), ptr(v_conic), ptr(v_col), ptr(v_op), *[ptr(t) for t in out], ptr(g_lin), ptr(g_ang),
+                ptr(g_vm))
+            v_viewmat = None
+            if want_vm:
+                v_viewmat = torch.zeros_like(viewmats)
+                v_viewmat[:, :3, :4] = g_vm
+            v_bg = None
+            if ctx.needs_input_grad[10]:
+                if torch.are_deterministic_algorithms_enabled():
+                    # per view, the single-view expression; the views added in order
+                    for v in range(B):
+                        g = (v_rgb[v].float() * Ts[v].mean(dim=-1).float()[..., None]).sum((0, 1))
+                        v_bg = g if v_bg is None else v_bg + g
+                else:
+                    v_bg = torch.matmul(v_rgb.float().reshape(B, -1, 3).transpose(1, 2),
+                                        Ts.mean(dim=-1).float().reshape(B, -1, 1)).sum(0).squeeze(-1)
+        v_lin = g_lin.reshape(ctx.vel_shapes[0]).to(ctx.vel_devs[0]) if (want_vel and ctx.needs_input_grad[8]) else None
+        v_ang = g_ang.reshape(ctx.vel_shapes[1]).to(ctx.vel_devs[1]) if (want_vel and ctx.needs_input_grad[9]) else None
+        return (*out, v_viewmat, None, v_lin, v_ang, v_bg, None, None, None)

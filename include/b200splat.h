@@ -336,6 +336,99 @@ B200_API int b200_fused_preprocess_backward(int num_points, const float *means, 
                                             float *g_sh_rest, float *g_lin_vel, float *g_ang_vel, float *g_viewmat,
                                             void *stream);
 
+/* ---- view batches: B cameras of one scene in one call ----------------------------------------------------------------
+ * The fused forward, culled binning and blend with a view dimension; camera v of the batch gives exactly the single-view
+ * result (the single-view entry points run the same kernels with B = 1).  Layout, for B views of N Gaussians, T =
+ * tiles_x * tiles_y tiles per view:
+ *   records   Gaussian g of view v is record r = v * N + g: packed (B * N * 64 bytes, record id = r), depths, radii,
+ *             num_tiles_hit (B * N), and the blend gradients (v_xy, v_xy_abs, v_pix_vels (B*N,2); v_conic, v_colors
+ *             (B*N,3); v_opacity (B*N)).
+ *   lists     tile t of view v is list key v * T + t: tile_bins (B * T, 2); the ids are record ids.  Each tile's list is
+ *             that view's single-view list (stable sorts: depth order, ties by Gaussian id); every view's phantom entries
+ *             (key v * T, id v * N, kept iff Gaussian 0 of the view can touch its tile 0) lead its tile 0.
+ *   images    out_img (B,H,W,3), final_Ts / final_idx (B,H,W,S), out_alpha / v_output_alpha (B,H,W), v_output (B,H,W,3).
+ *   cameras   viewmats (B,3,4) row major, cam_pos / lin_vel / ang_vel (B,3), intrinsics (B,4) = fx, fy, cx, cy per view
+ *             (16-byte aligned); camera gradients g_lin_vel / g_ang_vel (B,3), g_viewmat (B,3,4), overwritten.
+ * b200_fused_preprocess_forward_views: grid (ceil(N / 128), B).
+ * b200_fused_preprocess_backward_views(_deterministic): one thread per Gaussian, the views in order; the raw-parameter
+ *   gradients are the sums over the views, added in view order with separately rounded adds, so they equal the B
+ *   single-view gradients added one after the other.  ws of the deterministic variant: 16-byte aligned,
+ *   b200_fused_preprocess_backward_views_ws_bytes(B, N) bytes (18 floats per view and block of 128 Gaussians).
+ * b200_bin_cull_count_views / b200_bin_cull_emit_views: b200_bin_cull_count / _emit over the B * N records, ONE host read
+ *   for the batch.  ws_g: b200_bin_cull_views_ws_bytes(B, N) bytes (0: B * N exceeds int32); ws_e as for
+ *   b200_bin_cull_emit (b200_bin_cull_emit_ws_bytes(M)).  totals_host_pinned[7] (HOST, pinned, may be null): the five
+ *   words of b200_bin_cull_count summed over the views ([2]: view 0), then [5] phantom entries kept and [6] = 1 if the
+ *   batch's reserved-slot total [0] does not fit in int32 (the lists cannot be built).  view_isect (DEVICE int32[B]):
+ *   every view's reference num_intersects.
+ * b200_blend_forward_views / b200_blend_backward_views(_deterministic): the blends over the batch lists, one CTA per
+ *   (view, tile) in tile_order (b200_blend_tile_order over the B * T bins, required); a view whose view_isect is < 1 takes
+ *   the empty-render branch (background, final_Ts = 0, alpha = 1).  The deterministic backward's ws is
+ *   b200_blend_backward_deterministic_ws_bytes(B * N, M, block_width) bytes. */
+B200_API int b200_fused_preprocess_forward_views(int num_views, int num_points, const float *means,
+                                                 const float *log_scales, const float *quats, const float *opacity_logit,
+                                                 const float *sh_dc, const float *sh_rest, int sh_bases,
+                                                 int degrees_to_use, const float *viewmats, const float *cam_pos,
+                                                 const float *lin_vel, const float *ang_vel, const float *intrinsics,
+                                                 float rolling_shutter_time, float exposure_time, unsigned img_height,
+                                                 unsigned img_width, unsigned block_width, float clip_thresh,
+                                                 void *packed, float *depths, int32_t *radii, int32_t *num_tiles_hit,
+                                                 void *stream);
+B200_API int b200_fused_preprocess_backward_views(
+    int num_views, int num_points, const float *means, const float *log_scales, const float *quats,
+    const float *opacity_logit, const float *sh_dc, const float *sh_rest, int sh_bases, int degrees_to_use,
+    const float *viewmats, const float *cam_pos, const float *lin_vel, const float *ang_vel, const float *intrinsics,
+    float rolling_shutter_time, float exposure_time, unsigned img_height, unsigned img_width, unsigned block_width,
+    float clip_thresh, const void *packed, const int32_t *radii, const float *v_xy, const float *v_pix_vel,
+    const float *v_conic, const float *v_colors, const float *v_opacity, float *g_means, float *g_log_scales,
+    float *g_quats, float *g_opacity_logit, float *g_sh_dc, float *g_sh_rest, float *g_lin_vel, float *g_ang_vel,
+    float *g_viewmat, void *stream);
+B200_API size_t b200_fused_preprocess_backward_views_ws_bytes(int num_views, int num_points);
+B200_API int b200_fused_preprocess_backward_views_deterministic(
+    int num_views, int num_points, const float *means, const float *log_scales, const float *quats,
+    const float *opacity_logit, const float *sh_dc, const float *sh_rest, int sh_bases, int degrees_to_use,
+    const float *viewmats, const float *cam_pos, const float *lin_vel, const float *ang_vel, const float *intrinsics,
+    float rolling_shutter_time, float exposure_time, unsigned img_height, unsigned img_width, unsigned block_width,
+    float clip_thresh, const void *packed, const int32_t *radii, const float *v_xy, const float *v_pix_vel,
+    const float *v_conic, const float *v_colors, const float *v_opacity, float *g_means, float *g_log_scales,
+    float *g_quats, float *g_opacity_logit, float *g_sh_dc, float *g_sh_rest, float *g_lin_vel, float *g_ang_vel,
+    float *g_viewmat, void *ws, size_t ws_bytes, void *stream);
+B200_API size_t b200_bin_cull_views_ws_bytes(int num_views, int num_points);
+B200_API int b200_bin_cull_count_views(int num_views, int num_points, const void *packed, const float *depths,
+                                       const int32_t *radii, const int32_t *num_tiles_hit, unsigned img_height,
+                                       unsigned img_width, unsigned block_width, unsigned n_blur_samples,
+                                       float rolling_shutter_time, float exposure_time, void *ws_g, size_t ws_g_bytes,
+                                       int32_t *totals_host_pinned, int32_t *view_isect, const int32_t *flag_dev,
+                                       void *stream);
+B200_API int b200_bin_cull_emit_views(int num_views, int num_points, int num_entries, const void *packed,
+                                      const int32_t *radii, const int32_t *num_tiles_hit, unsigned img_height,
+                                      unsigned img_width, unsigned block_width, unsigned n_blur_samples,
+                                      float rolling_shutter_time, float exposure_time, const void *ws_g, void *ws_e,
+                                      size_t ws_e_bytes, int32_t *gaussian_ids_sorted, int32_t *tile_bins, void *stream);
+B200_API int b200_blend_forward_views(int num_views, unsigned img_height, unsigned img_width, unsigned block_width,
+                                      unsigned n_blur_samples, const int32_t *gaussian_ids_sorted,
+                                      const int32_t *tile_bins, const void *packed, float rolling_shutter_time,
+                                      float exposure_time, const float *background, const int32_t *view_isect,
+                                      const int32_t *tile_order, float *out_img, float *final_Ts, int32_t *final_idx,
+                                      float *out_alpha, void *stream);
+B200_API int b200_blend_backward_views(int num_views, int num_records, unsigned img_height, unsigned img_width,
+                                       unsigned block_width, unsigned n_blur_samples, const int32_t *gaussian_ids_sorted,
+                                       const int32_t *tile_bins, const void *packed, float rolling_shutter_time,
+                                       float exposure_time, const float *background, const float *final_Ts,
+                                       const int32_t *final_idx, const float *v_output, const float *v_output_alpha,
+                                       const int32_t *tile_order, float *v_xy, float *v_xy_abs, float *v_pix_vels,
+                                       float *v_conic, float *v_colors, float *v_opacity, int outputs_are_zero,
+                                       void *stream);
+B200_API int b200_blend_backward_views_deterministic(int num_views, int num_records, int num_entries,
+                                                     unsigned img_height, unsigned img_width, unsigned block_width,
+                                                     unsigned n_blur_samples, const int32_t *gaussian_ids_sorted,
+                                                     const int32_t *tile_bins, const void *packed,
+                                                     float rolling_shutter_time, float exposure_time,
+                                                     const float *background, const float *final_Ts,
+                                                     const int32_t *final_idx, const float *v_output,
+                                                     const float *v_output_alpha, const int32_t *tile_order, void *ws,
+                                                     size_t ws_bytes, float *v_xy, float *v_xy_abs, float *v_pix_vels,
+                                                     float *v_conic, float *v_colors, float *v_opacity, void *stream);
+
 /* ---- N-channel blend (no blur), fp16 accumulators like the reference ----------------------
  * replaces nd_rasterize_forward_tensor / nd_rasterize_backward_tensor (bindings.h:129-166,
  * bindings.cu:506-682; kernels forward.cu:185-304, backward.cu:22-141). */
