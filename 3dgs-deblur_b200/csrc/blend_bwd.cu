@@ -573,10 +573,10 @@ struct DetBwdLayout {
     size_t slots, slot_bytes, keys_a, keys_b, pos_a, pos_sorted, seg, cub, cub_bytes, total;
 };
 
-static DetBwdLayout det_bwd_layout(int n, int m, int warps) {
+static DetBwdLayout det_bwd_layout(int n, int m, int warps, int values = RED_VALUES) {
     DetBwdLayout L;
     WsCarver ws;
-    L.slot_bytes = (size_t)m * warps * RED_VALUES * sizeof(float);
+    L.slot_bytes = (size_t)m * warps * values * sizeof(float);
     L.slots = ws.take(L.slot_bytes);
     L.keys_a = ws.take(4 * (size_t)m); L.keys_b = ws.take(4 * (size_t)m);
     L.pos_a = ws.take(4 * (size_t)m); L.pos_sorted = ws.take(4 * (size_t)m);
@@ -585,6 +585,199 @@ static DetBwdLayout det_bwd_layout(int n, int m, int warps) {
     L.cub = ws.take(L.cub_bytes);
     L.total = ws.off;
     return L;
+}
+
+// ---- backward of the one-channel static depth blend (blend_fwd.cu: blend_depth_forward_kernel) ------------------------
+// blend_backward_kernel's walk at S = 1 (tau = 0, no background, no alpha cotangent) with the record's depth as the only
+// colour: back to front from the static pass's final_T / final_idx with cotangent v_D (H,W).  7 per-Gaussian sums per
+// warp visit (xy 2, conic 3, opacity 1, depth 1; no |xy| or velocity sums: tau = 0 makes the latter exactly 0), reduced
+// by a transposing butterfly that leaves sum k on lane 4k.  Pixels that fail a test skip the visit by branching, so a
+// non-finite v_D at a pixel nothing was blended into reaches no gradient.  PPL pixels per lane as in the forward.
+constexpr int DEPTH_RED_VALUES = 7;
+
+struct DepthBwdParams {
+    BlendGeom g;  // rs_time = exposure = 0
+    const int32_t *ids_sorted;
+    const int2 *tile_bins;
+    const int32_t *tile_order;  // or null: raster order
+    const PackedGaussian *packed;
+    const float *final_T;       // (views * H, W) of the depth forward
+    const int32_t *final_idx;
+    const float *v_D;           // (views * H, W)
+    float *v_xy, *v_conic, *v_opac, *v_depth;
+    float *slots;               // DET: the 7 sums of each warp visit at (list position, warp)
+    int views;
+};
+
+// depth sum k (butterfly8 lane 4k) -> destination array and row stride
+__device__ __forceinline__ float *depth_grad_dst(int k, const DepthBwdParams &p, int &stride) {
+    stride = k < 2 ? 2 : k < 5 ? 3 : 1;
+    return k < 2 ? p.v_xy + k : k < 5 ? p.v_conic + (k - 2) : k == 5 ? p.v_opac : p.v_depth;
+}
+
+// Sum 8 per-lane values across the warp; lane L returns the total of value (L >> 2) & 7.
+__device__ __forceinline__ float butterfly8(const float (&v)[8], int lane) {
+    float w4[4], w2[2], w1;
+    bool up = lane & 16;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const float send = up ? v[i] : v[i + 4], keep = up ? v[i + 4] : v[i];
+        w4[i] = keep + __shfl_xor_sync(0xffffffffu, send, 16);
+    }
+    up = lane & 8;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+        const float send = up ? w4[i] : w4[i + 2], keep = up ? w4[i + 2] : w4[i];
+        w2[i] = keep + __shfl_xor_sync(0xffffffffu, send, 8);
+    }
+    up = lane & 4;
+    {
+        const float send = up ? w2[0] : w2[1], keep = up ? w2[1] : w2[0];
+        w1 = keep + __shfl_xor_sync(0xffffffffu, send, 4);
+    }
+    w1 += __shfl_xor_sync(0xffffffffu, w1, 2);
+    w1 += __shfl_xor_sync(0xffffffffu, w1, 1);
+    return w1;
+}
+
+template <int PPL, bool DET>
+__global__ void __launch_bounds__(BLEND_THREADS / PPL) blend_depth_backward_kernel(const DepthBwdParams p) {
+    constexpr int NT = BLEND_THREADS / PPL;
+    __shared__ __align__(128) PackedGaussian s_rec[BLEND_STAGES][BLEND_BATCH];
+    __shared__ __align__(8) uint64_t s_bar[BLEND_STAGES];
+    __shared__ int s_max[NT / 32];
+
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    int view, tile;
+    cta_tile(p.tile_order, p.g, view, tile);
+    const int tile_x = tile % p.g.tbx, tile_y = tile / p.g.tbx;
+    const int2 range = p.tile_bins[view * (p.g.tbx * p.g.tby) + tile];
+
+    bool inside[PPL];
+    float px[PPL], py[PPL], roll[PPL], Tm[PPL], Dr[PPL], vd[PPL];
+    int bin_final[PPL];
+    int my_max = -1;
+#pragma unroll
+    for (int q = 0; q < PPL; ++q) {
+        int lx, ly;
+        bool has_pixel = true;
+        if (PPL == 2) tile_pixel_pair(tid, q, lx, ly); else tile_pixel(p.g.bw, tid, lx, ly, has_pixel);
+        const int j = tile_x * p.g.bw + lx, i = tile_y * p.g.bw + ly;
+        inside[q] = has_pixel && i < p.g.H && j < p.g.W;
+        px[q] = (float)j + 0.5f; py[q] = (float)i + 0.5f; roll[q] = 0.f;
+        Tm[q] = 1.f; Dr[q] = 0.f; vd[q] = 0.f; bin_final[q] = -1;  // Dr: -sum_behind(fac * depth * v_D)
+        if (inside[q]) {
+            const size_t pix = (size_t)(view * p.g.H + i) * p.g.W + j;
+            Tm[q] = p.final_T[pix];
+            vd[q] = p.v_D[pix];
+            bin_final[q] = min(p.final_idx[pix], range.y - 1);
+            my_max = max(my_max, bin_final[q]);
+        }
+    }
+    const int wmax = __reduce_max_sync(0xffffffffu, my_max);
+    if (lane == 0) s_max[warp] = wmax;
+    const WarpWindow win = warp_window<PPL>(inside, px, py, roll);
+
+    init_stages(s_bar, tid);
+    int hi = -1;
+#pragma unroll
+    for (int w = 0; w < NT / 32; ++w) hi = max(hi, s_max[w]);
+    const int total = hi - range.x + 1;
+    const int nb = total > 0 ? (total + BLEND_BATCH - 1) / BLEND_BATCH : 0;
+
+    int my_stride;
+    float *const my_dst = ((lane & 3) == 0 && (lane >> 2) < DEPTH_RED_VALUES) ? depth_grad_dst(lane >> 2, p, my_stride) : nullptr;
+    auto issue = [&](int b) {
+        const int top = hi - b * BLEND_BATCH;
+        issue_batch<NT, -1>(s_rec, s_bar, b, tid, p.ids_sorted, p.packed, top, min(BLEND_BATCH, top - range.x + 1));
+    };
+
+    if (nb > 0) issue(0);
+    for (int b = 0; b < nb; ++b) {
+        const int st = b & 1;
+        if (b + 1 < nb) issue(b + 1);
+        wait_batch(s_bar, b);
+        const int top = hi - b * BLEND_BATCH;
+        const int cnt = min(BLEND_BATCH, top - range.x + 1);
+        if (wmax >= range.x) {
+            for (int c0 = 0; c0 < cnt; c0 += 32) {
+                const int e = c0 + lane;
+                const unsigned my_mask =
+                    ((e < cnt) && (top - e <= wmax)) ? sample_mask_exact<1>(s_rec[st][e], win, 0.f) : 0u;
+                unsigned m = __ballot_sync(0xffffffffu, my_mask != 0u);
+                while (m) {
+                    const int k = c0 + __ffs(m) - 1;
+                    m &= m - 1;
+                    const int idx = top - k;
+                    const float4 A = *reinterpret_cast<const float4 *>(&s_rec[st][k].x);    // x y vx vy
+                    const float4 Bq = *reinterpret_cast<const float4 *>(&s_rec[st][k].ca);  // a b c opac
+                    const float cut = s_rec[st][k].thr + 1e-4f;
+                    const float depth = s_rec[st][k].depth;
+                    const SigmaEntry se = sigma_entry(A, Bq);
+                    float gxs = 0.f, gys = 0.f, sxx = 0.f, sxy = 0.f, syy = 0.f, vop = 0.f, vdep = 0.f;
+                    bool any = false;
+#pragma unroll
+                    for (int q = 0; q < PPL; ++q) {
+                        if (idx > bin_final[q]) continue;
+                        float dx, dy, sigma;
+                        sigma_eval(se, A.x - px[q], A.y - py[q], 0.f, dx, dy, sigma);
+                        if (sigma > cut || sigma < 0.f) continue;  // backward.cu:252-254,276
+                        const float vis = exp_neg_approx(sigma);
+                        const float ov = Bq.w * vis;
+                        const float alpha = fminf(0.99f, ov);
+                        if (alpha < 1.f / 255.f) continue;
+                        any = true;
+                        const float ra = rcp_approx(1.f - alpha);
+                        const float Tn = Tm[q] * ra;
+                        const float fac = alpha * Tn;
+                        const float cdot = depth * vd[q];
+                        const float v_alpha = Tn * cdot + ra * Dr[q];  // backward.cu:303-311
+                        const float v_sigma = -ov * v_alpha;
+                        Tm[q] = Tn;
+                        Dr[q] = Dr[q] - fac * cdot;
+                        vdep += fac * vd[q];
+                        const float u = v_sigma * dx, w = v_sigma * dy;
+                        sxx += u * dx; sxy += u * dy; syy += w * dy;
+                        gxs += Bq.x * u + Bq.y * w;
+                        gys += Bq.y * u + Bq.z * w;
+                        vop += vis * v_alpha;
+                    }
+                    if (!__any_sync(0xffffffffu, any)) continue;
+                    const float v[8] = {gxs, gys, 0.5f * sxx, sxy, 0.5f * syy, vop, vdep, 0.f};
+                    const float tot = butterfly8(v, lane);
+                    if constexpr (DET) {
+                        if (my_dst) p.slots[((size_t)idx * (NT / 32) + warp) * DEPTH_RED_VALUES + (lane >> 2)] = tot;
+                    } else if (my_dst && tot != 0.f) {
+                        atomicAdd(my_dst + (unsigned)s_rec[st][k].id * (unsigned)my_stride, tot);  // N * 3 < 2^32
+                    }
+                }
+            }
+        }
+        __syncthreads();  // stage `st` is refilled two batches from now
+    }
+}
+
+// deterministic mode: 8 threads per Gaussian, thread k < 7 sums value k over the Gaussian's slots in ascending list
+// position, then ascending warp, and overwrites its output (det_reduce_kernel's order)
+__global__ void __launch_bounds__(256) depth_det_reduce_kernel(int num_points, int warps, const float *__restrict__ slots,
+                                                               const int32_t *__restrict__ pos_sorted,
+                                                               const int2 *__restrict__ seg, const DepthBwdParams p) {
+    const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const int g = (int)(t >> 3), k = (int)(t & 7);
+    if (g >= num_points || k >= DEPTH_RED_VALUES) return;
+    int stride;
+    float *const dst = depth_grad_dst(k, p, stride);
+    const int2 r = seg[g];
+    float acc = 0.f;
+    for (int i = r.x; i < r.y; ++i) {
+        const float *s = slots + (size_t)__ldg(pos_sorted + i) * warps * DEPTH_RED_VALUES + k;
+        for (int w = 0; w < warps; ++w) acc += s[w * DEPTH_RED_VALUES];
+    }
+    dst[(size_t)g * stride] = acc;
+}
+
+static int depth_bwd_warps(unsigned block_width) {
+    return (block_width == 16 && !blend_force_one_pixel(true)) ? BLEND_THREADS / 2 / 32 : BLEND_THREADS / 32;
 }
 
 }  // namespace b200
@@ -796,4 +989,108 @@ extern "C" int b200_rasterize_backward(int num_points, unsigned img_height, unsi
     return run_blend_backward(num_points, img_height, img_width, block_width, n_blur_samples, gaussian_ids_sorted,
                               tile_bins, packed_ws, rolling_shutter_time, exposure_time, background, final_Ts, final_idx,
                               v_output, v_output_alpha, v_xy, v_xy_abs, v_pix_vels, v_conic, v_colors, v_opacity, false, st);
+}
+
+// Shared argument checks and launch of the depth backward; slots != null: the DET kernels
+static int run_depth_backward(int num_views, int num_records, unsigned img_height, unsigned img_width,
+                              unsigned block_width, const int32_t *gaussian_ids_sorted, const int32_t *tile_bins,
+                              const void *packed, const float *final_T, const int32_t *final_idx, const float *v_depth_img,
+                              const int32_t *tile_order, float *v_xy, float *v_conic, float *v_opacity, float *v_depth,
+                              float *slots, cudaStream_t st, DepthBwdParams &p) {
+    B200_REQUIRE(num_views >= 1, "num_views must be >= 1");
+    B200_REQUIRE(num_records >= 1, "num_records must be >= 1");
+    B200_REQUIRE(block_width > 1 && block_width <= 16, "block_width must be between 2 and 16");
+    B200_REQUIRE(img_height > 0 && img_width > 0, "image size must be positive");
+    const long long tiles = (long long)((img_width + block_width - 1) / block_width) * ((img_height + block_width - 1) / block_width);
+    B200_REQUIRE((long long)num_views * tiles < 0x7fffffffll && (long long)num_views * img_height < 0x7fffffffll,
+                 "num_views * tiles exceeds int32");
+    B200_REQUIRE(tile_bins && packed && aligned16(packed), "null / misaligned input pointer");
+    B200_REQUIRE(final_T && final_idx && v_depth_img, "null saved / cotangent pointer");
+    B200_REQUIRE(v_xy && v_conic && v_opacity && v_depth, "null output pointer");
+    p.g = blend_geom(img_height, img_width, block_width, 0.f, 0.f);
+    p.ids_sorted = gaussian_ids_sorted;
+    p.tile_bins = reinterpret_cast<const int2 *>(tile_bins);
+    p.tile_order = tile_order;
+    p.packed = reinterpret_cast<const PackedGaussian *>(packed);
+    p.final_T = final_T; p.final_idx = final_idx; p.v_D = v_depth_img;
+    p.v_xy = v_xy; p.v_conic = v_conic; p.v_opac = v_opacity; p.v_depth = v_depth;
+    p.slots = slots;
+    p.views = num_views;
+    if (!slots) B200_CUDA(cudaMemsetAsync(v_depth, 0, sizeof(float) * (size_t)num_records, st));  // atomics add into it
+    const int ctas = (int)(num_views * tiles);
+    const bool paired = depth_bwd_warps(block_width) == BLEND_THREADS / 2 / 32;
+    if (paired) {
+        if (slots) blend_depth_backward_kernel<2, true><<<ctas, BLEND_THREADS / 2, 0, st>>>(p);
+        else blend_depth_backward_kernel<2, false><<<ctas, BLEND_THREADS / 2, 0, st>>>(p);
+    } else {
+        if (slots) blend_depth_backward_kernel<1, true><<<ctas, BLEND_THREADS, 0, st>>>(p);
+        else blend_depth_backward_kernel<1, false><<<ctas, BLEND_THREADS, 0, st>>>(p);
+    }
+    B200_LAUNCH_CHECK();
+    return B200_OK;
+}
+
+extern "C" int b200_blend_depth_backward(int num_views, int num_records, unsigned img_height, unsigned img_width,
+                                         unsigned block_width, const int32_t *gaussian_ids_sorted,
+                                         const int32_t *tile_bins, const void *packed, const float *final_T,
+                                         const int32_t *final_idx, const float *v_depth_img, const int32_t *tile_order,
+                                         float *v_xy, float *v_conic, float *v_opacity, float *v_depth, void *stream) {
+    DepthBwdParams p;
+    return run_depth_backward(num_views, num_records, img_height, img_width, block_width, gaussian_ids_sorted, tile_bins,
+                              packed, final_T, final_idx, v_depth_img, tile_order, v_xy, v_conic, v_opacity, v_depth,
+                              nullptr, as_stream(stream), p);
+}
+
+extern "C" size_t b200_blend_depth_backward_deterministic_ws_bytes(int num_records, int num_entries,
+                                                                   unsigned block_width) {
+    if (num_records < 1 || num_entries < 0) return 0;
+    return det_bwd_layout(num_records, num_entries, depth_bwd_warps(block_width), DEPTH_RED_VALUES).total;
+}
+
+extern "C" int b200_blend_depth_backward_deterministic(int num_views, int num_records, int num_entries,
+                                                       unsigned img_height, unsigned img_width, unsigned block_width,
+                                                       const int32_t *gaussian_ids_sorted, const int32_t *tile_bins,
+                                                       const void *packed, const float *final_T,
+                                                       const int32_t *final_idx, const float *v_depth_img,
+                                                       const int32_t *tile_order, void *ws, size_t ws_bytes,
+                                                       float *v_xy, float *v_conic, float *v_opacity, float *v_depth,
+                                                       void *stream) {
+    B200_REQUIRE(num_records >= 1, "num_records must be >= 1");
+    B200_REQUIRE(num_entries >= 0, "num_entries must be >= 0");
+    B200_REQUIRE(num_entries == 0 || gaussian_ids_sorted, "null gaussian_ids_sorted");
+    B200_REQUIRE(ws && (reinterpret_cast<uintptr_t>(ws) & 255u) == 0, "ws must be a 256-byte aligned workspace");
+    const int warps = depth_bwd_warps(block_width);
+    const DetBwdLayout L = det_bwd_layout(num_records, num_entries, warps, DEPTH_RED_VALUES);
+    B200_REQUIRE(ws_bytes >= L.total,
+                 "ws too small: %zu bytes, b200_blend_depth_backward_deterministic_ws_bytes gives %zu", ws_bytes, L.total);
+    cudaStream_t st = as_stream(stream);
+    char *base = static_cast<char *>(ws);
+    float *slots = reinterpret_cast<float *>(base + L.slots);
+    const int32_t *pos_sorted = reinterpret_cast<const int32_t *>(base + L.pos_sorted);
+    int2 *seg = reinterpret_cast<int2 *>(base + L.seg);
+    DepthBwdParams p;
+    B200_CUDA(cudaMemsetAsync(seg, 0, 8 * (size_t)num_records, st));
+    if (num_entries > 0) {
+        B200_CUDA(cudaMemsetAsync(slots, 0, L.slot_bytes, st));  // slots no warp visits read as zero
+        int rc = run_depth_backward(num_views, num_records, img_height, img_width, block_width, gaussian_ids_sorted,
+                                    tile_bins, packed, final_T, final_idx, v_depth_img, tile_order, v_xy, v_conic,
+                                    v_opacity, v_depth, slots, st, p);
+        if (rc) return rc;
+        uint32_t *keys_a = reinterpret_cast<uint32_t *>(base + L.keys_a);
+        int32_t *pos_a = reinterpret_cast<int32_t *>(base + L.pos_a);
+        det_keys_kernel<<<ceil_div(num_entries, 256), 256, 0, st>>>(num_entries, num_records, gaussian_ids_sorted, nullptr,
+                                                                    keys_a, pos_a);
+        B200_LAUNCH_CHECK();
+        rc = sort_to_bins(num_entries, std::max(1, key_end_bit(num_records + 1) - 32), num_records, keys_a,
+                          reinterpret_cast<uint32_t *>(base + L.keys_b), pos_a, const_cast<int32_t *>(pos_sorted),
+                          reinterpret_cast<int32_t *>(seg), base + L.cub, L.cub_bytes, st);
+        if (rc) return rc;
+    } else {
+        B200_REQUIRE(v_xy && v_conic && v_opacity && v_depth, "null output pointer");
+        p.v_xy = v_xy; p.v_conic = v_conic; p.v_opac = v_opacity; p.v_depth = v_depth;
+    }
+    depth_det_reduce_kernel<<<(unsigned)(((long long)num_records * 8 + 255) / 256), 256, 0, st>>>(
+        num_records, warps, slots, pos_sorted, seg, p);
+    B200_LAUNCH_CHECK();
+    return B200_OK;
 }

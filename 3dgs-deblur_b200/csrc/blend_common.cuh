@@ -80,7 +80,7 @@ __device__ __forceinline__ PackedGaussian make_record(int id, float x, float y, 
     g.ca = ca; g.cb = cb; g.cc = cc; g.opac = opac;
     g.r = r; g.g = g_; g.b = b;
     g.id = id;
-    g.pad = 0.f;
+    g.depth = 0.f;
     const float thr = logf(255.f * g.opac);  // opac <= 0 -> -inf / NaN
     g.thr = thr;
     // a*c - b*b cancels for needle-shaped splats (eigenvalue ratio ~1e5 at 45 degrees loses two digits in fp32, which
@@ -104,7 +104,7 @@ __device__ __forceinline__ void store_record(PackedGaussian *dst, const PackedGa
     o[0] = make_float4(g.x, g.y, g.vx, g.vy);
     o[1] = make_float4(g.ca, g.cb, g.cc, g.opac);
     o[2] = make_float4(g.r, g.g, g.b, g.thr);
-    o[3] = make_float4(g.hx, g.hy, __int_as_float(g.id), 0.f);
+    o[3] = make_float4(g.hx, g.hy, __int_as_float(g.id), g.depth);
 }
 
 static __global__ void __launch_bounds__(256) pack_records_kernel(int n, const float2 *__restrict__ xys,

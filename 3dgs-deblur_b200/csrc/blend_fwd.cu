@@ -432,6 +432,131 @@ static __global__ void __launch_bounds__(ORDER_THREADS) tile_order_kernel(int n,
     for (int t = tid; t < n; t += ORDER_THREADS) order[atomicAdd(&s_off[bucket(len(t))], 1)] = t;
 }
 
+// ---- one-channel static depth blend (splatfacto.py:881-897: the second rasterize call with the depths as colours) ----
+// D = sum_i depth_i alpha_i T_i at S = 1, no rolling shutter, zero background, the depth read from the record's depth
+// word.  PPL pixels per lane: 2 on 16x16 tiles (the pixel mapping of blend_forward_kernel2), 1 otherwise (that of
+// blend_forward_kernel).  Each pixel's arithmetic is blend_forward_kernel2's at S = 1 with one channel, written with the
+// same explicitly rounded operations (the one-pixel kernel's contracted `acc += c * vis` is the same FMA), and the alpha,
+// T, cull and stop decisions are the same: D is bit for bit channel 0 of the three-channel blend of records recoloured
+// with the depths.  final_T / final_idx (null when no backward follows) are that pass's final_Ts / final_idx.
+struct DepthFwdParams {
+    BlendGeom g;  // rs_time = exposure = 0
+    const int32_t *ids_sorted;
+    const int2 *tile_bins;
+    const int32_t *tile_order;  // or null: raster order
+    const PackedGaussian *packed;
+    const int32_t *ref_isect;   // DEVICE int32[views] or null, as in BlendFwdParams
+    int views;
+    float *out_depth;           // (views * H, W)
+    float *final_T;             // (views * H, W) or null
+    int32_t *final_idx;         // (views * H, W) or null
+};
+
+template <int PPL>
+__global__ void __launch_bounds__(BLEND_THREADS / PPL) blend_depth_forward_kernel(const DepthFwdParams p) {
+    constexpr int NT = BLEND_THREADS / PPL;
+    __shared__ __align__(128) PackedGaussian s_rec[BLEND_STAGES][BLEND_BATCH];
+    __shared__ __align__(8) uint64_t s_bar[BLEND_STAGES];
+
+    const int tid = threadIdx.x, lane = tid & 31;
+    int view, tile;
+    cta_tile(p.tile_order, p.g, view, tile);
+    const int tile_x = tile % p.g.tbx, tile_y = tile / p.g.tbx;
+    bool inside[PPL];
+    float px[PPL], py[PPL], roll[PPL];
+    size_t pix[PPL];
+#pragma unroll
+    for (int q = 0; q < PPL; ++q) {
+        int lx, ly;
+        bool has_pixel = true;
+        if (PPL == 2) tile_pixel_pair(tid, q, lx, ly); else tile_pixel(p.g.bw, tid, lx, ly, has_pixel);
+        const int j = tile_x * p.g.bw + lx, i = tile_y * p.g.bw + ly;
+        inside[q] = has_pixel && i < p.g.H && j < p.g.W;
+        px[q] = (float)j + 0.5f; py[q] = (float)i + 0.5f;
+        roll[q] = (float)((double)p.g.rs_time * ((double)(py[q] / (float)p.g.H) - 0.5));
+        pix[q] = (size_t)(view * p.g.H + i) * p.g.W + j;
+    }
+    if (p.ref_isect && __ldg(p.ref_isect + view) < 1) {  // block-uniform: the empty render's zero background
+#pragma unroll
+        for (int q = 0; q < PPL; ++q) {
+            if (!inside[q]) continue;
+            p.out_depth[pix[q]] = 0.f;
+            if (p.final_T) { p.final_T[pix[q]] = 0.f; p.final_idx[pix[q]] = 0; }
+        }
+        return;
+    }
+    const WarpWindow win = warp_window<PPL>(inside, px, py, roll);
+    const int2 range = p.tile_bins[view * (p.g.tbx * p.g.tby) + tile];
+    const int nb = (range.y - range.x + BLEND_BATCH - 1) / BLEND_BATCH;
+
+    init_stages(s_bar, tid);
+    auto issue = [&](int b) {
+        const int start = range.x + b * BLEND_BATCH;
+        issue_batch<NT, 1>(s_rec, s_bar, b, tid, p.ids_sorted, p.packed, start, min(BLEND_BATCH, range.y - start));
+    };
+
+    float T[PPL], acc[PPL];
+    int last[PPL];
+    bool alive[PPL];
+#pragma unroll
+    for (int q = 0; q < PPL; ++q) { T[q] = 1.f; acc[q] = 0.f; last[q] = 0; alive[q] = inside[q]; }
+    bool walive = __any_sync(0xffffffffu, alive[0] || alive[PPL - 1]);
+
+    int b = 0;
+    bool pending = false;
+    if (nb > 0) { issue(0); pending = true; }
+    for (; b < nb; ++b) {
+        const int st = b & 1;
+        if (b + 1 < nb) issue(b + 1);
+        wait_batch(s_bar, b);
+        pending = (b + 1 < nb);
+        const int start = range.x + b * BLEND_BATCH;
+        const int cnt = min(BLEND_BATCH, range.y - start);
+        if (walive) {
+            for (int c0 = 0; c0 < cnt; c0 += 32) {
+                const int e = c0 + lane;
+                const unsigned my_mask = (e < cnt) ? sample_mask_exact<1>(s_rec[st][e], win, 0.f) : 0u;
+                unsigned m = __ballot_sync(0xffffffffu, my_mask != 0u);
+                while (m) {
+                    const int k = c0 + __ffs(m) - 1;
+                    m &= m - 1;
+                    const float4 A = *reinterpret_cast<const float4 *>(&s_rec[st][k].x);    // x y vx vy
+                    const float4 Bq = *reinterpret_cast<const float4 *>(&s_rec[st][k].ca);  // a b c opac
+                    const float cut = s_rec[st][k].thr + 1e-4f;
+                    const float depth = s_rec[st][k].depth;
+                    const float ha = 0.5f * Bq.x, hc = 0.5f * Bq.z;
+#pragma unroll
+                    for (int q = 0; q < PPL; ++q) {
+                        if (!alive[q]) continue;
+                        const float tau = 0.f + roll[q];
+                        const float dx = __fmaf_rn(tau, A.z, __fsub_rn(A.x, px[q]));
+                        const float dy = __fmaf_rn(tau, A.w, __fsub_rn(A.y, py[q]));
+                        const float sigma = __fmaf_rn(dx, __fmaf_rn(ha, dx, __fmul_rn(Bq.y, dy)), __fmul_rn(__fmul_rn(hc, dy), dy));
+                        if (sigma > cut || sigma < 0.f) continue;
+                        const float alpha = fminf(0.999f, __fmul_rn(Bq.w, exp_neg_approx(sigma)));
+                        if (alpha < 1.f / 255.f) continue;
+                        const float next_T = __fmul_rn(T[q], __fsub_rn(1.f, alpha));
+                        if (next_T <= 1e-4f) { alive[q] = false; continue; }  // forward.cu:421-427
+                        acc[q] = __fmaf_rn(depth, __fmul_rn(alpha, T[q]), acc[q]);
+                        T[q] = next_T;
+                        last[q] = start + k;
+                    }
+                }
+                walive = __any_sync(0xffffffffu, alive[0] || alive[PPL - 1]);
+                if (!walive) c0 = cnt;
+            }
+        }
+        if (!__syncthreads_or(walive)) { ++b; break; }  // stage `st` is refilled two batches from now + early exit
+    }
+    if (pending && b < nb) wait_batch(s_bar, b);  // drain the prefetch before exit
+#pragma unroll
+    for (int q = 0; q < PPL; ++q) {
+        if (!inside[q]) continue;
+        p.out_depth[pix[q]] = acc[q];
+        if (p.final_T) { p.final_T[pix[q]] = T[q]; p.final_idx[pix[q]] = last[q]; }
+    }
+}
+
 }  // namespace b200
 
 using namespace b200;
@@ -574,6 +699,38 @@ extern "C" int b200_set_record_colors(int num_points, const float *colors, void 
     B200_REQUIRE(colors && packed && aligned16(packed), "null / misaligned pointer");
     b200::set_record_colors_kernel<<<ceil_div(num_points, 256), 256, 0, as_stream(stream)>>>(
         num_points, colors, reinterpret_cast<PackedGaussian *>(packed));
+    B200_LAUNCH_CHECK();
+    return B200_OK;
+}
+
+extern "C" int b200_blend_depth_forward(int num_views, unsigned img_height, unsigned img_width, unsigned block_width,
+                                        const int32_t *gaussian_ids_sorted, const int32_t *tile_bins, const void *packed,
+                                        const int32_t *view_isect, const int32_t *tile_order, float *out_depth,
+                                        float *final_T, int32_t *final_idx, void *stream) {
+    B200_REQUIRE(num_views >= 1, "num_views must be >= 1");
+    B200_REQUIRE(block_width > 1 && block_width <= 16, "block_width must be between 2 and 16");
+    B200_REQUIRE(img_height > 0 && img_width > 0, "image size must be positive");
+    const long long tiles = (long long)((img_width + block_width - 1) / block_width) * ((img_height + block_width - 1) / block_width);
+    B200_REQUIRE((long long)num_views * tiles < 0x7fffffffll && (long long)num_views * img_height < 0x7fffffffll,
+                 "num_views * tiles exceeds int32");
+    B200_REQUIRE(tile_bins && packed && aligned16(packed), "null / misaligned input pointer");
+    B200_REQUIRE(out_depth, "null output pointer");
+    B200_REQUIRE((final_T == nullptr) == (final_idx == nullptr), "final_T and final_idx go together");
+    DepthFwdParams p;
+    p.g = blend_geom(img_height, img_width, block_width, 0.f, 0.f);
+    p.ids_sorted = gaussian_ids_sorted;
+    p.tile_bins = reinterpret_cast<const int2 *>(tile_bins);
+    p.tile_order = tile_order;
+    p.packed = reinterpret_cast<const PackedGaussian *>(packed);
+    p.ref_isect = view_isect;
+    p.views = num_views;
+    p.out_depth = out_depth; p.final_T = final_T; p.final_idx = final_idx;
+    const int ctas = (int)(num_views * tiles);
+    cudaStream_t st = as_stream(stream);
+    if (block_width == 16 && !blend_force_one_pixel(false))
+        blend_depth_forward_kernel<2><<<ctas, BLEND_THREADS / 2, 0, st>>>(p);
+    else
+        blend_depth_forward_kernel<1><<<ctas, BLEND_THREADS, 0, st>>>(p);
     B200_LAUNCH_CHECK();
     return B200_OK;
 }

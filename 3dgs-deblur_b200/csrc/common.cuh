@@ -67,7 +67,7 @@ struct __align__(16) PackedGaussian {
     float r, g, b, thr;          // colour, ln(255*opac): sigma above this cannot reach alpha >= 1/255
     float hx, hy;                // half extents of the alpha >= 1/255 ellipse (conservative), +inf if unbounded
     int id;                      // Gaussian index (backward scatters gradients to it)
-    float pad;
+    float depth;                 // view-space depth (fused forward kernels; 0 from pack_records): the depth blend's "colour"
 };
 static_assert(sizeof(PackedGaussian) == 64, "record must be 64 bytes");
 

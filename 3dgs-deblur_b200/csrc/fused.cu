@@ -99,6 +99,7 @@ __global__ void __launch_bounds__(FUSED_THREADS) fused_forward_kernel(FusedParam
         const float opac = sigmoidf_(f.opacity_logit[i]) * r.comp;  // splatfacto.py:853-854 ("antialiased")
         g = make_record(ri, r.xy[0], r.xy[1], r.vel[0], r.vel[1], r.conic[0], r.conic[1], r.conic[2], opac,
                         clamp_colour(c0 + 0.5f), clamp_colour(c1 + 0.5f), clamp_colour(c2 + 0.5f));  // :846
+        g.depth = r.depth;
     } else {
         g = make_record(ri, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f);  // hx = -1: never blended
     }
@@ -125,6 +126,7 @@ struct FusedBwdIO {
     float *g_lin, *g_ang, *g_viewmat;  // optional, pre-zeroed accumulators
     bool gq_al;                        // g_quats is 16-byte aligned
     float *cam_partials;               // DET only: 18 floats per block (cam_partials_sum_kernel)
+    const float *v_depth;              // DEPTH only: the depth blend's per-record depth gradient
 };
 
 // Coalesced store of a block's contiguous chunk of `row`-float rows staged in shared memory with pitch `pitch`.
@@ -145,7 +147,8 @@ __device__ __forceinline__ void add_view(float &a, float x, bool first) { a = fi
 // row is written once.  The camera gradients are per view: io.g_lin / g_ang / g_viewmat + 3 v / 3 v / 12 v.
 // DET: the camera partials of the block are stored to io.cam_partials (18 floats per (view, block)) instead of added to
 // the outputs (deterministic mode).  VIEWS = false: one view (f0.views == 1), the loop and the view sums compile away.
-template <int DEG_USE, bool DET, bool VIEWS>
+// DEPTH: io.v_depth[record] is the projection's depth cotangent (0 otherwise).
+template <int DEG_USE, bool DET, bool VIEWS, bool DEPTH>
 __global__ void __launch_bounds__(FUSED_THREADS) fused_backward_kernel(const FusedParams f0, FusedBwdIO io) {
     constexpr int KU = (DEG_USE + 1) * (DEG_USE + 1);
     extern __shared__ __align__(16) float s_rows[];  // [FUSED_THREADS][pitch] gradient rows of sh_rest
@@ -216,7 +219,7 @@ __global__ void __launch_bounds__(FUSED_THREADS) fused_backward_kernel(const Fus
             ProjGaussCot ct;
             const float2 gxy = reinterpret_cast<const float2 *>(io.v_xy)[ri], gpv = reinterpret_cast<const float2 *>(io.v_pix_vel)[ri];
             ct.v_xy[0] = gxy.x; ct.v_xy[1] = gxy.y; ct.v_pix_vel[0] = gpv.x; ct.v_pix_vel[1] = gpv.y;
-            ct.v_depth = 0.f;
+            if constexpr (DEPTH) ct.v_depth = io.v_depth[ri]; else ct.v_depth = 0.f;
             ct.v_conic[0] = io.v_conic[3 * ri]; ct.v_conic[1] = io.v_conic[3 * ri + 1]; ct.v_conic[2] = io.v_conic[3 * ri + 2];
             ct.v_comp = vo * sg;
             project_backward_one<true>(f.proj, want_cam, io.g_viewmat != nullptr, in, sv, ct, gr);
@@ -410,7 +413,7 @@ extern "C" int b200_fused_colors_forward(int num_points, const float *means, con
 }
 
 // cam_ws != null: deterministic camera sums (b200_fused_preprocess_backward_deterministic).  views / intr: the view batch
-// (1 / null for one camera with the scalar intrinsics).
+// (1 / null for one camera with the scalar intrinsics).  v_depth != null (view batches only): depth cotangents per record.
 static int run_fused_backward(int views, int num_points, const float *means, const float *log_scales, const float *quats,
                               const float *opacity_logit, const float *sh_dc, const float *sh_rest, int sh_bases,
                               int degrees_to_use, const float *viewmat, const float *cam_pos, const float *lin_vel,
@@ -420,7 +423,8 @@ static int run_fused_backward(int views, int num_points, const float *means, con
                               const float *v_xy, const float *v_pix_vel, const float *v_conic, const float *v_colors,
                               const float *v_opacity, float *g_means, float *g_log_scales, float *g_quats,
                               float *g_opacity_logit, float *g_sh_dc, float *g_sh_rest, float *g_lin_vel,
-                              float *g_ang_vel, float *g_viewmat, float *cam_ws, cudaStream_t st) {
+                              float *g_ang_vel, float *g_viewmat, float *cam_ws, cudaStream_t st,
+                              const float *v_depth = nullptr) {
     FusedParams f;
     int rc = fill_fused(f, num_points, means, log_scales, quats, opacity_logit, sh_dc, sh_rest, sh_bases, degrees_to_use,
                         viewmat, cam_pos, lin_vel, ang_vel, rolling_shutter_time, exposure_time, fx, fy, cx, cy, img_height,
@@ -428,6 +432,7 @@ static int run_fused_backward(int views, int num_points, const float *means, con
     if (rc) return rc;
     f.views = views; f.intr = intr;
     B200_REQUIRE(packed && radii && v_xy && v_pix_vel && v_conic && v_colors && v_opacity, "null input pointer");
+    B200_REQUIRE(!v_depth || intr, "depth cotangents need the view-batch entry point");
     B200_REQUIRE(g_means && g_log_scales && g_quats && g_opacity_logit && g_sh_dc && (sh_bases == 1 || g_sh_rest),
                  "null gradient pointer");
     // deterministic camera sums: the blocks store partials and cam_partials_sum_kernel overwrites the outputs
@@ -439,29 +444,29 @@ static int run_fused_backward(int views, int num_points, const float *means, con
     }
     FusedBwdIO io{reinterpret_cast<const PackedGaussian *>(packed), radii, v_xy, v_pix_vel, v_conic, v_colors, v_opacity,
                   g_means, g_log_scales, g_quats, g_opacity_logit, g_sh_dc, g_sh_rest, g_lin_vel, g_ang_vel, g_viewmat,
-                  aligned16(g_quats), cam_ws};
+                  aligned16(g_quats), cam_ws, v_depth};
     const int rest_row = 3 * (sh_bases - 1);
     const int pitch = (rest_row & 1) ? rest_row : rest_row + 1;
     const size_t smem = sizeof(float) * FUSED_THREADS * (size_t)(pitch > 0 ? pitch : 1);
     const int blocks = ceil_div(num_points, FUSED_THREADS);
-    auto launch = [&](auto det_c, auto views_c) {
-        constexpr bool D = decltype(det_c)::value, V = decltype(views_c)::value;
+    auto launch = [&](auto det_c, auto views_c, auto depth_c) {
+        constexpr bool D = decltype(det_c)::value, V = decltype(views_c)::value, Z = decltype(depth_c)::value;
         switch (degrees_to_use) {
-            case 0: fused_backward_kernel<0, D, V><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
-            case 1: fused_backward_kernel<1, D, V><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
-            case 2: fused_backward_kernel<2, D, V><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
-            case 3: fused_backward_kernel<3, D, V><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
-            default: fused_backward_kernel<4, D, V><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
+            case 0: fused_backward_kernel<0, D, V, Z><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
+            case 1: fused_backward_kernel<1, D, V, Z><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
+            case 2: fused_backward_kernel<2, D, V, Z><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
+            case 3: fused_backward_kernel<3, D, V, Z><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
+            default: fused_backward_kernel<4, D, V, Z><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
         }
     };
     using T_ = std::true_type;
     using F_ = std::false_type;
     if (det) {
-        if (intr) launch(T_{}, T_{}); else launch(T_{}, F_{});
+        if (v_depth) launch(T_{}, T_{}, T_{}); else if (intr) launch(T_{}, T_{}, F_{}); else launch(T_{}, F_{}, F_{});
         B200_LAUNCH_CHECK();
         cam_partials_sum_kernel<<<views, 32, 0, st>>>(blocks, cam_ws, g_lin_vel, g_ang_vel, g_viewmat);
     } else {
-        if (intr) launch(F_{}, T_{}); else launch(F_{}, F_{});
+        if (v_depth) launch(F_{}, T_{}, T_{}); else if (intr) launch(F_{}, T_{}, F_{}); else launch(F_{}, F_{}, F_{});
     }
     B200_LAUNCH_CHECK();
     return B200_OK;
@@ -557,4 +562,50 @@ extern "C" int b200_fused_preprocess_backward_views_deterministic(
                               radii, v_xy, v_pix_vel, v_conic, v_colors, v_opacity, g_means, g_log_scales, g_quats,
                               g_opacity_logit, g_sh_dc, g_sh_rest, g_lin_vel, g_ang_vel, g_viewmat,
                               static_cast<float *>(ws), as_stream(stream));
+}
+
+// b200_fused_preprocess_backward_views(_deterministic) with the depth blend's cotangents v_depth (B * N) chained into the
+// projection; one view (B = 1, intrinsics of the camera) gives the single-view gradients.
+extern "C" int b200_fused_preprocess_backward_views_depth(
+    int num_views, int num_points, const float *means, const float *log_scales, const float *quats,
+    const float *opacity_logit, const float *sh_dc, const float *sh_rest, int sh_bases, int degrees_to_use,
+    const float *viewmats, const float *cam_pos, const float *lin_vel, const float *ang_vel, const float *intrinsics,
+    float rolling_shutter_time, float exposure_time, unsigned img_height, unsigned img_width, unsigned block_width,
+    float clip_thresh, const void *packed, const int32_t *radii, const float *v_xy, const float *v_pix_vel,
+    const float *v_conic, const float *v_colors, const float *v_opacity, const float *v_depth, float *g_means,
+    float *g_log_scales, float *g_quats, float *g_opacity_logit, float *g_sh_dc, float *g_sh_rest, float *g_lin_vel,
+    float *g_ang_vel, float *g_viewmat, void *stream) {
+    int rc = check_views(num_views, num_points, viewmats, cam_pos, lin_vel, ang_vel, intrinsics);
+    if (rc) return rc;
+    B200_REQUIRE(v_depth, "null v_depth");
+    return run_fused_backward(num_views, num_points, means, log_scales, quats, opacity_logit, sh_dc, sh_rest, sh_bases,
+                              degrees_to_use, viewmats, cam_pos, lin_vel, ang_vel, intrinsics, rolling_shutter_time,
+                              exposure_time, 1.f, 1.f, 0.f, 0.f, img_height, img_width, block_width, clip_thresh, packed,
+                              radii, v_xy, v_pix_vel, v_conic, v_colors, v_opacity, g_means, g_log_scales, g_quats,
+                              g_opacity_logit, g_sh_dc, g_sh_rest, g_lin_vel, g_ang_vel, g_viewmat, nullptr,
+                              as_stream(stream), v_depth);
+}
+
+extern "C" int b200_fused_preprocess_backward_views_depth_deterministic(
+    int num_views, int num_points, const float *means, const float *log_scales, const float *quats,
+    const float *opacity_logit, const float *sh_dc, const float *sh_rest, int sh_bases, int degrees_to_use,
+    const float *viewmats, const float *cam_pos, const float *lin_vel, const float *ang_vel, const float *intrinsics,
+    float rolling_shutter_time, float exposure_time, unsigned img_height, unsigned img_width, unsigned block_width,
+    float clip_thresh, const void *packed, const int32_t *radii, const float *v_xy, const float *v_pix_vel,
+    const float *v_conic, const float *v_colors, const float *v_opacity, const float *v_depth, float *g_means,
+    float *g_log_scales, float *g_quats, float *g_opacity_logit, float *g_sh_dc, float *g_sh_rest, float *g_lin_vel,
+    float *g_ang_vel, float *g_viewmat, void *ws, size_t ws_bytes, void *stream) {
+    int rc = check_views(num_views, num_points, viewmats, cam_pos, lin_vel, ang_vel, intrinsics);
+    if (rc) return rc;
+    B200_REQUIRE(v_depth, "null v_depth");
+    B200_REQUIRE(ws && aligned16(ws), "ws must be a 16-byte aligned workspace");
+    const size_t need = b200_fused_preprocess_backward_views_ws_bytes(num_views, num_points);
+    B200_REQUIRE(ws_bytes >= need, "ws too small: %zu bytes, b200_fused_preprocess_backward_views_ws_bytes gives %zu",
+                 ws_bytes, need);
+    return run_fused_backward(num_views, num_points, means, log_scales, quats, opacity_logit, sh_dc, sh_rest, sh_bases,
+                              degrees_to_use, viewmats, cam_pos, lin_vel, ang_vel, intrinsics, rolling_shutter_time,
+                              exposure_time, 1.f, 1.f, 0.f, 0.f, img_height, img_width, block_width, clip_thresh, packed,
+                              radii, v_xy, v_pix_vel, v_conic, v_colors, v_opacity, g_means, g_log_scales, g_quats,
+                              g_opacity_logit, g_sh_dc, g_sh_rest, g_lin_vel, g_ang_vel, g_viewmat,
+                              static_cast<float *>(ws), as_stream(stream), v_depth);
 }

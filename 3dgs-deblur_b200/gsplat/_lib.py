@@ -104,6 +104,18 @@ SIGNATURES = {
                                        _p, _p, _i, _p]),
     "b200_blend_backward_views_deterministic": (_i, [_i, _i, _i, _u, _u, _u, _u, _p, _p, _p, _f, _f, _p, _p, _p, _p, _p,
                                                      _p, _p, _sz, _p, _p, _p, _p, _p, _p, _p]),
+    "b200_blend_depth_forward": (_i, [_i, _u, _u, _u, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "b200_blend_depth_backward": (_i, [_i, _i, _u, _u, _u, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "b200_blend_depth_backward_deterministic_ws_bytes": (_sz, [_i, _i, _u]),
+    "b200_blend_depth_backward_deterministic": (_i, [_i, _i, _i, _u, _u, _u, _p, _p, _p, _p, _p, _p, _p, _p, _sz, _p, _p,
+                                                     _p, _p, _p]),
+    "b200_fused_preprocess_backward_views_depth": (_i, [_i, _i, _p, _p, _p, _p, _p, _p, _i, _i, _p, _p, _p, _p, _p, _f, _f,
+                                                        _u, _u, _u, _f, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p,
+                                                        _p, _p, _p, _p, _p, _p]),
+    "b200_fused_preprocess_backward_views_depth_deterministic": (_i, [_i, _i, _p, _p, _p, _p, _p, _p, _i, _i, _p, _p, _p,
+                                                                      _p, _p, _f, _f, _u, _u, _u, _f, _p, _p, _p, _p,
+                                                                      _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p,
+                                                                      _p, _p, _sz, _p]),
     "b200_nd_rasterize_forward": (_i, [_i, _u, _u, _u, _u, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
     "b200_nd_rasterize_backward": (_i, [_i, _u, _u, _u, _u, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p,
                                         _p, _p, _p, _p, _p, _p]),

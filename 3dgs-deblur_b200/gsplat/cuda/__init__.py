@@ -536,6 +536,72 @@ def fused_preprocess_backward_views(device, *args):
         check(lib.b200_fused_preprocess_backward_views(*args, stream()))
 
 
+# ---- differentiable depth (include/b200splat.h "differentiable depth"): records of the fused forward ----------------
+
+def blend_depth_forward(views, img_height, img_width, block_width, gaussian_ids_sorted, tile_bins, packed, view_isect=None,
+                        want_state=False):
+    """Extension: the one-channel static depth blend -> D (B,H,W) [, final_T (B,H,W), final_idx (B,H,W)] (the saved
+    state of the backward when want_state).  view_isect (B,) int32 on the device or None: a view < 1 renders D = 0."""
+    require_cuda(gaussian_ids_sorted, tile_bins, packed, view_isect)
+    dev = packed.device
+    B, H, W, bw = int(views), int(img_height), int(img_width), int(block_width)
+    with on_device(dev):
+        D = torch.empty((B, H, W), dtype=torch.float32, device=dev)
+        fT = torch.empty((B, H, W), dtype=torch.float32, device=dev) if want_state else None
+        fi = torch.empty((B, H, W), dtype=torch.int32, device=dev) if want_state else None
+        order = _tile_order(tile_bins, H, W, bw, B)
+        check(_lib.load().b200_blend_depth_forward(B, H, W, bw, ptr(gaussian_ids_sorted), ptr(tile_bins), ptr(packed),
+                                                   ptr(view_isect), ptr(order), ptr(D), ptr(fT), ptr(fi), stream()))
+    return (D, fT, fi) if want_state else D
+
+
+def blend_depth_backward(views, num_records, img_height, img_width, block_width, gaussian_ids_sorted, tile_bins, packed,
+                         final_T, final_idx, v_depth_img, v_xy, v_conic, v_opacity):
+    """Extension: backward of blend_depth_forward with cotangent v_depth_img (B,H,W).  Adds the depth pass's xy, conic
+    and opacity gradients into v_xy (R,2), v_conic (R,3), v_opacity (R,1) in place (the colour backward's outputs, R =
+    num_records) and returns v_depth (R,).  Under torch.use_deterministic_algorithms(True) the sums run in a fixed order
+    and are added to the given arrays with one elementwise add each."""
+    require_cuda(gaussian_ids_sorted, tile_bins, packed, final_T, final_idx, v_xy, v_conic, v_opacity)
+    dev = packed.device
+    B, n, H, W, bw = int(views), int(num_records), int(img_height), int(img_width), int(block_width)
+    lib = _lib.load()
+    with on_device(dev):
+        f32 = dict(dtype=torch.float32, device=dev)
+        v_depth_img = _f32(v_depth_img).contiguous()
+        v_depth = torch.empty((n,), **f32)
+        order = _tile_order(tile_bins, H, W, bw, B)
+        if deterministic():
+            m = gaussian_ids_sorted.numel()
+            nbytes = lib.b200_blend_depth_backward_deterministic_ws_bytes(n, m, bw)
+            ws = _lib.workspace(nbytes, dev)
+            d_xy, d_conic, d_op = torch.empty((n, 2), **f32), torch.empty((n, 3), **f32), torch.empty((n, 1), **f32)
+            check(lib.b200_blend_depth_backward_deterministic(
+                B, n, m, H, W, bw, ptr(gaussian_ids_sorted), ptr(tile_bins), ptr(packed), ptr(_f32(final_T)),
+                ptr(final_idx), ptr(v_depth_img), ptr(order), ptr(ws), nbytes, ptr(d_xy), ptr(d_conic), ptr(d_op),
+                ptr(v_depth), stream()))
+            v_xy.add_(d_xy)
+            v_conic.add_(d_conic)
+            v_opacity.add_(d_op)
+        else:
+            check(lib.b200_blend_depth_backward(
+                B, n, H, W, bw, ptr(gaussian_ids_sorted), ptr(tile_bins), ptr(packed), ptr(_f32(final_T)), ptr(final_idx),
+                ptr(v_depth_img), ptr(order), ptr(v_xy), ptr(v_conic), ptr(v_opacity), ptr(v_depth), stream()))
+    return v_depth
+
+
+def fused_preprocess_backward_views_depth(device, *args):
+    """b200_fused_preprocess_backward_views_depth with `args` as in include/b200splat.h up to the stream; camera sums in
+    block order under torch.use_deterministic_algorithms(True)."""
+    lib = _lib.load()
+    views, n, g_cam = int(args[0]), int(args[1]), args[-3:]
+    if deterministic() and any(p is not None for p in g_cam):
+        nbytes = lib.b200_fused_preprocess_backward_views_ws_bytes(views, n)
+        ws = _lib.workspace(nbytes, device)
+        check(lib.b200_fused_preprocess_backward_views_depth_deterministic(*args, ptr(ws), nbytes, stream()))
+    else:
+        check(lib.b200_fused_preprocess_backward_views_depth(*args, stream()))
+
+
 def _geom(tile_bounds, block, img_size):
     return int(img_size[1]), int(img_size[0]), int(block[0])
 

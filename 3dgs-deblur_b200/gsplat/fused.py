@@ -26,55 +26,56 @@ def render_gaussians(means: Tensor, log_scales: Tensor, quats: Tensor, opacity_l
                      angular_velocity: Optional[Tensor], fx: float, fy: float, cx: float, cy: float, img_height: int,
                      img_width: int, block_width: int, background: Tensor, rolling_shutter_time: float = 0.0,
                      exposure_time: float = 0.0, blur_samples: int = 1, sh_degree_to_use: int = 3,
-                     clip_thresh: float = 0.01, grad_sink: Optional[Dict[str, Tensor]] = None, return_depth: bool = False):
+                     clip_thresh: float = 0.01, grad_sink: Optional[Dict[str, Tensor]] = None, return_depth: bool = False,
+                     depth_grad: bool = False):
     """Returns (rgb (H,W,3), alpha (H,W), info).  info["radii"] (N,) int32; after backward info["absgrad"] (N,2) holds the
     abs-grad densification statistic (the `xys.absgrad` side channel of the drop-in operator).
 
-    return_depth: also info["depth"] (H,W,1), the caller's eval depth image (splatfacto.py:881-897: a second, static
-    rasterize call with the depths as colours over a zero background, divided by alpha; the largest rendered depth where
-    alpha is 0) -- one more blend launch over the lists already built instead of a second projection-sized binning
-    (lists are rebuilt only when the colour pass had rolling shutter or an even sample count with exposure: then they do
-    not provably contain the static lists).  Not differentiable.
+    return_depth: also info["depth"] (H,W,1), Splatfacto's depth image (splatfacto.py:881-897): D = the static blend
+    (one sample, no rolling shutter, zero background) of the Gaussians' view-space depths, then
+    where(alpha > 0, D / alpha, D.detach().max()) with the colour pass's alpha.  D comes from a one-channel depth blend
+    over the lists already built (they are rebuilt only when the colour pass had rolling shutter or an even sample count
+    with exposure: then they do not provably contain the static lists).
+    depth_grad: make info["depth"] differentiable (needs return_depth): its gradient reaches the Gaussians' positions,
+    shapes, opacities and depths through D, and the colour pass through alpha.  The values are the same bit for bit as
+    without it; without it info["depth"] does not require grad.  As in Splatfacto, a pixel where alpha is 0 has a NaN
+    gradient (0 / 0 in the division's backward), so a depth loss belongs on pixels that something covers.
 
     grad_sink (optional): {"means", "log_scales", "quats", "opacity_logit", "sh_dc", "sh_rest"} -> preallocated
     gradient buffers (e.g. slices of a flat DP buffer).  When given, backward OVERWRITES them directly (every row,
     zeros for culled Gaussians) and autograd returns no gradient for those inputs -- no accumulate pass, no memset."""
+    if depth_grad and not return_depth:
+        raise ValueError("render_gaussians: depth_grad=True needs return_depth=True")
     if linear_velocity is None:
         linear_velocity = torch.zeros(3, device=means.device)
         angular_velocity = torch.zeros(3, device=means.device)
     info: Dict[str, Tensor] = {}
-    rgb, alpha = _FusedRender.apply(means, log_scales, quats, opacity_logit, sh_dc, sh_rest, viewmat, cam_pos,
-                                    linear_velocity, angular_velocity, background,
-                                    (float(fx), float(fy), float(cx), float(cy), int(img_height), int(img_width),
-                                     int(block_width), float(rolling_shutter_time), float(exposure_time),
-                                     int(blur_samples), int(sh_degree_to_use), float(clip_thresh)), grad_sink, info)
-    lists = info.pop("_lists")
+    rgb, alpha, D = _FusedRender.apply(means, log_scales, quats, opacity_logit, sh_dc, sh_rest, viewmat, cam_pos,
+                                       linear_velocity, angular_velocity, background,
+                                       (float(fx), float(fy), float(cx), float(cy), int(img_height), int(img_width),
+                                        int(block_width), float(rolling_shutter_time), float(exposure_time),
+                                        int(blur_samples), int(sh_degree_to_use), float(clip_thresh)), grad_sink, info,
+                                       _depth_mode(return_depth, depth_grad))
     if return_depth:
-        info["depth"] = _depth_pass(lists, alpha, int(img_height), int(img_width), int(block_width), int(blur_samples),
-                                    float(rolling_shutter_time), float(exposure_time))
+        d, a = D[..., None], (alpha if depth_grad else alpha.detach())[..., None]
+        info["depth"] = torch.where(a > 0, d / a, d.detach().max())  # splatfacto.py:895-897
     return rgb, alpha, info
 
 
-def _depth_pass(lists, alpha, H, W, bw, S, rs, ex):
-    packed, depths, radii, nth, ids, bins, total = lists
-    dev = depths.device
-    with torch.no_grad(), _lib.on_device(dev):
-        if total < 1:  # the reference's empty-render branch returns the (zero) background
-            depth_im = torch.zeros(H, W, 1, device=dev)
-        else:
-            rec = _C.set_record_colors(packed.clone(), depths[:, None].expand(-1, 3).contiguous())
-            if not (rs == 0 and (ex == 0 or S % 2 == 1)):  # see gsplat.rasterize: the static lists may hold other pairs
-                _, ids, bins = _C.bin_cull(rec, depths, radii, nth, H, W, bw, 1, 0.0, 0.0)
-            img, _, _ = _C.blend_forward_packed(H, W, bw, 1, ids, bins, rec, 0.0, 0.0, torch.zeros(3, device=dev))
-            depth_im = img[..., 0:1]
-        a = alpha.detach()[..., None]
-        return torch.where(a > 0, depth_im / a, depth_im.max())
+def _depth_mode(return_depth, depth_grad):
+    """0: no depth; 1: D without a graph; 2: D differentiable (the backward's state is kept)"""
+    return 2 if depth_grad else (1 if return_depth else 0)
+
+
+def _static_lists_reusable(S, rs, ex):
+    """The colour pass's lists contain the static (S = 1, no rolling shutter) lists: see gsplat.rasterize."""
+    return rs == 0 and (ex == 0 or S % 2 == 1)
 
 
 class _FusedRender(Function):
     @staticmethod
     def forward(ctx, means, log_scales, quats, opacity_logit, sh_dc, sh_rest, viewmat, cam_pos, lin, ang, background,
-                cfg, grad_sink, info):
+                cfg, grad_sink, info, depth):
         fx, fy, cx, cy, H, W, bw, rs, ex, S, deg, clip = cfg
         if not (0 < S <= 10):
             raise RuntimeError("unsupported blur size")
@@ -108,22 +109,37 @@ class _FusedRender(Function):
                 alpha = 1 - Ts.mean(dim=-1)
             else:
                 rgb, Ts, fi, alpha = _C.blend_forward_packed(H, W, bw, S, ids, bins, packed, rs, ex, bg, want_alpha=True)
-        ctx.cfg, ctx.K, ctx.total = cfg, K, total
+            D = d_ids = d_bins = d_T = d_idx = None
+            if depth and total < 1:  # the empty render's zero background
+                D = torch.zeros(H, W, device=dev)
+            elif depth:
+                d_ids, d_bins = ids, bins
+                if not _static_lists_reusable(S, rs, ex):
+                    _, d_ids, d_bins = _C.bin_cull(packed, depths, radii, nth, H, W, bw, 1, 0.0, 0.0)
+                out = _C.blend_depth_forward(1, H, W, bw, d_ids, d_bins, packed, want_state=depth == 2)
+                D, d_T, d_idx = out if depth == 2 else (out, None, None)
+                D = D.view(H, W)
+            if depth != 2:  # no backward through D: nothing of the depth pass is kept
+                d_ids = d_bins = None
+            else:  # the camera of the view-batch projection backward, built on the device (no host copy)
+                ctx.intr = torch.stack([torch.full((1,), k, dtype=torch.float32, device=dev) for k in (fx, fy, cx, cy)], 1)
+        ctx.cfg, ctx.K, ctx.total, ctx.depth = cfg, K, total, depth
         ctx.grad_sink, ctx.info = grad_sink, info
         ctx.vel_shapes = (lin.shape, ang.shape)
         ctx.vel_devs = (lin.device, ang.device)
         ctx.save_for_backward(means, log_scales, quats, opacity_logit, sh_dc, sh_rest, viewmat, cam_pos, lin_d, ang_d, bg,
-                              packed, radii, ids, bins, Ts, fi)
+                              packed, radii, ids, bins, Ts, fi, d_ids, d_bins, d_T, d_idx)
         info["radii"] = radii
-        info["_lists"] = (packed, depths, radii, nth, ids, bins, total)  # for render_gaussians' optional depth pass
         ctx.mark_non_differentiable(radii)
-        ctx.set_materialize_grads(False)  # an unused alpha (or rgb) arrives as None instead of a zero image
-        return rgb, alpha
+        if depth == 1:
+            ctx.mark_non_differentiable(D)
+        ctx.set_materialize_grads(False)  # an unused alpha (or rgb, or depth) arrives as None instead of a zero image
+        return rgb, alpha, D
 
     @staticmethod
-    def backward(ctx, v_rgb, v_alpha):
+    def backward(ctx, v_rgb, v_alpha, v_D):
         (means, log_scales, quats, opacity_logit, sh_dc, sh_rest, viewmat, cam_pos, lin_d, ang_d, bg, packed, radii, ids,
-         bins, Ts, fi) = ctx.saved_tensors
+         bins, Ts, fi, d_ids, d_bins, d_T, d_idx) = ctx.saved_tensors
         fx, fy, cx, cy, H, W, bw, rs, ex, S, deg, clip = ctx.cfg
         dev = means.device
         lib = _lib.load()
@@ -150,12 +166,25 @@ class _FusedRender(Function):
             g_lin = torch.empty(3, **f32) if want_vel else None
             g_ang = torch.empty(3, **f32) if want_vel else None
             g_vm = torch.empty(3, 4, **f32) if want_vm else None
-            _C.fused_preprocess_backward(
-                dev, n, ptr(means), ptr(log_scales), ptr(quats), ptr(opacity_logit), ptr(sh_dc), ptr(sh_rest), K, deg,
-                ptr(viewmat), ptr(cam_pos), ptr(lin_d), ptr(ang_d), rs, ex, fx, fy, cx, cy, H, W, bw, clip, ptr(packed),
-                ptr(radii), ptr(v_xy), ptr(v_pix), ptr(v_conic), ptr(v_col), ptr(v_op), ptr(out["means"]),
-                ptr(out["log_scales"]), ptr(out["quats"]), ptr(out["opacity_logit"]), ptr(out["sh_dc"]), ptr(out["sh_rest"]),
-                ptr(g_lin), ptr(g_ang), ptr(g_vm))
+            grads = (ptr(out["means"]), ptr(out["log_scales"]), ptr(out["quats"]), ptr(out["opacity_logit"]),
+                     ptr(out["sh_dc"]), ptr(out["sh_rest"]), ptr(g_lin), ptr(g_ang), ptr(g_vm))
+            if ctx.depth == 2:
+                if v_D is None or ctx.total < 1:
+                    v_depth = torch.zeros(n, **f32)
+                else:
+                    v_depth = _C.blend_depth_backward(1, n, H, W, bw, d_ids, d_bins, packed, d_T, d_idx, v_D, v_xy, v_conic,
+                                                      v_op)
+                # the view-batch kernel with one view: the single-view gradients
+                _C.fused_preprocess_backward_views_depth(
+                    dev, 1, n, ptr(means), ptr(log_scales), ptr(quats), ptr(opacity_logit), ptr(sh_dc), ptr(sh_rest), K,
+                    deg, ptr(viewmat), ptr(cam_pos), ptr(lin_d), ptr(ang_d), ptr(ctx.intr), rs, ex, H, W, bw, clip,
+                    ptr(packed), ptr(radii), ptr(v_xy), ptr(v_pix), ptr(v_conic), ptr(v_col), ptr(v_op), ptr(v_depth),
+                    *grads)
+            else:
+                _C.fused_preprocess_backward(
+                    dev, n, ptr(means), ptr(log_scales), ptr(quats), ptr(opacity_logit), ptr(sh_dc), ptr(sh_rest), K, deg,
+                    ptr(viewmat), ptr(cam_pos), ptr(lin_d), ptr(ang_d), rs, ex, fx, fy, cx, cy, H, W, bw, clip, ptr(packed),
+                    ptr(radii), ptr(v_xy), ptr(v_pix), ptr(v_conic), ptr(v_col), ptr(v_op), *grads)
         ret = [None if name in sink else out[name].view_as(like)
                for name, like in (("means", means), ("log_scales", log_scales), ("quats", quats),
                                   ("opacity_logit", opacity_logit), ("sh_dc", sh_dc), ("sh_rest", sh_rest))]
@@ -171,7 +200,7 @@ class _FusedRender(Function):
                 v_bg = (v_rgb.float() * Ts.mean(dim=-1).float()[..., None]).sum((0, 1))
             else:
                 v_bg = torch.matmul(v_rgb.float().reshape(-1, 3).t(), Ts.mean(dim=-1).float().reshape(-1, 1)).squeeze()
-        return (*ret, v_viewmat, None, v_lin, v_ang, v_bg, None, None, None)
+        return (*ret, v_viewmat, None, v_lin, v_ang, v_bg, None, None, None, None)
 
 
 _INT32_MAX = 2**31 - 1
@@ -182,7 +211,7 @@ def render_gaussians_batch(means: Tensor, log_scales: Tensor, quats: Tensor, opa
                            angular_velocity: Optional[Tensor], fx, fy, cx, cy, img_height: int, img_width: int,
                            block_width: int, background: Tensor, rolling_shutter_time: float = 0.0,
                            exposure_time: float = 0.0, blur_samples: int = 1, sh_degree_to_use: int = 3,
-                           clip_thresh: float = 0.01, return_depth: bool = False):
+                           clip_thresh: float = 0.01, return_depth: bool = False, depth_grad: bool = False):
     """`render_gaussians` for B cameras of one scene in one call: one fused pre-processing launch over B * N records,
     one culled binning with one host sync, one blend grid over the B * T tiles (longest lists first across all views).
 
@@ -191,7 +220,8 @@ def render_gaussians_batch(means: Tensor, log_scales: Tensor, quats: Tensor, opa
     and background (3,) are shared by the batch.
 
     Returns (rgb (B,H,W,3), alpha (B,H,W), info): info["radii"] (B,N) int32; after backward info["absgrad"] (B,N,2)
-    (per view: feed Densifier.accumulate once per view); with return_depth info["depth"] (B,H,W,1).
+    (per view: feed Densifier.accumulate once per view); with return_depth info["depth"] (B,H,W,1), differentiable with
+    depth_grad as in render_gaussians.
 
     View v is the single-view render of camera v: rgb[v], alpha[v], radii[v] and depth[v] are bit-identical to
     render_gaussians with camera v's arguments (a view with nothing to intersect takes the empty-render branch on its
@@ -199,6 +229,8 @@ def render_gaussians_batch(means: Tensor, log_scales: Tensor, quats: Tensor, opa
     of the single-view ones over the views, the view-matrix and velocity gradients are per view; under
     torch.use_deterministic_algorithms(True) every gradient equals the single-view gradients added in view order, bit
     for bit."""
+    if depth_grad and not return_depth:
+        raise ValueError("render_gaussians_batch: depth_grad=True needs return_depth=True")
     if viewmats.dim() != 3 or tuple(viewmats.shape[1:]) not in ((3, 4), (4, 4)):
         raise ValueError(f"render_gaussians_batch: viewmats must be (B,3,4) or (B,4,4), got {tuple(viewmats.shape)}")
     B, n = int(viewmats.shape[0]), int(means.shape[0])
@@ -227,36 +259,21 @@ def render_gaussians_batch(means: Tensor, log_scales: Tensor, quats: Tensor, opa
                         else torch.full((B,), float(k), dtype=torch.float32, device=dev)
                         for k in (fx, fy, cx, cy)], dim=1).contiguous()
     info: Dict[str, Tensor] = {}
-    rgb, alpha = _FusedRenderBatch.apply(means, log_scales, quats, opacity_logit, sh_dc, sh_rest, viewmats, cam_pos, lin,
-                                         ang, background, intr,
-                                         (H, W, bw, float(rolling_shutter_time), float(exposure_time), S,
-                                          int(sh_degree_to_use), float(clip_thresh)), info)
-    lists = info.pop("_lists")
-    if return_depth:
-        info["depth"] = _depth_pass_views(lists, alpha, B, H, W, bw, S, float(rolling_shutter_time), float(exposure_time))
+    rgb, alpha, D = _FusedRenderBatch.apply(means, log_scales, quats, opacity_logit, sh_dc, sh_rest, viewmats, cam_pos,
+                                            lin, ang, background, intr,
+                                            (H, W, bw, float(rolling_shutter_time), float(exposure_time), S,
+                                             int(sh_degree_to_use), float(clip_thresh)), info,
+                                            _depth_mode(return_depth, depth_grad))
+    if return_depth:  # each view filled with its own maximum where its alpha is 0
+        d, a = D[..., None], (alpha if depth_grad else alpha.detach())[..., None]
+        info["depth"] = torch.where(a > 0, d / a, d.detach().amax(dim=(1, 2, 3), keepdim=True))
     return rgb, alpha, info
-
-
-def _depth_pass_views(lists, alpha, B, H, W, bw, S, rs, ex):
-    """`_depth_pass` over a view batch: the same static depth blend and lists reuse rule, each view filled with its own
-    maximum where its alpha is 0."""
-    packed, depths, radii, nth, ids, bins, view_isect = lists
-    dev = depths.device
-    with torch.no_grad(), _lib.on_device(dev):
-        rec = _C.set_record_colors(packed.clone(), depths[:, None].expand(-1, 3).contiguous())
-        if not (rs == 0 and (ex == 0 or S % 2 == 1)):  # see _depth_pass
-            view_isect, ids, bins = _C.bin_cull_views(B, rec, depths, radii, nth, H, W, bw, 1, 0.0, 0.0)
-        img, _, _ = _C.blend_forward_views(B, H, W, bw, 1, ids, bins, rec, 0.0, 0.0, torch.zeros(3, device=dev), view_isect,
-                                           want_alpha=False)
-        depth_im = img[..., 0:1]
-        a = alpha.detach()[..., None]
-        return torch.where(a > 0, depth_im / a, depth_im.amax(dim=(1, 2, 3), keepdim=True))
 
 
 class _FusedRenderBatch(Function):
     @staticmethod
     def forward(ctx, means, log_scales, quats, opacity_logit, sh_dc, sh_rest, viewmats, cam_pos, lin, ang, background,
-                intr, cfg, info):
+                intr, cfg, info, depth):
         H, W, bw, rs, ex, S, deg, clip = cfg
         dev = means.device
         lib = _lib.load()
@@ -280,22 +297,32 @@ class _FusedRenderBatch(Function):
             view_isect, ids, bins = _C.bin_cull_views(B, packed, depths, radii, nth, H, W, bw, S, rs, ex)
             bg = background.contiguous()
             rgb, Ts, fi, alpha = _C.blend_forward_views(B, H, W, bw, S, ids, bins, packed, rs, ex, bg, view_isect)
-        ctx.cfg, ctx.K, ctx.B = cfg, K, B
+            D = d_ids = d_bins = d_T = d_idx = None
+            if depth:
+                d_isect, d_ids, d_bins = view_isect, ids, bins
+                if not _static_lists_reusable(S, rs, ex):
+                    d_isect, d_ids, d_bins = _C.bin_cull_views(B, packed, depths, radii, nth, H, W, bw, 1, 0.0, 0.0)
+                out = _C.blend_depth_forward(B, H, W, bw, d_ids, d_bins, packed, d_isect, want_state=depth == 2)
+                D, d_T, d_idx = out if depth == 2 else (out, None, None)
+                if depth != 2:  # no backward through D: nothing of the depth pass is kept
+                    d_ids = d_bins = None
+        ctx.cfg, ctx.K, ctx.B, ctx.depth = cfg, K, B, depth
         ctx.info = info
         ctx.vel_shapes = (lin.shape, ang.shape)
         ctx.vel_devs = (lin.device, ang.device)
         ctx.save_for_backward(means, log_scales, quats, opacity_logit, sh_dc, sh_rest, viewmats, vm, cam_pos, lin_d, ang_d,
-                              intr, bg, packed, radii, ids, bins, Ts, fi)
+                              intr, bg, packed, radii, ids, bins, Ts, fi, d_ids, d_bins, d_T, d_idx)
         info["radii"] = radii.view(B, n)
-        info["_lists"] = (packed, depths, radii, nth, ids, bins, view_isect)  # for the optional depth pass
         ctx.mark_non_differentiable(radii)
+        if depth == 1:
+            ctx.mark_non_differentiable(D)
         ctx.set_materialize_grads(False)
-        return rgb, alpha
+        return rgb, alpha, D
 
     @staticmethod
-    def backward(ctx, v_rgb, v_alpha):
+    def backward(ctx, v_rgb, v_alpha, v_D):
         (means, log_scales, quats, opacity_logit, sh_dc, sh_rest, viewmats, vm, cam_pos, lin_d, ang_d, intr, bg, packed,
-         radii, ids, bins, Ts, fi) = ctx.saved_tensors
+         radii, ids, bins, Ts, fi, d_ids, d_bins, d_T, d_idx) = ctx.saved_tensors
         H, W, bw, rs, ex, S, deg, clip = ctx.cfg
         dev = means.device
         B, n, K = ctx.B, means.shape[0], ctx.K
@@ -313,11 +340,19 @@ class _FusedRenderBatch(Function):
             g_lin = torch.empty(B, 3, **f32) if want_vel else None
             g_ang = torch.empty(B, 3, **f32) if want_vel else None
             g_vm = torch.empty(B, 3, 4, **f32) if want_vm else None
-            _C.fused_preprocess_backward_views(
-                dev, B, n, ptr(means), ptr(log_scales), ptr(quats), ptr(opacity_logit), ptr(sh_dc), ptr(sh_rest), K, deg,
-                ptr(vm), ptr(cam_pos), ptr(lin_d), ptr(ang_d), ptr(intr), rs, ex, H, W, bw, clip, ptr(packed), ptr(radii),
-                ptr(v_xy), ptr(v_pix), ptr(v_conic), ptr(v_col), ptr(v_op), *[ptr(t) for t in out], ptr(g_lin), ptr(g_ang),
-                ptr(g_vm))
+            args = (dev, B, n, ptr(means), ptr(log_scales), ptr(quats), ptr(opacity_logit), ptr(sh_dc), ptr(sh_rest), K,
+                    deg, ptr(vm), ptr(cam_pos), ptr(lin_d), ptr(ang_d), ptr(intr), rs, ex, H, W, bw, clip, ptr(packed),
+                    ptr(radii), ptr(v_xy), ptr(v_pix), ptr(v_conic), ptr(v_col), ptr(v_op))
+            grads = (*[ptr(t) for t in out], ptr(g_lin), ptr(g_ang), ptr(g_vm))
+            if ctx.depth == 2:
+                if v_D is None:
+                    v_depth = torch.zeros(B * n, **f32)
+                else:
+                    v_depth = _C.blend_depth_backward(B, B * n, H, W, bw, d_ids, d_bins, packed, d_T, d_idx, v_D, v_xy,
+                                                      v_conic, v_op)
+                _C.fused_preprocess_backward_views_depth(*args, ptr(v_depth), *grads)
+            else:
+                _C.fused_preprocess_backward_views(*args, *grads)
             v_viewmat = None
             if want_vm:
                 v_viewmat = torch.zeros_like(viewmats)
@@ -334,4 +369,4 @@ class _FusedRenderBatch(Function):
                                         Ts.mean(dim=-1).float().reshape(B, -1, 1)).sum(0).squeeze(-1)
         v_lin = g_lin.reshape(ctx.vel_shapes[0]).to(ctx.vel_devs[0]) if (want_vel and ctx.needs_input_grad[8]) else None
         v_ang = g_ang.reshape(ctx.vel_shapes[1]).to(ctx.vel_devs[1]) if (want_vel and ctx.needs_input_grad[9]) else None
-        return (*out, v_viewmat, None, v_lin, v_ang, v_bg, None, None, None)
+        return (*out, v_viewmat, None, v_lin, v_ang, v_bg, None, None, None, None)

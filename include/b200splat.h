@@ -429,6 +429,61 @@ B200_API int b200_blend_backward_views_deterministic(int num_views, int num_reco
                                                      size_t ws_bytes, float *v_xy, float *v_xy_abs, float *v_pix_vels,
                                                      float *v_conic, float *v_colors, float *v_opacity, void *stream);
 
+/* ---- differentiable depth (splatfacto.py:881-897) ---------------------------------------------------------------------
+ * D = the static blend (S = 1, no rolling shutter, zero background) of the records' view-space depths: the second
+ * rasterize call Splatfacto makes with the depths as colours.  The records must come from the fused forward entry points
+ * (b200_fused_preprocess_forward(_views), b200_fused_geometry_forward), which store the depth in the record's last
+ * word; b200_pack_records stores 0 there.  Lists: the static lists of the same records (b200_bin_cull* with S = 1,
+ * rs = exposure = 0), or lists that contain them (the colour pass's when rs == 0 and (exposure == 0 or S odd)).
+ * Layouts are those of the view batches above, with B = num_views (1 for one camera): images (B,H,W), records B * N.
+ * b200_blend_depth_forward: out_depth (B,H,W); final_T (B,H,W) float and final_idx (B,H,W) int32 for a backward, or
+ *   both null.  view_isect (DEVICE int32[B]) may be null; a view whose entry is < 1 takes the empty-render branch
+ *   (D = 0, final_T = 0, final_idx = 0).  tile_order: b200_blend_tile_order of tile_bins, or null for raster order.
+ *   D is bit for bit channel 0 of b200_blend_forward_views / _packed at S = 1 on records whose colours are the depths.
+ * b200_blend_depth_backward: with cotangent v_depth_img (B,H,W), ADDS the depth pass's gradients into v_xy (B*N,2),
+ *   v_conic (B*N,3) and v_opacity (B*N) -- the colour backward's outputs -- and overwrites v_depth (B*N).
+ * b200_blend_depth_backward_deterministic: the same sums in a fixed order (per Gaussian: ascending list position, then
+ *   warp), every output OVERWRITTEN (add them to the colour pass's gradients yourself).  ws: 256-byte aligned,
+ *   b200_blend_depth_backward_deterministic_ws_bytes(B * N, num_entries, block_width) bytes, num_entries = the list
+ *   length.
+ * b200_fused_preprocess_backward_views_depth(_deterministic): b200_fused_preprocess_backward_views(_deterministic) with
+ *   v_depth (B*N) as the projection's depth cotangent; B = 1 with the camera's intrinsics gives the single-view result. */
+B200_API int b200_blend_depth_forward(int num_views, unsigned img_height, unsigned img_width, unsigned block_width,
+                                      const int32_t *gaussian_ids_sorted, const int32_t *tile_bins, const void *packed,
+                                      const int32_t *view_isect, const int32_t *tile_order, float *out_depth,
+                                      float *final_T, int32_t *final_idx, void *stream);
+B200_API int b200_blend_depth_backward(int num_views, int num_records, unsigned img_height, unsigned img_width,
+                                       unsigned block_width, const int32_t *gaussian_ids_sorted, const int32_t *tile_bins,
+                                       const void *packed, const float *final_T, const int32_t *final_idx,
+                                       const float *v_depth_img, const int32_t *tile_order, float *v_xy, float *v_conic,
+                                       float *v_opacity, float *v_depth, void *stream);
+B200_API size_t b200_blend_depth_backward_deterministic_ws_bytes(int num_records, int num_entries, unsigned block_width);
+B200_API int b200_blend_depth_backward_deterministic(int num_views, int num_records, int num_entries,
+                                                     unsigned img_height, unsigned img_width, unsigned block_width,
+                                                     const int32_t *gaussian_ids_sorted, const int32_t *tile_bins,
+                                                     const void *packed, const float *final_T, const int32_t *final_idx,
+                                                     const float *v_depth_img, const int32_t *tile_order, void *ws,
+                                                     size_t ws_bytes, float *v_xy, float *v_conic, float *v_opacity,
+                                                     float *v_depth, void *stream);
+B200_API int b200_fused_preprocess_backward_views_depth(
+    int num_views, int num_points, const float *means, const float *log_scales, const float *quats,
+    const float *opacity_logit, const float *sh_dc, const float *sh_rest, int sh_bases, int degrees_to_use,
+    const float *viewmats, const float *cam_pos, const float *lin_vel, const float *ang_vel, const float *intrinsics,
+    float rolling_shutter_time, float exposure_time, unsigned img_height, unsigned img_width, unsigned block_width,
+    float clip_thresh, const void *packed, const int32_t *radii, const float *v_xy, const float *v_pix_vel,
+    const float *v_conic, const float *v_colors, const float *v_opacity, const float *v_depth, float *g_means,
+    float *g_log_scales, float *g_quats, float *g_opacity_logit, float *g_sh_dc, float *g_sh_rest, float *g_lin_vel,
+    float *g_ang_vel, float *g_viewmat, void *stream);
+B200_API int b200_fused_preprocess_backward_views_depth_deterministic(
+    int num_views, int num_points, const float *means, const float *log_scales, const float *quats,
+    const float *opacity_logit, const float *sh_dc, const float *sh_rest, int sh_bases, int degrees_to_use,
+    const float *viewmats, const float *cam_pos, const float *lin_vel, const float *ang_vel, const float *intrinsics,
+    float rolling_shutter_time, float exposure_time, unsigned img_height, unsigned img_width, unsigned block_width,
+    float clip_thresh, const void *packed, const int32_t *radii, const float *v_xy, const float *v_pix_vel,
+    const float *v_conic, const float *v_colors, const float *v_opacity, const float *v_depth, float *g_means,
+    float *g_log_scales, float *g_quats, float *g_opacity_logit, float *g_sh_dc, float *g_sh_rest, float *g_lin_vel,
+    float *g_ang_vel, float *g_viewmat, void *ws, size_t ws_bytes, void *stream);
+
 /* ---- N-channel blend (no blur), fp16 accumulators like the reference ----------------------
  * replaces nd_rasterize_forward_tensor / nd_rasterize_backward_tensor (bindings.h:129-166,
  * bindings.cu:506-682; kernels forward.cu:185-304, backward.cu:22-141). */
