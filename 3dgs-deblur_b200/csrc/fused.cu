@@ -146,9 +146,10 @@ __device__ __forceinline__ void add_view(float &a, float x, bool first) { a = fi
 // one, the raw-parameter gradients are summed over the views in registers (the sh_rest rows in shared memory) and each
 // row is written once.  The camera gradients are per view: io.g_lin / g_ang / g_viewmat + 3 v / 3 v / 12 v.
 // DET: the camera partials of the block are stored to io.cam_partials (18 floats per (view, block)) instead of added to
-// the outputs (deterministic mode).  VIEWS = false: one view (f0.views == 1), the loop and the view sums compile away.
+// the outputs (deterministic mode).  VIEWS: 0 one camera with f0's own intrinsics; 1 one view whose intrinsics are
+// f0.intr[0] (a view batch of one); 2 f0.views views.  With 0 and 1 the loop and the view sums compile away.
 // DEPTH: io.v_depth[record] is the projection's depth cotangent (0 otherwise).
-template <int DEG_USE, bool DET, bool VIEWS, bool DEPTH>
+template <int DEG_USE, bool DET, int VIEWS, bool DEPTH>
 __global__ void __launch_bounds__(FUSED_THREADS) fused_backward_kernel(const FusedParams f0, FusedBwdIO io) {
     constexpr int KU = (DEG_USE + 1) * (DEG_USE + 1);
     extern __shared__ __align__(16) float s_rows[];  // [FUSED_THREADS][pitch] gradient rows of sh_rest
@@ -164,11 +165,11 @@ __global__ void __launch_bounds__(FUSED_THREADS) fused_backward_kernel(const Fus
     float g_mean[3] = {0.f, 0.f, 0.f}, g_ls[3] = {0.f, 0.f, 0.f}, g_q[4] = {0.f, 0.f, 0.f, 0.f}, g_op = 0.f,
           g_dc[3] = {0.f, 0.f, 0.f};
     float *my_rows = s_rows + t * pitch;
-    const int views = VIEWS ? f0.views : 1;
+    const int views = VIEWS == 2 ? f0.views : 1;
     for (int v = 0; v < views; ++v) {
         FusedParams f = f0;
-        if (VIEWS) select_view(f, v);
-        const bool first = !VIEWS || v == 0;
+        if (VIEWS != 0) select_view(f, v);
+        const bool first = VIEWS != 2 || v == 0;
         const size_t ri = (size_t)v * f0.proj.n + i;  // record of Gaussian i in view v
         ProjGaussGrad gr;
 #pragma unroll
@@ -450,7 +451,8 @@ static int run_fused_backward(int views, int num_points, const float *means, con
     const size_t smem = sizeof(float) * FUSED_THREADS * (size_t)(pitch > 0 ? pitch : 1);
     const int blocks = ceil_div(num_points, FUSED_THREADS);
     auto launch = [&](auto det_c, auto views_c, auto depth_c) {
-        constexpr bool D = decltype(det_c)::value, V = decltype(views_c)::value, Z = decltype(depth_c)::value;
+        constexpr bool D = decltype(det_c)::value, Z = decltype(depth_c)::value;
+        constexpr int V = decltype(views_c)::value;
         switch (degrees_to_use) {
             case 0: fused_backward_kernel<0, D, V, Z><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
             case 1: fused_backward_kernel<1, D, V, Z><<<blocks, FUSED_THREADS, smem, st>>>(f, io); break;
@@ -461,12 +463,24 @@ static int run_fused_backward(int views, int num_points, const float *means, con
     };
     using T_ = std::true_type;
     using F_ = std::false_type;
+    using One_ = std::integral_constant<int, 0>;      // one camera, scalar intrinsics
+    using OneView_ = std::integral_constant<int, 1>;  // a view batch of one: no view loop
+    using Views_ = std::integral_constant<int, 2>;
+    auto dispatch = [&](auto det_c) {
+        if (views > 1) {
+            if (v_depth) launch(det_c, Views_{}, T_{}); else launch(det_c, Views_{}, F_{});
+        } else if (intr) {
+            if (v_depth) launch(det_c, OneView_{}, T_{}); else launch(det_c, OneView_{}, F_{});
+        } else {
+            launch(det_c, One_{}, F_{});
+        }
+    };
     if (det) {
-        if (v_depth) launch(T_{}, T_{}, T_{}); else if (intr) launch(T_{}, T_{}, F_{}); else launch(T_{}, F_{}, F_{});
+        dispatch(T_{});
         B200_LAUNCH_CHECK();
         cam_partials_sum_kernel<<<views, 32, 0, st>>>(blocks, cam_ws, g_lin_vel, g_ang_vel, g_viewmat);
     } else {
-        if (v_depth) launch(F_{}, T_{}, T_{}); else if (intr) launch(F_{}, T_{}, F_{}); else launch(F_{}, F_{}, F_{});
+        dispatch(F_{});
     }
     B200_LAUNCH_CHECK();
     return B200_OK;

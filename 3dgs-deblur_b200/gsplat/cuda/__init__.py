@@ -358,47 +358,46 @@ def blend_backward_packed(num_points, img_height, img_width, block_width, n_blur
     block the lists were built with (its entry count marks where the padding starts); only read in that mode."""
     require_cuda(gaussian_ids_sorted, tile_bins, packed, background)
     dev = packed.device
+    n, H, W, bw, S = int(num_points), int(img_height), int(img_width), int(block_width), int(n_blur_samples)
+    rs, ex = float(rolling_shutter_time), float(exposure_time)
+    lib = _lib.load()
     with on_device(dev):
-        n = int(num_points)
-        f32 = dict(dtype=torch.float32, device=dev)
         v_output = _f32(v_output).contiguous()
         v_output_alpha = _f32(v_output_alpha).contiguous() if v_output_alpha is not None else None
-        if deterministic():
-            return _blend_backward_deterministic(n, int(img_height), int(img_width), int(block_width),
-                                                 int(n_blur_samples), gaussian_ids_sorted, tile_bins, packed,
-                                                 float(rolling_shutter_time), float(exposure_time), _f32(background),
-                                                 _f32(final_Ts), final_idx, v_output, v_output_alpha, status)
-        # one zero-filled allocation for the 13 floats per Gaussian the kernel accumulates into (each array 64-byte
-        # aligned inside it): one fill instead of six memsets
-        pitch = (n + 15) & ~15
-        acc = torch.zeros(13 * pitch, **f32)
-        v_xy, v_xy_abs, v_pix = (acc[k * 2 * pitch:k * 2 * pitch + 2 * n].view(n, 2) for k in range(3))
-        v_conic, v_colors = (acc[6 * pitch + k * 3 * pitch:6 * pitch + k * 3 * pitch + 3 * n].view(n, 3) for k in range(2))
-        v_opacity = acc[12 * pitch:12 * pitch + n].view(n, 1)
-        order = _tile_order(tile_bins, int(img_height), int(img_width), int(block_width))
-        check(_lib.load().b200_blend_backward_packed_ordered(
-            n, int(img_height), int(img_width), int(block_width), int(n_blur_samples), ptr(gaussian_ids_sorted),
-            ptr(tile_bins), ptr(packed), float(rolling_shutter_time), float(exposure_time), ptr(_f32(background)),
-            ptr(_f32(final_Ts)), ptr(final_idx), ptr(v_output), ptr(v_output_alpha), ptr(order), ptr(v_xy), ptr(v_xy_abs),
-            ptr(v_pix), ptr(v_conic), ptr(v_colors), ptr(v_opacity), 1, stream()))
-    return v_xy, v_xy_abs, v_pix, v_conic, v_colors, v_opacity
-
-
-def _blend_backward_deterministic(n, H, W, bw, S, ids, bins, packed, rs, ex, bg, final_Ts, final_idx, v_output,
-                                  v_output_alpha, status):
-    lib = _lib.load()
-    dev = packed.device
-    f32 = dict(dtype=torch.float32, device=dev)
-    m = ids.numel()
-    nbytes = lib.b200_blend_backward_deterministic_ws_bytes(n, m, bw)
-    ws = _lib.workspace(nbytes, dev)
-    outs = (torch.empty((n, 2), **f32), torch.empty((n, 2), **f32), torch.empty((n, 2), **f32),
-            torch.empty((n, 3), **f32), torch.empty((n, 3), **f32), torch.empty((n, 1), **f32))
-    order = _tile_order(bins, H, W, bw)
-    check(lib.b200_blend_backward_packed_deterministic(
-        n, m, H, W, bw, S, ptr(ids), ptr(bins), ptr(packed), rs, ex, ptr(bg), ptr(final_Ts), ptr(final_idx),
-        ptr(v_output), ptr(v_output_alpha), ptr(status), ptr(order), ptr(ws), nbytes, *[ptr(t) for t in outs], stream()))
+        m = gaussian_ids_sorted.numel()
+        outs, ws, nbytes = _blend_backward_outputs(n, m, bw, dev)
+        order = _tile_order(tile_bins, H, W, bw)
+        if ws is not None:
+            check(lib.b200_blend_backward_packed_deterministic(
+                n, m, H, W, bw, S, ptr(gaussian_ids_sorted), ptr(tile_bins), ptr(packed), rs, ex, ptr(_f32(background)),
+                ptr(_f32(final_Ts)), ptr(final_idx), ptr(v_output), ptr(v_output_alpha), ptr(status), ptr(order), ptr(ws),
+                nbytes, *[ptr(t) for t in outs], stream()))
+        else:
+            check(lib.b200_blend_backward_packed_ordered(
+                n, H, W, bw, S, ptr(gaussian_ids_sorted), ptr(tile_bins), ptr(packed), rs, ex, ptr(_f32(background)),
+                ptr(_f32(final_Ts)), ptr(final_idx), ptr(v_output), ptr(v_output_alpha), ptr(order),
+                *[ptr(t) for t in outs], 1, stream()))
     return outs
+
+
+def _blend_backward_outputs(n, num_entries, block_width, device):
+    """The six per-record outputs of a colour blend backward (v_xy, v_xy_abs, v_pix_vels, v_conic, v_colors, v_opacity)
+    -> (outs, ws, nbytes).  Under torch.use_deterministic_algorithms(True) the deterministic kernels overwrite the
+    outputs and need the workspace `ws` of `nbytes`; otherwise ws is None and the kernels accumulate into the outputs,
+    carved from one zero-filled allocation of 13 floats per record (each array 64-byte aligned inside it): one fill
+    instead of six memsets."""
+    f32 = dict(dtype=torch.float32, device=device)
+    if deterministic():
+        nbytes = _lib.load().b200_blend_backward_deterministic_ws_bytes(n, num_entries, block_width)
+        outs = (torch.empty((n, 2), **f32), torch.empty((n, 2), **f32), torch.empty((n, 2), **f32),
+                torch.empty((n, 3), **f32), torch.empty((n, 3), **f32), torch.empty((n, 1), **f32))
+        return outs, _lib.workspace(nbytes, device), nbytes
+    pitch = (n + 15) & ~15
+    acc = torch.zeros(13 * pitch, **f32)
+    v_xy, v_xy_abs, v_pix = (acc[k * 2 * pitch:k * 2 * pitch + 2 * n].view(n, 2) for k in range(3))
+    v_conic, v_colors = (acc[6 * pitch + k * 3 * pitch:6 * pitch + k * 3 * pitch + 3 * n].view(n, 3) for k in range(2))
+    v_opacity = acc[12 * pitch:12 * pitch + n].view(n, 1)
+    return (v_xy, v_xy_abs, v_pix, v_conic, v_colors, v_opacity), None, 0
 
 
 def fused_preprocess_backward(device, *args):
@@ -496,44 +495,42 @@ def blend_backward_views(views, num_records, img_height, img_width, block_width,
     rs, ex = float(rolling_shutter_time), float(exposure_time)
     lib = _lib.load()
     with on_device(dev):
-        f32 = dict(dtype=torch.float32, device=dev)
         v_output = _f32(v_output).contiguous()
         v_output_alpha = _f32(v_output_alpha).contiguous() if v_output_alpha is not None else None
+        m = gaussian_ids_sorted.numel()
+        outs, ws, nbytes = _blend_backward_outputs(n, m, bw, dev)
         order = _tile_order(tile_bins, H, W, bw, B)
-        if deterministic():
-            m = gaussian_ids_sorted.numel()
-            nbytes = lib.b200_blend_backward_deterministic_ws_bytes(n, m, bw)
-            ws = _lib.workspace(nbytes, dev)
-            outs = (torch.empty((n, 2), **f32), torch.empty((n, 2), **f32), torch.empty((n, 2), **f32),
-                    torch.empty((n, 3), **f32), torch.empty((n, 3), **f32), torch.empty((n, 1), **f32))
+        if ws is not None:
             check(lib.b200_blend_backward_views_deterministic(
                 B, n, m, H, W, bw, S, ptr(gaussian_ids_sorted), ptr(tile_bins), ptr(packed), rs, ex, ptr(_f32(background)),
                 ptr(_f32(final_Ts)), ptr(final_idx), ptr(v_output), ptr(v_output_alpha), ptr(order), ptr(ws), nbytes,
                 *[ptr(t) for t in outs], stream()))
-            return outs
-        pitch = (n + 15) & ~15  # one zero-filled allocation, as in blend_backward_packed
-        acc = torch.zeros(13 * pitch, **f32)
-        v_xy, v_xy_abs, v_pix = (acc[k * 2 * pitch:k * 2 * pitch + 2 * n].view(n, 2) for k in range(3))
-        v_conic, v_colors = (acc[6 * pitch + k * 3 * pitch:6 * pitch + k * 3 * pitch + 3 * n].view(n, 3) for k in range(2))
-        v_opacity = acc[12 * pitch:12 * pitch + n].view(n, 1)
-        check(lib.b200_blend_backward_views(
-            B, n, H, W, bw, S, ptr(gaussian_ids_sorted), ptr(tile_bins), ptr(packed), rs, ex, ptr(_f32(background)),
-            ptr(_f32(final_Ts)), ptr(final_idx), ptr(v_output), ptr(v_output_alpha), ptr(order), ptr(v_xy), ptr(v_xy_abs),
-            ptr(v_pix), ptr(v_conic), ptr(v_colors), ptr(v_opacity), 1, stream()))
-    return v_xy, v_xy_abs, v_pix, v_conic, v_colors, v_opacity
+        else:
+            check(lib.b200_blend_backward_views(
+                B, n, H, W, bw, S, ptr(gaussian_ids_sorted), ptr(tile_bins), ptr(packed), rs, ex, ptr(_f32(background)),
+                ptr(_f32(final_Ts)), ptr(final_idx), ptr(v_output), ptr(v_output_alpha), ptr(order),
+                *[ptr(t) for t in outs], 1, stream()))
+    return outs
 
 
-def fused_preprocess_backward_views(device, *args):
-    """b200_fused_preprocess_backward_views with `args` as in include/b200splat.h up to the stream; camera sums in block
-    order under torch.use_deterministic_algorithms(True)."""
+def fused_preprocess_backward_views(device, *args, v_depth=None):
+    """b200_fused_preprocess_backward_views with `args` as in include/b200splat.h up to the stream.  v_depth (a device
+    pointer to views * N depth cotangents, or None): b200_fused_preprocess_backward_views_depth, which takes it after
+    v_opacity.  Camera sums in block order under torch.use_deterministic_algorithms(True)."""
     lib = _lib.load()
     views, n, g_cam = int(args[0]), int(args[1]), args[-3:]
+    if v_depth is None:
+        run, run_det = lib.b200_fused_preprocess_backward_views, lib.b200_fused_preprocess_backward_views_deterministic
+    else:
+        run = lib.b200_fused_preprocess_backward_views_depth
+        run_det = lib.b200_fused_preprocess_backward_views_depth_deterministic
+        args = (*args[:-9], v_depth, *args[-9:])  # ahead of the 6 raw-parameter and 3 camera gradient pointers
     if deterministic() and any(p is not None for p in g_cam):
         nbytes = lib.b200_fused_preprocess_backward_views_ws_bytes(views, n)
         ws = _lib.workspace(nbytes, device)
-        check(lib.b200_fused_preprocess_backward_views_deterministic(*args, ptr(ws), nbytes, stream()))
+        check(run_det(*args, ptr(ws), nbytes, stream()))
     else:
-        check(lib.b200_fused_preprocess_backward_views(*args, stream()))
+        check(run(*args, stream()))
 
 
 # ---- differentiable depth (include/b200splat.h "differentiable depth"): records of the fused forward ----------------
@@ -587,19 +584,6 @@ def blend_depth_backward(views, num_records, img_height, img_width, block_width,
                 B, n, H, W, bw, ptr(gaussian_ids_sorted), ptr(tile_bins), ptr(packed), ptr(_f32(final_T)), ptr(final_idx),
                 ptr(v_depth_img), ptr(order), ptr(v_xy), ptr(v_conic), ptr(v_opacity), ptr(v_depth), stream()))
     return v_depth
-
-
-def fused_preprocess_backward_views_depth(device, *args):
-    """b200_fused_preprocess_backward_views_depth with `args` as in include/b200splat.h up to the stream; camera sums in
-    block order under torch.use_deterministic_algorithms(True)."""
-    lib = _lib.load()
-    views, n, g_cam = int(args[0]), int(args[1]), args[-3:]
-    if deterministic() and any(p is not None for p in g_cam):
-        nbytes = lib.b200_fused_preprocess_backward_views_ws_bytes(views, n)
-        ws = _lib.workspace(nbytes, device)
-        check(lib.b200_fused_preprocess_backward_views_depth_deterministic(*args, ptr(ws), nbytes, stream()))
-    else:
-        check(lib.b200_fused_preprocess_backward_views_depth(*args, stream()))
 
 
 def _geom(tile_bounds, block, img_size):
