@@ -96,6 +96,23 @@ __device__ __forceinline__ float butterfly16(const float (&v)[16], int lane) {
     return w1;
 }
 
+// Whether something was blended into the pixel: final T < 1 at some sample.  Both kernels read a pixel's cotangents
+// only then.  A pixel with final T = 1 at every sample passes no Gaussian in the backward either: its final_idx is 0,
+// and the only entry that index admits, list position 0, was rejected there by the forward's identical sigma and alpha
+// tests.  So it contributes nothing, as in the reference's per-pixel skip, even where its cotangent is not finite
+// (Splatfacto's depth division at alpha = 0 gives 0 / 0 there).  Without this, the terms that stay outside the
+// per-sample tests would carry such a NaN into every Gaussian the warp visits: the masked halves of the paired
+// kernel, and the one-pixel kernel's rgb sums (facsum * v_out).
+template <int S>
+__device__ __forceinline__ bool covered_pixel(const BlendBwdParams &p, bool inside, size_t pix) {
+    bool covered = false;
+    if (inside) {
+#pragma unroll
+        for (int s = 0; s < S; ++s) covered = covered || p.final_Ts[pix * S + s] < 1.f;
+    }
+    return covered;
+}
+
 // ---- one pixel per lane: tiles other than 16x16 ---------------------------------------------------------------------
 // DET: the visit epilogue stores its sums to p.slots instead of adding them to the gradient arrays (deterministic mode)
 template <int S, bool DET>
@@ -122,7 +139,7 @@ __global__ void __launch_bounds__(BLEND_THREADS, 3) blend_backward_kernel(const 
     // per-pixel cotangents and per-sample state (backward.cu:198-217)
     const size_t pix = inside ? (size_t)(view * p.g.H + i) * p.g.W + j : 0;
     float vo0 = 0.f, vo1 = 0.f, vo2 = 0.f, voa = 0.f;
-    if (inside) {
+    if (covered_pixel<S>(p, inside, pix)) {
         vo0 = p.v_out[3 * pix]; vo1 = p.v_out[3 * pix + 1]; vo2 = p.v_out[3 * pix + 2];
         voa = p.v_out_alpha ? p.v_out_alpha[pix] : 0.f;
     }
@@ -299,7 +316,7 @@ __global__ void __launch_bounds__(128, BWD_MIN_CTAS) blend_backward_kernel2(cons
         const size_t pix = inside[q] ? (size_t)(view * p.g.H + i) * p.g.W + j : 0;
         float voa = 0.f;
         vo[q][0] = vo[q][1] = vo[q][2] = 0.f;
-        if (inside[q]) {
+        if (covered_pixel<S>(p, inside[q], pix)) {
             vo[q][0] = p.v_out[3 * pix]; vo[q][1] = p.v_out[3 * pix + 1]; vo[q][2] = p.v_out[3 * pix + 2];
             voa = p.v_out_alpha ? p.v_out_alpha[pix] : 0.f;
         }
@@ -441,6 +458,7 @@ __global__ void __launch_bounds__(128, BWD_MIN_CTAS) blend_backward_kernel2(cons
                         if (ok0) B200_COUNT(4, 1);
                         if (ok1) B200_COUNT(4, 1);
                         // masked pixels: vis = alpha = 0  =>  ra = 1, fac = 0, v_sigma = 0, every accumulated term exactly 0
+                        // (the cotangents are finite or, at a pixel nothing was blended into, not read: covered_pixel)
                         const f2 vis = f2_make(ok0 ? v0 : 0.f, ok1 ? v1 : 0.f);
                         const f2 alpha = f2_make(ok0 ? a0 : 0.f, ok1 ? a1 : 0.f);
                         const f2 nov = f2_mul(NOP, vis);  // -opacity * exp(-sigma)

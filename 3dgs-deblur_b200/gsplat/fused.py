@@ -41,8 +41,11 @@ def render_gaussians(means: Tensor, log_scales: Tensor, quats: Tensor, opacity_l
     with exposure: then they do not provably contain the static lists).
     depth_grad: make info["depth"] differentiable (needs return_depth): its gradient reaches the Gaussians' positions,
     shapes, opacities and depths through D, and the colour pass through alpha.  The values are the same bit for bit as
-    without it; without it info["depth"] does not require grad.  As in Splatfacto, a pixel where alpha is 0 has a NaN
-    gradient (0 / 0 in the division's backward), so a depth loss belongs on pixels that something covers.
+    without it; without it info["depth"] does not require grad.  As in Splatfacto, the division's backward gives a pixel
+    where alpha is 0 a NaN cotangent for D and alpha (0 / 0), whatever the depth loss is there.  Nothing was blended into
+    such a pixel, so, as in the reference kernels, it contributes nothing to any gradient: the Gaussians' and the
+    cameras' gradients stay finite.  (The static depth pass can still reach a pixel the colour pass missed, when the
+    colour pass has motion blur or rolling shutter; its NaN then reaches the Gaussians that cover it in the depth pass.)
 
     grad_sink (optional): {"means", "log_scales", "quats", "opacity_logit", "sh_dc", "sh_rest"} -> preallocated
     gradient buffers (e.g. slices of a flat DP buffer).  When given, backward OVERWRITES them directly (every row,

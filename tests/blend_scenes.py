@@ -194,6 +194,18 @@ def ragged(rng, H, W, S=3, rs=0.02, exposure=0.02, empty_tile=False):
     return make(f"ragged_{H}x{W}", H, W, S, rs, exposure, g, rng)
 
 
+def silhouette(rng, name, H, W, S, rs, exposure):
+    """Small sparse Gaussians confined to the part of the image left of x = 0.45 W, on an image that is not whole tiles:
+    the covered region ends inside 8x8 warp blocks and partial bottom tiles, and leaves holes, so uncovered pixels
+    (final T = 1 at every sample) share warps, and in the paired kernels a lane's pixel pair, with covered ones, in
+    tiles whose lists are not empty."""
+    n = 90
+    g = gaussians(rng, n, H, W, sig=(0.8, 2.5), op=(0.3, 0.95), vel=40.0 if S > 1 or rs else 0.0, S=S, rs=rs,
+                  exposure=exposure)
+    g["xys"] = np.stack([rng.uniform(0, 0.45 * W, n), rng.uniform(0, H, n)], 1)
+    return make(name, H, W, S, rs, exposure, g, rng)
+
+
 def _builders():
     b = {
         "deep_stacks": lambda r: deep_stacks(r),
@@ -210,11 +222,27 @@ def _builders():
     for H, W in RAGGED_SIZES:
         b[f"ragged_{H}x{W}"] = functools.partial(ragged, H=H, W=W, empty_tile=(H, W) == (47, 49))
     b["ragged_1080x24"] = functools.partial(ragged, H=1080, W=24, S=2, rs=0.03, exposure=0.02)
+    b["silhouette_45x61"] = lambda r: silhouette(r, "silhouette_45x61", 45, 61, 1, 0.0, 0.0)
+    b["silhouette_37x53_rs"] = lambda r: silhouette(r, "silhouette_37x53_rs", 37, 53, 3, 0.03, 0.02)
     return b
 
 
 BUILDERS = _builders()
 NAMES = list(BUILDERS)
+# the scenes with uncovered pixels in tiles whose lists are not empty
+UNCOVERED_NAMES = ["ragged_47x49", "silhouette_45x61", "silhouette_37x53_rs"]
+
+
+def uncovered(sc):
+    """(H, W) bool: the pixels where the reference's final T is 1 at every sample (nothing was blended into them)."""
+    return (sc["ref"]["final_Ts"] == 1.0).all(-1)
+
+
+def with_nan(sc, v_out, v_alpha, where):
+    """Copies of the cotangents with NaN in v_out (`where` = "rgb") or in v_alpha ("alpha") at the uncovered pixels."""
+    v_out, v_alpha = v_out.copy(), v_alpha.copy()
+    (v_out if where == "rgb" else v_alpha)[uncovered(sc)] = np.nan
+    return v_out, v_alpha
 
 
 @functools.lru_cache(maxsize=None)

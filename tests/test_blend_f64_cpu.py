@@ -80,6 +80,41 @@ def test_scene_families_exercise_their_edges():
         assert B.get(f"ragged_{H}x{W}")["H"] == H
     mo = B.get("motion_S10_long")
     assert (np.abs(mo["pix_vels"]).max(1) * mo["exposure"] > mo["W"]).any()
+    # uncovered pixels beside covered ones: in a lane's pixel pair, in a listed partial tile
+    for name in B.UNCOVERED_NAMES:
+        sc = B.get(name)
+        H, W, bins = sc["H"], sc["W"], sc["bins"]["tile_bins"]
+        unc = B.uncovered(sc)
+        i, j = np.mgrid[:H, :W]
+        listed = (bins[(i // 16) * ((W + 15) // 16) + j // 16] @ np.array([-1, 1])) > 0
+        partner = np.where(i % 8 < 4, i + 4, i - 4)  # rows r and r + 4 of an 8x8 warp block share a lane
+        mixed = unc & listed & (partner < H) & ~unc[np.minimum(partner, H - 1), j]
+        edge = (i >= H // 16 * 16) | (j >= W // 16 * 16)
+        assert mixed.any() and (name.startswith("ragged") or (unc & listed & edge).any()), name
+    assert B.get("silhouette_45x61")["S"] == 1 and B.get("silhouette_37x53_rs")["rs"] != 0.0
+
+
+@pytest.mark.parametrize("where", ["alpha", "rgb"])
+@pytest.mark.parametrize("name", B.UNCOVERED_NAMES)
+def test_nan_cotangents_at_uncovered_pixels_reach_no_gaussian(name, where):
+    """NaN in v_alpha, or in v_rgb, at the pixels nothing was blended into: the float64 reference gives exactly the
+    gradients of zeros there, and the C oracle, which skips such pixels as the reference kernel does, stays finite and
+    within the float64 bound of those gradients."""
+    sc = B.get(name)
+    b, ref = sc["bins"], sc["ref"]
+    Ts32 = ref["final_Ts"].astype(np.float32)
+    v_nan, a_nan = B.with_nan(sc, *cotangents(sc, 7, True), where)
+    v_zero, a_zero = np.nan_to_num(v_nan, nan=0.0), np.nan_to_num(a_nan, nan=0.0)
+    with np.errstate(invalid="ignore"):
+        g_nan = ref_backward(sc, Ts32, ref["final_idx"], v_nan, a_nan)
+    g_ref = ref_backward(sc, Ts32, ref["final_idx"], v_zero, a_zero)
+    g = O.rasterize_backward(sc["H"], sc["W"], B.BW, sc["S"], b["gaussian_ids_sorted"], b["tile_bins"], sc["xys"],
+                             sc["pix_vels"], sc["rs"], sc["exposure"], sc["conics"], sc["colors"], sc["opac"],
+                             sc["background"], Ts32, ref["final_idx"], v_nan, a_nan)
+    for k in F.GRAD_KEYS:
+        assert np.array_equal(g_nan[k], g_ref[k]) and np.array_equal(g_nan["err"][k], g_ref["err"][k]), k
+        assert np.isfinite(g[k]).all(), f"C oracle {k}: non-finite"
+        assert_within(g[k], g_ref[k], g_ref["err"][k], f"C oracle {k}, NaN in v_{where}")
 
 
 @pytest.mark.parametrize("name,n,S,rs,exposure,H,W", [("c2", 6000, 3, 1 / 50, 1 / 60, 64, 96),

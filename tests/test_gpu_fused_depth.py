@@ -69,8 +69,11 @@ def test_depth_forward_is_channel_0_of_the_recoloured_blend(case, lists):
 
 def _backdrop(sc, view):
     """Append one large, opaque Gaussian 50 units in front of the camera (behind the scene's room, out of sight of the
-    camera that looks away), so alpha > 0 at every pixel: where alpha is 0,
-    Splatfacto's `where(alpha > 0, D / alpha, ...)` has a NaN gradient (0 / 0), on the drop-in chain and here alike."""
+    camera that looks away), so alpha > 0 at every pixel and every pixel's depth is D / alpha.  Where alpha is 0,
+    Splatfacto's `where(alpha > 0, D / alpha, ...)` gives D and alpha NaN cotangents (0 / 0).  Pixels nothing was
+    blended into then add nothing (tests/test_gpu_uncovered_pixels.py), but with blur or rolling shutter the static
+    depth pass can cover a pixel the colour pass missed, and that pixel's NaN legitimately reaches the Gaussians
+    covering it."""
     vm = view["viewmat"][:3, :4].double()
     p = vm[:, :3].t() @ (torch.tensor([0.0, 0.0, 50.0], device="cuda", dtype=torch.float64) - vm[:, 3])
     extra = dict(means=p.float()[None], log_scales=torch.full((1, 3), 4.0, device="cuda"),
@@ -188,29 +191,43 @@ def test_depth_grad_changes_no_value(case):
     assert out[1][2]["depth"].requires_grad and not out[0][2]["depth"].requires_grad
 
 
+CAM = ("viewmat", "lin", "ang")
+
+
 def _batch_grads(sc, views, cot, deterministic):
-    """(batch gradients, single-view gradients added in view order) of <v_rgb, rgb> + <v_a, alpha> + <v_d, depth>."""
+    """(batch gradients, single-view gradients) of <v_rgb, rgb> + <v_a, alpha> + <v_d, depth>, each a dict: the raw
+    parameters and "bg" (the single views' added in view order), "viewmat" / "lin" / "ang" stacked per view, and
+    "absgrad" (B,N,2)."""
     torch.use_deterministic_algorithms(deterministic)
     try:
         B = len(views)
         p = {k: sc[k].detach().clone().requires_grad_(True) for k in RAW}
-        args = [torch.stack([v[k] for v in views]) for k in ("viewmat", "cam_pos", "lin", "ang")]
+        cam = {k: torch.stack([v[k] for v in views]).requires_grad_(True) for k in CAM}
+        bg = sc["background"].clone().requires_grad_(True)
         intr = [torch.tensor([v[k] for v in views], device="cuda") for k in ("fx", "fy", "cx", "cy")]
-        rgb, alpha, info = render_gaussians_batch(*(p[k] for k in RAW), *args, *intr, sc["H"], sc["W"], sc["bw"],
-                                                  sc["background"], sc["rs"], sc["ex"], sc["S"], return_depth=True,
-                                                  depth_grad=True)
+        pos = torch.stack([v["cam_pos"] for v in views])
+        rgb, alpha, info = render_gaussians_batch(*(p[k] for k in RAW), cam["viewmat"], pos, cam["lin"], cam["ang"],
+                                                  *intr, sc["H"], sc["W"], sc["bw"], bg, sc["rs"], sc["ex"], sc["S"],
+                                                  return_depth=True, depth_grad=True)
         loss = sum((rgb[v] * cot[v][0]).sum() + (alpha[v] * cot[v][1]).sum() + (info["depth"][v] * cot[v][2]).sum()
                    for v in range(B))
-        batch = torch.autograd.grad(loss, [p[k] for k in RAW])
-        single = None
+        keys = RAW + CAM + ("bg",)
+        batch = dict(zip(keys, torch.autograd.grad(loss, [p[k] for k in RAW] + [cam[k] for k in CAM] + [bg])))
+        batch["absgrad"] = info["absgrad"]
+        single = {}
         for v in range(B):
-            q = {k: sc[k].detach().clone().requires_grad_(True) for k in RAW}
-            r1, a1, i1 = _fused(sc, views[v], dict(q, lin=views[v]["lin"], ang=views[v]["ang"], viewmat=views[v]["viewmat"],
-                                                   bg=sc["background"]))
+            q = _leaves(sc, views[v])
+            r1, a1, i1 = _fused(sc, views[v], q)
             assert torch.equal(r1, rgb[v]) and torch.equal(a1, alpha[v]) and torch.equal(i1["depth"], info["depth"][v])
             l1 = (r1 * cot[v][0]).sum() + (a1 * cot[v][1]).sum() + (i1["depth"] * cot[v][2]).sum()
-            g1 = torch.autograd.grad(l1, [q[k] for k in RAW])
-            single = g1 if single is None else tuple(x + y for x, y in zip(single, g1))
+            g1 = dict(zip(keys, torch.autograd.grad(l1, [q[k] for k in keys])))
+            for k in RAW + ("bg",):
+                single[k] = g1[k] if v == 0 else single[k] + g1[k]
+            for k in CAM:
+                single.setdefault(k, []).append(g1[k])
+            single.setdefault("absgrad", []).append(i1["absgrad"])
+        for k in CAM + ("absgrad",):
+            single[k] = torch.stack(single[k])
         return batch, single
     finally:
         torch.use_deterministic_algorithms(False)
@@ -218,20 +235,23 @@ def _batch_grads(sc, views, cot, deterministic):
 
 @pytest.mark.parametrize("case", ["blur5", "bw8"])
 def test_batch_depth_grad_is_the_sum_of_single_views(case):
-    """Views: camera 0, a camera that sees nothing (empty render, D = 0), camera 0 again.  Default mode: close to the
-    single-view sums; deterministic mode: equal to them bit for bit, and bit-identical from run to run."""
+    """Views: camera 0, a camera that sees nothing (empty render, D = 0), camera 0 again.  Raw-parameter and background
+    gradients against the single views' sums, view-matrix / velocity gradients and absgrad against each single view's.
+    Default mode: close to them; deterministic mode: equal to them bit for bit, and bit-identical from run to run."""
     sc = _scene(case)
     views = _views(sc, 3)
     sc = _backdrop(sc, views[0])
     cot = [_cotangents(sc, seed=10 + v) for v in range(3)]
     batch, single = _batch_grads(sc, views, cot, deterministic=False)
-    for k, x, y in zip(RAW, batch, single):
-        grad_close(x, y, name=k)
+    for k in single:
+        grad_close(batch[k], single[k], name=k)
     batch, single = _batch_grads(sc, views, cot, deterministic=True)
     again, _ = _batch_grads(sc, views, cot, deterministic=True)
-    for k, x, y, z in zip(RAW, batch, single, again):
-        assert torch.equal(x, y), k
-        assert torch.equal(x, z), k
+    for k in single:
+        assert torch.equal(batch[k], single[k]), k
+        assert torch.equal(batch[k], again[k]), k
+    for k in CAM + ("absgrad",):
+        assert bool((batch[k][1] == 0).all()), f"{k}: the empty view has a nonzero gradient"
 
 
 def test_empty_render_gives_zero_depth_and_zero_depth_gradients():
