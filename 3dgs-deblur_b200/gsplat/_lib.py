@@ -120,6 +120,31 @@ SIGNATURES = {
     "b200_nd_rasterize_backward": (_i, [_i, _u, _u, _u, _u, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p,
                                         _p, _p, _p, _p, _p, _p]),
 }
+# render modes: each *_mode entry point is its base entry point behind a leading mode word (the view-batch backward's base
+# is the _depth one: v_depth is nullable there)
+OPACITY_CLASSIC, COLOR_SIGMOID = 1, 2  # B200_OPACITY_CLASSIC, B200_COLOR_SIGMOID
+for _mode_fn, _base in (("b200_fused_preprocess_forward_views_mode", "b200_fused_preprocess_forward_views"),
+                        ("b200_fused_preprocess_backward_views_mode", "b200_fused_preprocess_backward_views_depth"),
+                        ("b200_fused_preprocess_backward_views_mode_deterministic",
+                         "b200_fused_preprocess_backward_views_depth_deterministic"),
+                        ("b200_fused_geometry_forward_mode", "b200_fused_geometry_forward"),
+                        ("b200_fused_colors_forward_mode", "b200_fused_colors_forward"),
+                        ("b200_fused_preprocess_backward_mode", "b200_fused_preprocess_backward"),
+                        ("b200_fused_preprocess_backward_mode_deterministic",
+                         "b200_fused_preprocess_backward_deterministic")):
+    SIGNATURES[_mode_fn] = (_i, [_u, *SIGNATURES[_base][1]])
+del _mode_fn, _base
+
+
+def render_mode(rasterize_mode: str, color_mode: str, caller: str) -> int:
+    """The mode word of Splatfacto's two render switches: rasterize_mode "antialiased" (sigmoid(logit) * compensation) or
+    "classic" (sigmoid(logit)); color_mode "sh" (clamp(SH + 0.5, 0)) or "sigmoid" (sigmoid(sh_dc), sh_degree 0).
+    Anything else is a ValueError."""
+    if rasterize_mode not in ("antialiased", "classic"):
+        raise ValueError(f"{caller}: rasterize_mode must be 'antialiased' or 'classic', got {rasterize_mode!r}")
+    if color_mode not in ("sh", "sigmoid"):
+        raise ValueError(f"{caller}: color_mode must be 'sh' or 'sigmoid', got {color_mode!r}")
+    return (OPACITY_CLASSIC if rasterize_mode == "classic" else 0) | (COLOR_SIGMOID if color_mode == "sigmoid" else 0)
 
 _LIB = None
 

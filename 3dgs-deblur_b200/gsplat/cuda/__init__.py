@@ -5,6 +5,8 @@ Same names, argument order and return tuples as the reference pybind module
 code and tests that do `import gsplat.cuda as _C` keep working.  Tensors are allocated here by
 PyTorch and handed to the C ABI (include/b200splat.h) as raw device pointers on the current stream.
 """
+import functools
+
 import torch
 
 from .. import _lib
@@ -400,15 +402,21 @@ def _blend_backward_outputs(n, num_entries, block_width, device):
     return (v_xy, v_xy_abs, v_pix, v_conic, v_colors, v_opacity), None, 0
 
 
-def fused_preprocess_backward(device, *args):
+def fused_preprocess_backward(device, *args, mode=0):
     """b200_fused_preprocess_backward with `args` as in include/b200splat.h up to the stream; under
-    torch.use_deterministic_algorithms(True) the camera sums go through the _deterministic entry point."""
+    torch.use_deterministic_algorithms(True) the camera sums go through the _deterministic entry point.  mode: the render
+    mode word (gsplat._lib.render_mode; 0 = "antialiased" opacities and SH colours), run by the _mode entry points."""
     lib = _lib.load()
     n, g_cam = int(args[0]), args[-3:]
     if deterministic() and any(p is not None for p in g_cam):
         nbytes = lib.b200_fused_preprocess_backward_ws_bytes(n)
         ws = _lib.workspace(nbytes, device)
-        check(lib.b200_fused_preprocess_backward_deterministic(*args, ptr(ws), nbytes, stream()))
+        if mode:
+            check(lib.b200_fused_preprocess_backward_mode_deterministic(mode, *args, ptr(ws), nbytes, stream()))
+        else:
+            check(lib.b200_fused_preprocess_backward_deterministic(*args, ptr(ws), nbytes, stream()))
+    elif mode:
+        check(lib.b200_fused_preprocess_backward_mode(mode, *args, stream()))
     else:
         check(lib.b200_fused_preprocess_backward(*args, stream()))
 
@@ -513,13 +521,18 @@ def blend_backward_views(views, num_records, img_height, img_width, block_width,
     return outs
 
 
-def fused_preprocess_backward_views(device, *args, v_depth=None):
+def fused_preprocess_backward_views(device, *args, v_depth=None, mode=0):
     """b200_fused_preprocess_backward_views with `args` as in include/b200splat.h up to the stream.  v_depth (a device
     pointer to views * N depth cotangents, or None): b200_fused_preprocess_backward_views_depth, which takes it after
-    v_opacity.  Camera sums in block order under torch.use_deterministic_algorithms(True)."""
+    v_opacity.  Camera sums in block order under torch.use_deterministic_algorithms(True).  mode: the render mode word
+    (gsplat._lib.render_mode), run by b200_fused_preprocess_backward_views_mode(_deterministic) when not 0."""
     lib = _lib.load()
     views, n, g_cam = int(args[0]), int(args[1]), args[-3:]
-    if v_depth is None:
+    if mode:
+        run = functools.partial(lib.b200_fused_preprocess_backward_views_mode, mode)
+        run_det = functools.partial(lib.b200_fused_preprocess_backward_views_mode_deterministic, mode)
+        args = (*args[:-9], v_depth, *args[-9:])  # nullable there
+    elif v_depth is None:
         run, run_det = lib.b200_fused_preprocess_backward_views, lib.b200_fused_preprocess_backward_views_deterministic
     else:
         run = lib.b200_fused_preprocess_backward_views_depth

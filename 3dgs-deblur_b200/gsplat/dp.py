@@ -17,6 +17,7 @@ The densification statistics (xys.absgrad norms, visibility counts, max 2D radiu
 splatfacto.py:417-434) are exposed by `reduce_densify_stats` with the matching sum / sum / max
 reductions so a caller can keep topology changes identical across ranks.
 """
+import functools
 import gc
 import math
 import os
@@ -340,12 +341,14 @@ class ImageShardedTrainer:
 # update of step k hidden behind the geometry of image k+1.
 # ------------------------------------------------------------------------------------------------------------------
 
-def geometry_phase(model: FlatGaussians, st: Dict, scene: Dict, capacity: int, status: torch.Tensor):
+def geometry_phase(model: FlatGaussians, st: Dict, scene: Dict, capacity: int, status: torch.Tensor,
+                   rasterize_mode: str = "antialiased", color_mode: str = "sh"):
     """Phase A of a step -- everything that depends only on the GEOMETRY parameters (means, scales, quaternions,
     opacities, camera rows): the projection block of splatfacto.py:816-834 on the public operator, the opacity
     activation (:853-856) and the tile lists (gsplat.rasterize.prepare_lists: capacity mode, no host sync).
     `st` holds the step's camera as device tensors: cam (21 floats: viewmat 12 | lin_vel 3 | ang_vel 3 | cam_pos 3)
-    and cam_index (int64[1])."""
+    and cam_index (int64[1]).  rasterize_mode: "antialiased" (sigmoid(logit) * compensation) or "classic" (sigmoid(logit),
+    Splatfacto's default); color_mode is read by the shading phase."""
     from gsplat import project_gaussians
     from gsplat.rasterize import prepare_lists
 
@@ -363,7 +366,9 @@ def geometry_phase(model: FlatGaussians, st: Dict, scene: Dict, capacity: int, s
     xys, depths, pix_vels, radii, conics, comp, num_tiles_hit, _ = project_gaussians(
         p["means"], torch.exp(p["log_scales"]), 1, quats, lin, ang, rs, ex, viewmat, scene["fx"], scene["fy"], scene["cx"],
         scene["cy"], H, W, bw)
-    opacities = torch.sigmoid(p["opacity_logit"]) * comp[:, None]  # "antialiased" mode, splatfacto.py:853-854
+    opacities = torch.sigmoid(p["opacity_logit"])  # splatfacto.py:853-856
+    if rasterize_mode == "antialiased":
+        opacities = opacities * comp[:, None]
     blur = scene["blur_samples"] if ex > 0 else 1
     prep = prepare_lists(xys, depths, pix_vels, radii, conics, num_tiles_hit, opacities, H, W, bw, rs, ex, blur,
                          capacity=capacity, status=status)
@@ -371,10 +376,12 @@ def geometry_phase(model: FlatGaussians, st: Dict, scene: Dict, capacity: int, s
                 opacities=opacities, prep=prep, cam_pos=cam_pos, blur=blur)
 
 
-def shading_phase(model: FlatGaussians, geo: Dict, scene: Dict, target: torch.Tensor, loss_fn, sh_degree_to_use: int = 3):
+def shading_phase(model: FlatGaussians, geo: Dict, scene: Dict, target: torch.Tensor, loss_fn, sh_degree_to_use: int = 3,
+                  rasterize_mode: str = "antialiased", color_mode: str = "sh"):
     """Phase B -- needs the SH parameters: colours (splatfacto.py:840-852), blend on the prepared lists, loss, and the
     backward pass through BOTH phases.  With the block layout the SH gradient goes straight into the flat gradient
-    buffer (gsplat.sh.coeff_grad_sink).  Returns the (device) loss."""
+    buffer (gsplat.sh.coeff_grad_sink).  color_mode "sigmoid": sigmoid of the dc coefficients (Splatfacto at sh_degree 0,
+    splatfacto.py:847-848) instead of clamp(SH + 0.5, 0).  Returns the (device) loss."""
     from gsplat import rasterize_gaussians, spherical_harmonics
     from gsplat.sh import coeff_grad_sink
 
@@ -382,8 +389,11 @@ def shading_phase(model: FlatGaussians, geo: Dict, scene: Dict, target: torch.Te
     H, W, bw = scene["H"], scene["W"], scene["block_width"]
     viewdirs = p["means"].detach() - geo["cam_pos"]
     sink = model.flat_grad[model.sh_start:model.sh_start + model.N * model.K * 3] if model.sh_layout == "block" else None
-    with coeff_grad_sink(sink):
-        rgbs = torch.clamp(spherical_harmonics(sh_degree_to_use, viewdirs, model.sh_coeffs()) + 0.5, min=0.0)
+    if color_mode == "sigmoid":
+        rgbs = torch.sigmoid(model.sh_coeffs()[:, 0, :])
+    else:
+        with coeff_grad_sink(sink):
+            rgbs = torch.clamp(spherical_harmonics(sh_degree_to_use, viewdirs, model.sh_coeffs()) + 0.5, min=0.0)
     rgb, alpha = rasterize_gaussians(geo["xys"], geo["depths"], geo["pix_vels"], geo["radii"], geo["conics"],
                                      geo["num_tiles_hit"], rgbs, geo["opacities"], H, W, bw,
                                      rolling_shutter_time=scene["rolling_shutter_time"], exposure_time=scene["exposure_time"],
@@ -394,12 +404,13 @@ def shading_phase(model: FlatGaussians, geo: Dict, scene: Dict, target: torch.Te
     return loss.detach()
 
 
-def fused_geometry_phase(model: FlatGaussians, st: Dict, scene: Dict, capacity: int, status: torch.Tensor):
+def fused_geometry_phase(model: FlatGaussians, st: Dict, scene: Dict, capacity: int, status: torch.Tensor,
+                         rasterize_mode: str = "antialiased", color_mode: str = "sh"):
     """Phase A straight on the C ABI, raw parameters in: ONE kernel (b200_fused_geometry_forward: exp, quaternion
     normalisation, projection, sigmoid * compensation, blend record -- what `geometry_phase` spends 11 launches on, 8 of
     them PyTorch glue) + the capacity-mode binning.  Same interface and the same numbers as `geometry_phase` up to
     float rounding of the activations.  No autograd graph: `fused_shading_phase` differentiates with
-    b200_fused_preprocess_backward."""
+    b200_fused_preprocess_backward.  rasterize_mode as in `geometry_phase` (b200_fused_geometry_forward_mode)."""
     import gsplat.cuda as _C
     from gsplat import _lib
     from gsplat._lib import check, ptr, stream
@@ -421,21 +432,27 @@ def fused_geometry_phase(model: FlatGaussians, st: Dict, scene: Dict, capacity: 
             depths = torch.empty((n,), dtype=torch.float32, device=dev)
             radii = torch.empty((n,), dtype=torch.int32, device=dev)
             nth = torch.empty((n,), dtype=torch.int32, device=dev)
-            check(lib.b200_fused_geometry_forward(
-                n, ptr(p["means"]), ptr(p["log_scales"]), ptr(p["quats"]), ptr(p["opacity_logit"]), ptr(cam), ptr(vel[:3]),
-                ptr(vel[3:]), rs, ex, float(scene["fx"]), float(scene["fy"]), float(scene["cx"]), float(scene["cy"]), H, W, bw,
-                _CLIP_THRESH, ptr(packed), ptr(depths), ptr(radii), ptr(nth), stream()))
+            args = (n, ptr(p["means"]), ptr(p["log_scales"]), ptr(p["quats"]), ptr(p["opacity_logit"]), ptr(cam),
+                    ptr(vel[:3]), ptr(vel[3:]), rs, ex, float(scene["fx"]), float(scene["fy"]), float(scene["cx"]),
+                    float(scene["cy"]), H, W, bw, _CLIP_THRESH, ptr(packed), ptr(depths), ptr(radii), ptr(nth), stream())
+            mode = _lib.render_mode(rasterize_mode, color_mode, "fused_geometry_phase")
+            if mode:
+                check(lib.b200_fused_geometry_forward_mode(mode, *args))
+            else:
+                check(lib.b200_fused_geometry_forward(*args))
             ids, bins = _C.bin_cull_capacity(packed, depths, radii, nth, H, W, bw, blur, rs, ex, capacity, status)
     return dict(packed=packed, depths=depths, radii=radii, num_tiles_hit=nth, ids=ids, bins=bins, vel=vel, cam=cam,
                 cam_index=st["cam_index"], status=status, blur=blur, absgrad=None)
 
 
-def fused_shading_phase(model: FlatGaussians, geo: Dict, scene: Dict, target: torch.Tensor, loss_fn, sh_degree_to_use: int = 3):
+def fused_shading_phase(model: FlatGaussians, geo: Dict, scene: Dict, target: torch.Tensor, loss_fn, sh_degree_to_use: int = 3,
+                        rasterize_mode: str = "antialiased", color_mode: str = "sh"):
     """Phase B on the C ABI: SH colours into the records (b200_fused_colors_forward), blend, `loss_fn` (autograd sees
     only loss_fn(rgb, target)), blend backward, and ONE kernel for everything behind it (b200_fused_preprocess_backward:
     SH, clamp, sigmoid * compensation, projection VJP, exp, normalisation) that writes the model's flat gradient buffer
     row by row -- no accumulate passes, no memsets.  The gradient rows are OVERWRITTEN (the buffer is zero between steps:
-    FlatAdam clears what it consumes); the camera-velocity row is accumulated."""
+    FlatAdam clears what it consumes); the camera-velocity row is accumulated.  The two render modes as in
+    `geometry_phase` / `shading_phase`, through the _mode entry points."""
     import gsplat.cuda as _C
     from gsplat import _lib
     from gsplat._lib import check, ptr, stream
@@ -451,9 +468,16 @@ def fused_shading_phase(model: FlatGaussians, geo: Dict, scene: Dict, target: to
     cam_pos = cam[18:21]
     bg = scene["background"]
     lib = _lib.load()
+    mode = _lib.render_mode(rasterize_mode, color_mode, "fused_shading_phase")
+    if mode & _lib.COLOR_SIGMOID:
+        sh_degree_to_use = 0  # sigmoid(sh_dc) reads no SH basis
     with torch.no_grad(), _lib.on_device(dev):
-        check(lib.b200_fused_colors_forward(n, ptr(p["means"]), ptr(p["sh_dc"]), ptr(p["sh_rest"]), K, sh_degree_to_use,
-                                            ptr(cam_pos), ptr(radii), ptr(packed), stream()))
+        args = (n, ptr(p["means"]), ptr(p["sh_dc"]), ptr(p["sh_rest"]), K, sh_degree_to_use, ptr(cam_pos), ptr(radii),
+                ptr(packed), stream())
+        if mode:
+            check(lib.b200_fused_colors_forward_mode(mode, *args))
+        else:
+            check(lib.b200_fused_colors_forward(*args))
         rgb, Ts, fi = _C.blend_forward_packed(H, W, bw, S, geo["ids"], geo["bins"], packed, rs, ex, bg, status=geo["status"])
     from gsplat.losses import l1_loss, l1_loss_and_grad
     if loss_fn is l1_loss:  # the default: value and cotangent from the one kernel
@@ -473,7 +497,7 @@ def fused_shading_phase(model: FlatGaussians, geo: Dict, scene: Dict, target: to
             ptr(p["sh_rest"]), K, sh_degree_to_use, ptr(cam), ptr(cam_pos), ptr(vel[:3]), ptr(vel[3:]), rs, ex, fx, fy, cx, cy,
             H, W, bw, _CLIP_THRESH, ptr(packed), ptr(radii), ptr(v_xy), ptr(v_pix), ptr(v_conic), ptr(v_col), ptr(v_op),
             ptr(g["means"]), ptr(g["log_scales"]), ptr(g["quats"]), ptr(g["opacity_logit"]), ptr(g["sh_dc"]), ptr(g["sh_rest"]),
-            ptr(g_vel[:3]) if g_vel is not None else None, ptr(g_vel[3:]) if g_vel is not None else None, None)
+            ptr(g_vel[:3]) if g_vel is not None else None, ptr(g_vel[3:]) if g_vel is not None else None, None, mode=mode)
         if g_vel is not None:
             g["cam_vel"].view(-1, 6).index_add_(0, geo["cam_index"], g_vel.view(1, 6))
     geo["absgrad"] = v_abs   # the `xys.absgrad` side channel of the drop-in operator (densification statistic)
@@ -528,15 +552,21 @@ class PipelinedTrainer:
 
     def __init__(self, model: FlatGaussians, scene: Dict, lr: float = 1e-3, group=None, loss_fn=None, use_graphs: bool = True,
                  capacity: Optional[int] = None, sh_degree_to_use: int = 3, geometry_fn=None, shading_fn=None,
-                 optimizer: str = "b200", sh_chunks: int = 1, operators: Optional[str] = None):
+                 optimizer: str = "b200", sh_chunks: int = 1, operators: Optional[str] = None,
+                 rasterize_mode: str = "antialiased", color_mode: str = "sh"):
         """operators: "dropin" = the two phases on the reference-compatible operators under autograd (`geometry_phase` /
         `shading_phase`); "fused" = on the fused raw-parameter kernels (`fused_geometry_phase` / `fused_shading_phase`:
-        same numbers, ~45 fewer launches per step); None = fused where it applies (CUDA, sh_layout "split"), else drop-in."""
+        same numbers, ~45 fewer launches per step); None = fused where it applies (CUDA, sh_layout "split"), else drop-in.
+        rasterize_mode ("antialiased" / "classic") and color_mode ("sh" / "sigmoid"): Splatfacto's two render switches, as
+        in gsplat.fused.render_gaussians; both operator sets serve them (injected phases are called as they are)."""
         self.model, self.scene = model, dict(scene)
         if loss_fn is None:
             from gsplat.losses import l1_loss as loss_fn
         self.loss_fn = loss_fn
         self.sh_degree = sh_degree_to_use
+        from gsplat._lib import render_mode
+        render_mode(rasterize_mode, color_mode, "PipelinedTrainer")  # ValueError for an unknown mode
+        self.rasterize_mode, self.color_mode = rasterize_mode, color_mode
         fusable = model.flat.device.type == "cuda" and model.sh_layout == "split"
         if operators is None:
             operators = "fused" if fusable else "dropin"
@@ -546,8 +576,9 @@ class PipelinedTrainer:
             raise ValueError("operators='fused' needs a CUDA model with sh_layout='split'")
         self.operators = operators
         phases = (fused_geometry_phase, fused_shading_phase) if operators == "fused" else (geometry_phase, shading_phase)
-        self.geometry_fn = geometry_fn or phases[0]   # (tests inject CPU stand-ins with the same interface)
-        self.shading_fn = shading_fn or phases[1]
+        modes = dict(rasterize_mode=rasterize_mode, color_mode=color_mode)
+        self.geometry_fn = geometry_fn or functools.partial(phases[0], **modes)  # (tests inject CPU stand-ins with the
+        self.shading_fn = shading_fn or functools.partial(phases[1], **modes)     # same interface)
         self.distributed = dist.is_available() and dist.is_initialized() and dist.get_world_size(group) > 1
         self.group = group
         self.rank = dist.get_rank(group) if self.distributed else 0
@@ -653,7 +684,7 @@ class PipelinedTrainer:
         # the deterministic mode records other kernels (and workspaces): toggling torch's flag captures new graphs
         return (s["H"], s["W"], s["fx"], s["fy"], s["cx"], s["cy"], s["block_width"], s["blur_samples"], s["exposure_time"],
                 s["rolling_shutter_time"], self.sh_degree, self.capacity, self.model.N,
-                torch.are_deterministic_algorithms_enabled())
+                torch.are_deterministic_algorithms_enabled(), self.rasterize_mode, self.color_mode)
 
     def _entry(self, target_shape_dtype):
         key = self._key() + (target_shape_dtype,)

@@ -7,7 +7,9 @@ rasterizer.  `render_gaussians` takes the raw parameter tensors, runs one fused 
 binning, the blend, and in backward one fused post-processing kernel.  It needs a caller change (hence "next");
 `gsplat.project_gaussians / spherical_harmonics / rasterize_gaussians` stay the drop-in surface.
 
-Outputs are the same as chaining the three drop-in operators the way Splatfacto does (tests/test_gpu_fused.py).
+Outputs are the same as chaining the three drop-in operators the way Splatfacto does (tests/test_gpu_fused.py), in
+either of its opacity modes and with SH or degree-0 sigmoid colours (`rasterize_mode`, `color_mode`;
+tests/test_gpu_fused_modes.py).
 `render_gaussians_batch` renders B cameras of the scene in one call (view v = the single-view render of camera v).
 Both run one autograd Function over the view-batch kernels: a single view is a batch of one.
 """
@@ -30,7 +32,7 @@ def render_gaussians(means: Tensor, log_scales: Tensor, quats: Tensor, opacity_l
                      img_width: int, block_width: int, background: Tensor, rolling_shutter_time: float = 0.0,
                      exposure_time: float = 0.0, blur_samples: int = 1, sh_degree_to_use: int = 3,
                      clip_thresh: float = 0.01, grad_sink: Optional[Dict[str, Tensor]] = None, return_depth: bool = False,
-                     depth_grad: bool = False):
+                     depth_grad: bool = False, rasterize_mode: str = "antialiased", color_mode: str = "sh"):
     """Returns (rgb (H,W,3), alpha (H,W), info).  info["radii"] (N,) int32; after backward info["absgrad"] (N,2) holds the
     abs-grad densification statistic (the `xys.absgrad` side channel of the drop-in operator).
 
@@ -51,7 +53,14 @@ def render_gaussians(means: Tensor, log_scales: Tensor, quats: Tensor, opacity_l
     gradient buffers (e.g. slices of a flat DP buffer).  When given, backward OVERWRITES them directly (every row,
     zeros for culled Gaussians) and autograd returns no gradient for those inputs -- no accumulate pass, no memset.
 
+    rasterize_mode, color_mode: Splatfacto's two render switches (splatfacto.py:842-858).  rasterize_mode "antialiased"
+    (the default) blends sigmoid(opacity_logit) * compensation, "classic" (Splatfacto's default config) sigmoid(opacity_logit).
+    color_mode "sh" (the default) colours clamp(SH(sh_dc, sh_rest) + 0.5, 0) up to sh_degree_to_use, "sigmoid" (Splatfacto
+    at sh_degree 0) sigmoid(sh_dc): sh_degree_to_use is then ignored, sh_rest may have any number of rows (also (N, 0, 3))
+    and its gradient is zeros.  The depth pass blends the same records, so it sees the same opacities.
+
     The camera is rendered as a batch of one view (render_gaussians_batch's kernels and autograd Function)."""
+    mode = _lib.render_mode(rasterize_mode, color_mode, "render_gaussians")
     if depth_grad and not return_depth:
         raise ValueError("render_gaussians: depth_grad=True needs return_depth=True")
     if linear_velocity is None:
@@ -66,7 +75,7 @@ def render_gaussians(means: Tensor, log_scales: Tensor, quats: Tensor, opacity_l
     rgb, alpha, info = _render(means, log_scales, quats, opacity_logit, sh_dc, sh_rest, viewmat[None], cam_pos.reshape(1, 3),
                                lin, ang, (fx, fy, cx, cy), img_height, img_width, block_width, background,
                                rolling_shutter_time, exposure_time, blur_samples, sh_degree_to_use, clip_thresh,
-                               return_depth, depth_grad, grad_sink, rows=(means.shape[0],))
+                               return_depth, depth_grad, grad_sink, rows=(means.shape[0],), mode=mode)
     if return_depth:
         info["depth"] = info["depth"].squeeze(0)
     return rgb.squeeze(0), alpha.squeeze(0), info
@@ -80,7 +89,8 @@ def render_gaussians_batch(means: Tensor, log_scales: Tensor, quats: Tensor, opa
                            angular_velocity: Optional[Tensor], fx, fy, cx, cy, img_height: int, img_width: int,
                            block_width: int, background: Tensor, rolling_shutter_time: float = 0.0,
                            exposure_time: float = 0.0, blur_samples: int = 1, sh_degree_to_use: int = 3,
-                           clip_thresh: float = 0.01, return_depth: bool = False, depth_grad: bool = False):
+                           clip_thresh: float = 0.01, return_depth: bool = False, depth_grad: bool = False,
+                           rasterize_mode: str = "antialiased", color_mode: str = "sh"):
     """`render_gaussians` for B cameras of one scene in one call: one fused pre-processing launch over B * N records,
     one culled binning with one host sync, one blend grid over the B * T tiles (longest lists first across all views).
 
@@ -97,7 +107,8 @@ def render_gaussians_batch(means: Tensor, log_scales: Tensor, quats: Tensor, opa
     own; the alpha-0 depth fill is that view's own maximum).  The raw-parameter and background gradients are the sums
     of the single-view ones over the views, the view-matrix and velocity gradients are per view; under
     torch.use_deterministic_algorithms(True) every gradient equals the single-view gradients added in view order, bit
-    for bit."""
+    for bit.  rasterize_mode and color_mode as in render_gaussians, for every view."""
+    mode = _lib.render_mode(rasterize_mode, color_mode, "render_gaussians_batch")
     if depth_grad and not return_depth:
         raise ValueError("render_gaussians_batch: depth_grad=True needs return_depth=True")
     if viewmats.dim() != 3 or tuple(viewmats.shape[1:]) not in ((3, 4), (4, 4)):
@@ -122,13 +133,16 @@ def render_gaussians_batch(means: Tensor, log_scales: Tensor, quats: Tensor, opa
     ang = angular_velocity if angular_velocity is not None else torch.zeros(B, 3, device=dev)
     return _render(means, log_scales, quats, opacity_logit, sh_dc, sh_rest, viewmats, cam_pos, lin, ang, (fx, fy, cx, cy),
                    H, W, bw, background, rolling_shutter_time, exposure_time, blur_samples, sh_degree_to_use, clip_thresh,
-                   return_depth, depth_grad, None, rows=(B, n))
+                   return_depth, depth_grad, None, rows=(B, n), mode=mode)
 
 
 def _render(means, log_scales, quats, opacity_logit, sh_dc, sh_rest, viewmats, cam_pos, lin, ang, intrinsics, H, W, bw,
-            background, rs, ex, S, deg, clip, return_depth, depth_grad, grad_sink, rows):
+            background, rs, ex, S, deg, clip, return_depth, depth_grad, grad_sink, rows, mode):
     """Both entry points after their argument checks: viewmats (B,3,4) or (B,4,4), cam_pos / lin / ang (B,3).  rows: the
-    shape of info's per-Gaussian entries, (N,) for render_gaussians and (B,N) for a batch."""
+    shape of info's per-Gaussian entries, (N,) for render_gaussians and (B,N) for a batch.  mode: the render mode word
+    (gsplat._lib.render_mode)."""
+    if mode & _lib.COLOR_SIGMOID:
+        deg = 0  # sigmoid(sh_dc) reads no SH basis
     S = int(S)
     if not (0 < S <= 10):
         raise RuntimeError("unsupported blur size")
@@ -136,7 +150,8 @@ def _render(means, log_scales, quats, opacity_logit, sh_dc, sh_rest, viewmats, c
     depth = 2 if depth_grad else (1 if return_depth else 0)
     rgb, alpha, D = _FusedRender.apply(means, log_scales, quats, opacity_logit, sh_dc, sh_rest, viewmats, cam_pos, lin, ang,
                                        background, intrinsics,
-                                       (int(H), int(W), int(bw), float(rs), float(ex), S, int(deg), float(clip)), info,
+                                       (int(H), int(W), int(bw), float(rs), float(ex), S, int(deg), float(clip), int(mode)),
+                                       info,
                                        rows, grad_sink, depth)
     if return_depth:  # each view filled with its own maximum where its alpha is 0 (splatfacto.py:895-897)
         d, a = D[..., None], (alpha if depth_grad else alpha.detach())[..., None]
@@ -164,7 +179,7 @@ class _FusedRender(Function):
     @staticmethod
     def forward(ctx, means, log_scales, quats, opacity_logit, sh_dc, sh_rest, viewmats, cam_pos, lin, ang, background,
                 intrinsics, cfg, info, rows, grad_sink, depth):
-        H, W, bw, rs, ex, S, deg, clip = cfg
+        H, W, bw, rs, ex, S, deg, clip, mode = cfg
         dev = means.device
         lib = _lib.load()
         B, n = viewmats.shape[0], means.shape[0]
@@ -183,10 +198,13 @@ class _FusedRender(Function):
             depths = torch.empty((B * n,), dtype=torch.float32, device=dev)
             radii = torch.empty((B * n,), dtype=torch.int32, device=dev)
             nth = torch.empty((B * n,), dtype=torch.int32, device=dev)
-            check(lib.b200_fused_preprocess_forward_views(
-                B, n, ptr(means), ptr(log_scales), ptr(quats), ptr(opacity_logit), ptr(sh_dc), ptr(sh_rest), K, deg,
-                ptr(vm), ptr(cam_pos), ptr(lin_d), ptr(ang_d), ptr(intr), rs, ex, H, W, bw, clip, ptr(packed),
-                ptr(depths), ptr(radii), ptr(nth), stream()))
+            args = (B, n, ptr(means), ptr(log_scales), ptr(quats), ptr(opacity_logit), ptr(sh_dc), ptr(sh_rest), K, deg,
+                    ptr(vm), ptr(cam_pos), ptr(lin_d), ptr(ang_d), ptr(intr), rs, ex, H, W, bw, clip, ptr(packed),
+                    ptr(depths), ptr(radii), ptr(nth), stream())
+            if mode:
+                check(lib.b200_fused_preprocess_forward_views_mode(mode, *args))
+            else:
+                check(lib.b200_fused_preprocess_forward_views(*args))
             view_isect, ids, bins = _C.bin_cull_views(B, packed, depths, radii, nth, H, W, bw, S, rs, ex)
             rgb, Ts, fi, alpha = _C.blend_forward_views(B, H, W, bw, S, ids, bins, packed, rs, ex, bg, view_isect)
             D = d_ids = d_bins = d_T = d_idx = None
@@ -214,7 +232,7 @@ class _FusedRender(Function):
     def backward(ctx, v_rgb, v_alpha, v_D):
         (means, log_scales, quats, opacity_logit, sh_dc, sh_rest, viewmats, vm, cam_pos, lin_d, ang_d, intr, bg, packed,
          radii, ids, bins, Ts, fi, d_ids, d_bins, d_T, d_idx) = ctx.saved_tensors
-        H, W, bw, rs, ex, S, deg, clip = ctx.cfg
+        H, W, bw, rs, ex, S, deg, clip, mode = ctx.cfg
         dev = means.device
         B, n, K = ctx.B, means.shape[0], ctx.K
         f32 = dict(dtype=torch.float32, device=dev)
@@ -245,7 +263,7 @@ class _FusedRender(Function):
                 dev, B, n, ptr(means), ptr(log_scales), ptr(quats), ptr(opacity_logit), ptr(sh_dc), ptr(sh_rest), K, deg,
                 ptr(vm), ptr(cam_pos), ptr(lin_d), ptr(ang_d), ptr(intr), rs, ex, H, W, bw, clip, ptr(packed), ptr(radii),
                 ptr(v_xy), ptr(v_pix), ptr(v_conic), ptr(v_col), ptr(v_op), *[ptr(out[name]) for name in _RAW], ptr(g_lin),
-                ptr(g_ang), ptr(g_vm), v_depth=ptr(v_depth))
+                ptr(g_ang), ptr(g_vm), v_depth=ptr(v_depth), mode=mode)
             v_viewmat = None
             if want_vm:
                 v_viewmat = torch.zeros_like(viewmats)

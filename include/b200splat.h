@@ -48,6 +48,12 @@ extern "C" {
                               (backward.cu:454-532 ignores the fov clamp; project_gaussians.py:272-307
                               approximates dL/dR) */
 
+/* render-mode word of the fused *_mode entry points (Splatfacto's two render switches, splatfacto.py:842-858); 0 = the
+ * entry points without _mode */
+#define B200_OPACITY_CLASSIC 1u /* rasterize_mode "classic": opacity = sigmoid(logit), no compensation factor */
+#define B200_COLOR_SIGMOID 2u   /* sh_degree 0: colour = sigmoid(sh_dc), no SH basis and no clamp; sh_rest unread */
+#define B200_MODE_BITS (B200_OPACITY_CLASSIC | B200_COLOR_SIGMOID)
+
 B200_API int b200_abi_version(void);
 B200_API const char *b200_last_error(void);
 /* Number of kernels this library has launched in this process (hand-written kernels 1 each, a cub
@@ -481,6 +487,70 @@ B200_API int b200_fused_preprocess_backward_views_depth_deterministic(
     float rolling_shutter_time, float exposure_time, unsigned img_height, unsigned img_width, unsigned block_width,
     float clip_thresh, const void *packed, const int32_t *radii, const float *v_xy, const float *v_pix_vel,
     const float *v_conic, const float *v_colors, const float *v_opacity, const float *v_depth, float *g_means,
+    float *g_log_scales, float *g_quats, float *g_opacity_logit, float *g_sh_dc, float *g_sh_rest, float *g_lin_vel,
+    float *g_ang_vel, float *g_viewmat, void *ws, size_t ws_bytes, void *stream);
+
+/* ---- render modes: Splatfacto's "classic" opacities and degree-0 sigmoid colours ------------------------------------
+ * Each *_mode entry point is the entry point named without _mode, with a leading mode word of B200_* flags:
+ *   B200_OPACITY_CLASSIC  the record's opacity is sigmoid(opacity_logit) (rasterize_mode "classic", splatfacto.py:155,
+ *                         :853-856); the backward drops the compensation VJP.
+ *   B200_COLOR_SIGMOID    the record's colour is sigmoid(sh_dc) (sh_degree 0, splatfacto.py:847-848): no view direction,
+ *                         no clamp; degrees_to_use is ignored, sh_bases may be any K >= 1, sh_rest and cam_pos are not
+ *                         read, and the backward writes g_sh_rest ((N, K-1, 3)) as zeros.
+ * mode 0 runs exactly the kernels of the entry point without _mode; a bit outside B200_MODE_BITS is B200_ERR_INVALID,
+ * checked before any GPU work.  The geometry-only forward reads only the opacity bit and the colour fill only the colour
+ * bit, so a trainer passes one word to all of them.  b200_fused_preprocess_backward_views_mode(_deterministic) take
+ * v_depth after v_opacity like the _depth entry points, but nullable: null is the backward without depth. */
+B200_API int b200_fused_preprocess_forward_views_mode(
+    unsigned mode, int num_views, int num_points, const float *means, const float *log_scales, const float *quats,
+    const float *opacity_logit, const float *sh_dc, const float *sh_rest, int sh_bases, int degrees_to_use,
+    const float *viewmats, const float *cam_pos, const float *lin_vel, const float *ang_vel, const float *intrinsics,
+    float rolling_shutter_time, float exposure_time, unsigned img_height, unsigned img_width, unsigned block_width,
+    float clip_thresh, void *packed, float *depths, int32_t *radii, int32_t *num_tiles_hit, void *stream);
+B200_API int b200_fused_preprocess_backward_views_mode(
+    unsigned mode, int num_views, int num_points, const float *means, const float *log_scales, const float *quats,
+    const float *opacity_logit, const float *sh_dc, const float *sh_rest, int sh_bases, int degrees_to_use,
+    const float *viewmats, const float *cam_pos, const float *lin_vel, const float *ang_vel, const float *intrinsics,
+    float rolling_shutter_time, float exposure_time, unsigned img_height, unsigned img_width, unsigned block_width,
+    float clip_thresh, const void *packed, const int32_t *radii, const float *v_xy, const float *v_pix_vel,
+    const float *v_conic, const float *v_colors, const float *v_opacity, const float *v_depth, float *g_means,
+    float *g_log_scales, float *g_quats, float *g_opacity_logit, float *g_sh_dc, float *g_sh_rest, float *g_lin_vel,
+    float *g_ang_vel, float *g_viewmat, void *stream);
+B200_API int b200_fused_preprocess_backward_views_mode_deterministic(
+    unsigned mode, int num_views, int num_points, const float *means, const float *log_scales, const float *quats,
+    const float *opacity_logit, const float *sh_dc, const float *sh_rest, int sh_bases, int degrees_to_use,
+    const float *viewmats, const float *cam_pos, const float *lin_vel, const float *ang_vel, const float *intrinsics,
+    float rolling_shutter_time, float exposure_time, unsigned img_height, unsigned img_width, unsigned block_width,
+    float clip_thresh, const void *packed, const int32_t *radii, const float *v_xy, const float *v_pix_vel,
+    const float *v_conic, const float *v_colors, const float *v_opacity, const float *v_depth, float *g_means,
+    float *g_log_scales, float *g_quats, float *g_opacity_logit, float *g_sh_dc, float *g_sh_rest, float *g_lin_vel,
+    float *g_ang_vel, float *g_viewmat, void *ws, size_t ws_bytes, void *stream);
+B200_API int b200_fused_geometry_forward_mode(unsigned mode, int num_points, const float *means, const float *log_scales,
+                                              const float *quats, const float *opacity_logit, const float *viewmat,
+                                              const float *lin_vel, const float *ang_vel, float rolling_shutter_time,
+                                              float exposure_time, float fx, float fy, float cx, float cy,
+                                              unsigned img_height, unsigned img_width, unsigned block_width,
+                                              float clip_thresh, void *packed, float *depths, int32_t *radii,
+                                              int32_t *num_tiles_hit, void *stream);
+B200_API int b200_fused_colors_forward_mode(unsigned mode, int num_points, const float *means, const float *sh_dc,
+                                            const float *sh_rest, int sh_bases, int degrees_to_use, const float *cam_pos,
+                                            const int32_t *radii, void *packed, void *stream);
+B200_API int b200_fused_preprocess_backward_mode(
+    unsigned mode, int num_points, const float *means, const float *log_scales, const float *quats,
+    const float *opacity_logit, const float *sh_dc, const float *sh_rest, int sh_bases, int degrees_to_use,
+    const float *viewmat, const float *cam_pos, const float *lin_vel, const float *ang_vel, float rolling_shutter_time,
+    float exposure_time, float fx, float fy, float cx, float cy, unsigned img_height, unsigned img_width,
+    unsigned block_width, float clip_thresh, const void *packed, const int32_t *radii, const float *v_xy,
+    const float *v_pix_vel, const float *v_conic, const float *v_colors, const float *v_opacity, float *g_means,
+    float *g_log_scales, float *g_quats, float *g_opacity_logit, float *g_sh_dc, float *g_sh_rest, float *g_lin_vel,
+    float *g_ang_vel, float *g_viewmat, void *stream);
+B200_API int b200_fused_preprocess_backward_mode_deterministic(
+    unsigned mode, int num_points, const float *means, const float *log_scales, const float *quats,
+    const float *opacity_logit, const float *sh_dc, const float *sh_rest, int sh_bases, int degrees_to_use,
+    const float *viewmat, const float *cam_pos, const float *lin_vel, const float *ang_vel, float rolling_shutter_time,
+    float exposure_time, float fx, float fy, float cx, float cy, unsigned img_height, unsigned img_width,
+    unsigned block_width, float clip_thresh, const void *packed, const int32_t *radii, const float *v_xy,
+    const float *v_pix_vel, const float *v_conic, const float *v_colors, const float *v_opacity, float *g_means,
     float *g_log_scales, float *g_quats, float *g_opacity_logit, float *g_sh_dc, float *g_sh_rest, float *g_lin_vel,
     float *g_ang_vel, float *g_viewmat, void *ws, size_t ws_bytes, void *stream);
 
