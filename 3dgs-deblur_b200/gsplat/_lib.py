@@ -76,6 +76,7 @@ SIGNATURES = {
     "b200_l1_loss": (_i, [C.c_longlong, _p, _p, _p, _p, _p, _i, _p]),
     "b200_l1_loss_gamma": (_i, [C.c_longlong, _p, _p, _f, _p, _p, _p, _i, _p]),
     "b200_l1_loss_u8": (_i, [C.c_longlong, _i, _p, _p, _p, _f, _f, _p, _p, _p, _p, _p, _i, _p]),
+    "b200_l1_loss_u8_area": (_i, [_i, _i, _i, _i, _p, _p, _p, _f, _f, _p, _p, _p, _p, _p, _i, _p]),
     "b200_blend_backward_deterministic_ws_bytes": (_sz, [_i, _i, _u]),
     "b200_blend_backward_packed_deterministic": (_i, [_i, _i, _u, _u, _u, _u, _p, _p, _p, _f, _f, _p, _p, _p, _p, _p, _p,
                                                       _p, _p, _sz, _p, _p, _p, _p, _p, _p, _p]),

@@ -399,7 +399,8 @@ def shading_phase(model: FlatGaussians, geo: Dict, scene: Dict, target: torch.Te
                                      rolling_shutter_time=scene["rolling_shutter_time"], exposure_time=scene["exposure_time"],
                                      blur_samples=geo["blur"], background=scene["background"], return_alpha=True,
                                      prepared=geo["prep"])
-    loss = loss_fn(rgb, target)
+    ds = scene.get("target_downscale", 1)  # > 1: the full-resolution uint8 image, pooled by the loss (PipelinedTrainer)
+    loss = loss_fn(rgb, target) if ds == 1 else loss_fn(rgb, target, downscale=ds)
     loss.backward()
     return loss.detach()
 
@@ -480,12 +481,14 @@ def fused_shading_phase(model: FlatGaussians, geo: Dict, scene: Dict, target: to
             check(lib.b200_fused_colors_forward(*args))
         rgb, Ts, fi = _C.blend_forward_packed(H, W, bw, S, geo["ids"], geo["bins"], packed, rs, ex, bg, status=geo["status"])
     from gsplat.losses import l1_loss, l1_loss_and_grad
+    ds = scene.get("target_downscale", 1)  # (as in shading_phase)
+    kw = {} if ds == 1 else dict(downscale=ds)
     if loss_fn is l1_loss:  # the default: value and cotangent from the one kernel
-        loss, v_rgb = l1_loss_and_grad(rgb, target)
+        loss, v_rgb = l1_loss_and_grad(rgb, target, **kw)
     else:
         rgb.requires_grad_(True)
         with torch.enable_grad():
-            loss = loss_fn(rgb, target)
+            loss = loss_fn(rgb, target, **kw)
         (v_rgb,) = torch.autograd.grad(loss, rgb)
     with torch.no_grad(), _lib.on_device(dev):
         v_xy, v_abs, v_pix, v_conic, v_col, v_op = _C.blend_backward_packed(
@@ -548,18 +551,35 @@ class PipelinedTrainer:
     API:  prepare(cam, cam_index)            -- A for the first image (and after anything that invalidates it)
           train_step(target, next_cam=None, next_index=0) -> device loss
     `cam` = dict(viewmat (3,4), lin_vel (3), ang_vel (3), cam_pos (3)) tensors on any device, or `cam_floats`
-    (21 floats in that order, e.g. a pinned host row from gsplat.data.ImagePrefetcher)."""
+    (21 floats in that order, e.g. a pinned host row from gsplat.data.ImagePrefetcher).
+
+    Resolution schedule (`num_downscales` > 0, Splatfacto's splatfacto.py:660-667): image k (k = the step that trains on
+    it) renders at 1/d_k of the scene's size, d_k = 2 ** max(num_downscales - k // resolution_schedule, 0), with fx, fy,
+    cx, cy scaled by 1/d_k (Cameras.rescale_output_resolution, floor rounding); the loss still gets the full-resolution
+    target (see `_as_target`).  `render_size` = (H, W) of the image whose backward just ran, valid in `after_backward`."""
 
     def __init__(self, model: FlatGaussians, scene: Dict, lr: float = 1e-3, group=None, loss_fn=None, use_graphs: bool = True,
                  capacity: Optional[int] = None, sh_degree_to_use: int = 3, geometry_fn=None, shading_fn=None,
                  optimizer: str = "b200", sh_chunks: int = 1, operators: Optional[str] = None,
-                 rasterize_mode: str = "antialiased", color_mode: str = "sh"):
+                 rasterize_mode: str = "antialiased", color_mode: str = "sh", num_downscales: int = 0,
+                 resolution_schedule: int = 3000):
         """operators: "dropin" = the two phases on the reference-compatible operators under autograd (`geometry_phase` /
         `shading_phase`); "fused" = on the fused raw-parameter kernels (`fused_geometry_phase` / `fused_shading_phase`:
         same numbers, ~45 fewer launches per step); None = fused where it applies (CUDA, sh_layout "split"), else drop-in.
         rasterize_mode ("antialiased" / "classic") and color_mode ("sh" / "sigmoid"): Splatfacto's two render switches, as
-        in gsplat.fused.render_gaussians; both operator sets serve them (injected phases are called as they are)."""
+        in gsplat.fused.render_gaussians; both operator sets serve them (injected phases are called as they are).
+        num_downscales / resolution_schedule: Splatfacto's resolution schedule (class docstring); 0 trains at full size."""
         self.model, self.scene = model, dict(scene)
+        if int(num_downscales) != num_downscales or not 0 <= num_downscales <= 4:
+            raise ValueError("num_downscales must be an integer from 0 to 4 (factors up to 16)")
+        if int(resolution_schedule) != resolution_schedule or resolution_schedule < 1:
+            raise ValueError("resolution_schedule must be a positive integer")
+        self.num_downscales, self.resolution_schedule = int(num_downscales), int(resolution_schedule)
+        # full-resolution size and intrinsics: the scene holds the current image's scaled values, so scaling never compounds
+        # (intrinsics may also arrive with the first camera dict)
+        self._full = {k: self.scene[k] for k in ("H", "W", "fx", "fy", "cx", "cy") if k in self.scene} if self.num_downscales else None
+        self._d = 1                     # downscale factor of the image the scene is currently set up for
+        self.render_size = None         # (H, W) of the image whose backward just ran
         if loss_fn is None:
             from gsplat.losses import l1_loss as loss_fn
         self.loss_fn = loss_fn
@@ -652,9 +672,21 @@ class PipelinedTrainer:
                              cam["ang_vel"].reshape(-1)[:3].to(d0), cam["cam_pos"].reshape(-1)[:3].to(d0)]).float()
             for k in ("fx", "fy", "cx", "cy"):  # intrinsics are launch constants (part of the graph key)
                 if k in cam:
-                    self.scene[k] = float(cam[k])
+                    (self._full if self._full is not None else self.scene)[k] = float(cam[k])
         self.st["cam"].copy_(row, non_blocking=True)
         self.st["cam_index"].fill_(int(cam_index))
+
+    def downscale_factor(self, image: int) -> int:
+        """Splatfacto's _get_downscale_factor (splatfacto.py:660-667) for the image trained at step `image`."""
+        return 2 ** max(self.num_downscales - int(image) // self.resolution_schedule, 0)
+
+    def _set_resolution(self, image):
+        d = self._d = self.downscale_factor(image)
+        f, s = self._full, self.scene
+        s["H"], s["W"] = f["H"] // d, f["W"] // d  # floor, exact for powers of two
+        for k in ("fx", "fy", "cx", "cy"):
+            if k in f:
+                s[k] = f[k] * (1.0 / d)
 
     def _size_capacity(self):
         """First use: one synchronous probe of the entry count with a generous capacity; later growth comes from the
@@ -690,8 +722,18 @@ class PipelinedTrainer:
         key = self._key() + (target_shape_dtype,)
         e = self._graphs.get(key)
         if e is None:
-            e = self._graphs[key] = dict(gA=None, gB=None, geo=None, target=None, warm=0)
+            e = self._graphs[key] = dict(gA=None, gB=None, geo=None, target=None, warm=0, d=self._d)
         return e
+
+    def _drop_coarser_graphs(self):
+        """The schedule only ever lowers d: entries of a coarser stage never replay again.  Called at the start of a step,
+        when the last of them (phase B of the previous image) is already queued: the stream is drained first (once per
+        stage change) so that no graph or graph-pool memory is released while a replay still uses it."""
+        stale = [k for k, e in self._graphs.items() if e["d"] > self._d]
+        if stale and self.cuda:
+            torch.cuda.current_stream().synchronize()
+        for key in stale:
+            del self._graphs[key]
 
     def _lib_launches(self):
         from gsplat import _lib
@@ -744,10 +786,24 @@ class PipelinedTrainer:
     def _as_target(self, target):
         """The dataset's uint8 image goes to the loss as it is when the loss converts it in its own kernel
         (gsplat.losses.l1_loss / photometric_loss); any other loss gets the float image the reference builds
-        (get_gt_img, splatfacto.py:906-907)."""
-        if target.dtype != torch.uint8 or getattr(self.loss_fn, "accepts_uint8", False):
+        (get_gt_img, splatfacto.py:906-907).  With a resolution schedule the image stays at full resolution: a loss that
+        declares `accepts_downscale` pools the uint8 image in its kernel (scene["target_downscale"] tells the shading
+        phase to pass `downscale=d`); any other loss, or a float image, gets get_gt_img's float target, / 255 then the area
+        mean over d x d blocks (resize_image, splatfacto.py:83-95)."""
+        if self._full is None:
+            if target.dtype != torch.uint8 or getattr(self.loss_fn, "accepts_uint8", False):
+                return target
+            return target.float() / 255
+        d = self._d
+        if d > 1 and target.dtype == torch.uint8 and getattr(self.loss_fn, "accepts_downscale", False):
+            self.scene["target_downscale"] = d
             return target
-        return target.float() / 255
+        self.scene["target_downscale"] = 1
+        if target.dtype == torch.uint8 and not (d == 1 and getattr(self.loss_fn, "accepts_uint8", False)):
+            target = target.float() / 255
+        if d == 1:
+            return target
+        return torch.nn.functional.avg_pool2d(target.permute(2, 0, 1)[None], d)[0].permute(1, 2, 0).contiguous()
 
     # ---- public API ----------------------------------------------------------------------------------------------
     class _OnMain:
@@ -776,10 +832,12 @@ class PipelinedTrainer:
         """Stage the camera of the image the next train_step trains on (phase A itself is queued by train_step: at once
         for the first image, behind the previous step's geometry update afterwards)."""
         with self._OnMain(self):
-            self._prepare(cam, cam_index)
+            self._prepare(cam, cam_index, self.steps)
 
-    def _prepare(self, cam, cam_index):
+    def _prepare(self, cam, cam_index, image):
         self._set_camera(cam, cam_index)
+        if self._full is not None:  # the scene takes this image's resolution: A(image) and B(image) read it
+            self._set_resolution(image)
         self._size_capacity()
         self._prepared = True
         self._A_done = False
@@ -800,11 +858,14 @@ class PipelinedTrainer:
 
     def _train_step(self, target, next_cam, next_index):
         m = self.model
+        if self._full is not None:
+            self._drop_coarser_graphs()
         e = self._entry((tuple(target.shape), target.dtype))
         self._ensure_A(e)
         if self.cuda and self._pending_sh is not None:
             torch.cuda.current_stream().wait_event(self.ev_sh_done)   # SH parameters of the previous step are final
             self._pending_sh = None
+        self.render_size = (self.scene["H"], self.scene["W"])
         self._run_B(e, target)
         if self.after_backward is not None:
             # e.g. gsplat.densify.Densifier.accumulate: this image's radii and |d loss / d xy| (the `xys.absgrad` side channel)
@@ -831,7 +892,7 @@ class PipelinedTrainer:
         # the next image's camera row is staged while the geometry gradients are on the wire (B, its last reader, is queued)
         self._prepared = False
         if next_cam is not None:
-            self._prepare(next_cam, next_index)
+            self._prepare(next_cam, next_index, self.steps + 1)
         if works is not None:
             works[0].wait()
         self._update(0, lo, scale, veto_host, 0)

@@ -21,10 +21,20 @@ def _workspace(dev):
     return ws
 
 
-def _target_options(name, pred, target, background, min_rgb_level, mask):
-    """Checks of the uint8-target form shared by l1_loss / photometric_loss -> (channels, background, min level, mask)."""
-    if pred.dim() != 3 or pred.shape[-1] != 3 or target.dim() != 3 or target.shape[:2] != pred.shape[:2] or target.shape[2] not in (3, 4):
-        raise ValueError(f"{name}: a uint8 target must be (H, W, 3) or (H, W, 4) for an (H, W, 3) render, got "
+def _downscale_factor(name, downscale):
+    d = int(downscale)
+    if d != downscale or d not in (1, 2, 4, 8, 16):
+        raise ValueError(f"{name}: downscale must be 1, 2, 4, 8 or 16, got {downscale!r}")
+    return d
+
+
+def _target_options(name, pred, target, background, min_rgb_level, mask, d=1):
+    """Checks of the uint8-target form shared by l1_loss / photometric_loss -> (channels, background, min level, mask).
+    d > 1: the target (and mask) are at full resolution, the render at (H // d, W // d)."""
+    if (pred.dim() != 3 or pred.shape[-1] != 3 or target.dim() != 3 or target.shape[2] not in (3, 4)
+            or (target.shape[0] // d, target.shape[1] // d) != tuple(pred.shape[:2])):
+        want = "an (H, W, 3) render" if d == 1 else f"an (H // {d}, W // {d}, 3) render"
+        raise ValueError(f"{name}: a uint8 target must be (H, W, 3) or (H, W, 4) for {want}, got "
                          f"{tuple(target.shape)} / {tuple(pred.shape)}")
     ch = int(target.shape[2])
     if ch == 4:
@@ -36,9 +46,10 @@ def _target_options(name, pred, target, background, min_rgb_level, mask):
     else:
         background = None  # (an RGB image is used as it is, splatfacto.py:919-923)
     if mask is not None:
-        if tuple(mask.shape[:2]) != tuple(pred.shape[:2]) or mask.numel() != pred.shape[0] * pred.shape[1]:
-            raise ValueError(f"{name}: mask must be (H, W) or (H, W, 1)")
-        mask = mask.detach().to(device=pred.device, dtype=torch.float32).reshape(pred.shape[0], pred.shape[1]).contiguous()
+        H, W = int(target.shape[0]), int(target.shape[1])
+        if tuple(mask.shape[:2]) != (H, W) or mask.numel() != H * W:
+            raise ValueError(f"{name}: mask must be (H, W) or (H, W, 1), the target's size")
+        mask = mask.detach().to(device=pred.device, dtype=torch.float32).reshape(H, W).contiguous()
     level = float(min_rgb_level)
     if level < 0:
         raise ValueError(f"{name}: min_rgb_level must be >= 0")
@@ -47,8 +58,9 @@ def _target_options(name, pred, target, background, min_rgb_level, mask):
 
 class _L1Loss(Function):
     @staticmethod
-    def forward(ctx, pred, target, gamma=None, background=None, min_rgb_level=0.0, mask=None, want_target=False):
+    def forward(ctx, pred, target, gamma=None, background=None, min_rgb_level=0.0, mask=None, want_target=False, downscale=1):
         _lib.require_cuda(pred, target)
+        d = _downscale_factor("l1_loss", downscale)
         if pred.dtype != torch.float32:
             raise RuntimeError("l1_loss: expected a float32 render")
         if pred.numel() < 1:
@@ -60,19 +72,24 @@ class _L1Loss(Function):
         ctx.prepared_target = None
         if target.dtype == torch.uint8:
             # the dataset's image as it is stored: conversion, compositing, minimum level and mask ride in the loss kernel
-            ch, bg, level, mk = _target_options("l1_loss", pred, target, background, min_rgb_level, mask)
+            ch, bg, level, mk = _target_options("l1_loss", pred, target, background, min_rgb_level, mask, d)
             with _lib.on_device(dev):
                 loss = torch.empty((), dtype=torch.float32, device=dev)
                 grad = torch.empty_like(pred_c) if ctx.needs_input_grad[0] else None
                 tout = torch.empty_like(pred_c) if want_target else None
-                check(_lib.load().b200_l1_loss_u8(pred_c.shape[0] * pred_c.shape[1], ch, ptr(pred_c), ptr(target_c), ptr(bg), level,
-                                                  float(gamma) if gamma is not None else 0.0, ptr(mk), ptr(loss), ptr(grad), ptr(tout),
-                                                  ptr(_workspace(dev)), 1, stream()))
+                gm = float(gamma) if gamma is not None else 0.0
+                if d == 1:
+                    check(_lib.load().b200_l1_loss_u8(pred_c.shape[0] * pred_c.shape[1], ch, ptr(pred_c), ptr(target_c), ptr(bg), level,
+                                                      gm, ptr(mk), ptr(loss), ptr(grad), ptr(tout), ptr(_workspace(dev)), 1, stream()))
+                else:  # Splatfacto's area downscale of the full-resolution image rides in the same pass
+                    check(_lib.load().b200_l1_loss_u8_area(target_c.shape[0], target_c.shape[1], ch, d, ptr(pred_c), ptr(target_c),
+                                                           ptr(bg), level, gm, ptr(mk), ptr(loss), ptr(grad), ptr(tout),
+                                                           ptr(_workspace(dev)), 1, stream()))
             ctx.prepared_target = tout
         else:
-            if background is not None or mask is not None or float(min_rgb_level) > 0:
-                raise ValueError("l1_loss: background / min_rgb_level / mask apply to a uint8 target (the dataset's image); a float "
-                                 "target is taken as already prepared")
+            if background is not None or mask is not None or float(min_rgb_level) > 0 or d != 1:
+                raise ValueError("l1_loss: background / min_rgb_level / mask / downscale apply to a uint8 target (the dataset's "
+                                 "image); a float target is taken as already prepared")
             if pred.shape != target.shape:
                 raise ValueError(f"l1_loss: shapes differ: {tuple(pred.shape)} vs {tuple(target.shape)}")
             if target.dtype != torch.float32:
@@ -96,11 +113,11 @@ class _L1Loss(Function):
             raise RuntimeError("l1_loss: the target image is a constant (no gradient)")
         g = ctx.grad
         ctx.grad = None
-        return (g * v_loss if g is not None else None), None, None, None, None, None, None
+        return (g * v_loss if g is not None else None), None, None, None, None, None, None, None
 
 
 def l1_loss(pred: torch.Tensor, target: torch.Tensor, gamma: float = None, *, background: torch.Tensor = None,
-            min_rgb_level: float = 0.0, mask: torch.Tensor = None) -> torch.Tensor:
+            min_rgb_level: float = 0.0, mask: torch.Tensor = None, downscale: int = 1) -> torch.Tensor:
     """mean |pred - target| as a 0-d tensor; differentiable w.r.t. `pred` only.
 
     gamma (extension): `pred` is the LINEAR render and the loss is taken on the caller's gamma-corrected image,
@@ -110,28 +127,33 @@ def l1_loss(pred: torch.Tensor, target: torch.Tensor, gamma: float = None, *, ba
     target may be the dataset's uint8 image, (H, W, 3) or (H, W, 4): the caller's ground-truth preparation then runs inside
     the loss kernel -- / 255 (get_gt_img, splatfacto.py:900-910), RGBA composited over `background`
     (composite_with_background, :912-923), clamp(min=min_rgb_level / 255) (:952-953), and with `mask` ((H, W) or (H, W, 1))
-    both images are multiplied by it before the mean (:957-964)."""
-    return _L1Loss.apply(pred, target, gamma, background, min_rgb_level, mask, False)
+    both images are multiplied by it before the mean (:957-964).
+
+    downscale = d (2, 4, 8 or 16; Splatfacto's resolution schedule, splatfacto.py:660-667): `pred` is (H // d, W // d, 3)
+    and the uint8 target (and mask) stay at full resolution; the kernel takes their area mean over d x d blocks
+    (`resize_image`, :83-95) before compositing, as get_gt_img does.  A float target with downscale > 1 raises ValueError."""
+    return _L1Loss.apply(pred, target, gamma, background, min_rgb_level, mask, False, downscale)
 
 
 def l1_loss_and_grad(pred: torch.Tensor, target: torch.Tensor, gamma: float = None, *, background: torch.Tensor = None,
-                     min_rgb_level: float = 0.0, mask: torch.Tensor = None, return_target: bool = False):
+                     min_rgb_level: float = 0.0, mask: torch.Tensor = None, return_target: bool = False, downscale: int = 1):
     """(mean |pred - target|, d loss / d pred) from the one kernel, outside autograd -- for callers that chain the
     cotangent themselves (gsplat.dp.fused_shading_phase).  Same arguments and checks as `l1_loss`; with `return_target`
     (uint8 targets) the prepared float target comes back as a third value."""
     with torch.no_grad():
         ctx = _Ctx()
-        loss = _L1Loss.forward(ctx, pred, target, gamma, background, min_rgb_level, mask, return_target)
+        loss = _L1Loss.forward(ctx, pred, target, gamma, background, min_rgb_level, mask, return_target, downscale)
     if return_target:
         return loss, ctx.grad, (ctx.prepared_target if ctx.prepared_target is not None else target)
     return loss, ctx.grad
 
 
 l1_loss.accepts_uint8 = True  # gsplat.dp hands the dataset's uint8 image straight to such a loss
+l1_loss.accepts_downscale = True  # ... at full resolution with `downscale=d` while the trainer renders at 1/d
 
 
 class _Ctx:
-    needs_input_grad = (True, False, False, False, False, False, False)
+    needs_input_grad = (True, False, False, False, False, False, False, False)
 
 
 # ---- SSIM and the full photometric loss (splatfacto.py:957-975) -------------------------------------------------
@@ -177,19 +199,20 @@ class _Photometric(Function):
     returns the plain SSIM value instead."""
 
     @staticmethod
-    def forward(ctx, pred, target, lam, background=None, min_rgb_level=0.0):
+    def forward(ctx, pred, target, lam, background=None, min_rgb_level=0.0, downscale=1):
         name = "photometric_loss" if lam is not None else "ssim"
+        d = _downscale_factor(name, downscale)
         u8 = target.dtype == torch.uint8
         if u8:
             _lib.require_cuda(pred, target)
             if pred.dtype != torch.float32:
                 raise RuntimeError(f"{name}: expected a float32 render")
-            ch, bg, level, _ = _target_options(name, pred, target, background, min_rgb_level, None)
+            ch, bg, level, _ = _target_options(name, pred, target, background, min_rgb_level, None, d)
             if pred.shape[0] < 11 or pred.shape[1] < 11:
                 raise ValueError(f"{name}: SSIM needs an image of at least 11 x 11 pixels")
         else:
-            if background is not None or float(min_rgb_level) > 0:
-                raise ValueError(f"{name}: background / min_rgb_level apply to a uint8 target")
+            if background is not None or float(min_rgb_level) > 0 or d != 1:
+                raise ValueError(f"{name}: background / min_rgb_level / downscale apply to a uint8 target")
             _check_images(name, pred, target)
         pred_c, target_c = pred.contiguous(), target.contiguous()
         H, W, C = pred_c.shape
@@ -207,8 +230,13 @@ class _Photometric(Function):
                 l1 = torch.empty((), **f32)
                 g1 = torch.empty_like(pred_c) if (need and lam is not None) else None
                 prepared = torch.empty_like(pred_c)
-                check(lib.b200_l1_loss_u8(H * W, ch, ptr(pred_c), ptr(target_c), ptr(bg), level, 0.0, None, ptr(l1), ptr(g1),
-                                          ptr(prepared), ptr(_workspace(dev)), 1, stream()))
+                if d == 1:
+                    check(lib.b200_l1_loss_u8(H * W, ch, ptr(pred_c), ptr(target_c), ptr(bg), level, 0.0, None, ptr(l1), ptr(g1),
+                                              ptr(prepared), ptr(_workspace(dev)), 1, stream()))
+                else:  # the pooled, prepared target (splatfacto.py:83-95, :900-923) goes to the SSIM kernels
+                    check(lib.b200_l1_loss_u8_area(target_c.shape[0], target_c.shape[1], ch, d, ptr(pred_c), ptr(target_c), ptr(bg),
+                                                   level, 0.0, None, ptr(l1), ptr(g1), ptr(prepared), ptr(_workspace(dev)), 1,
+                                                   stream()))
                 target_c = prepared
                 if lam is None:
                     l1 = None
@@ -242,23 +270,27 @@ class _Photometric(Function):
             check(_lib.load().b200_ssim_backward(H, W, C, ptr(pred_c), ptr(target_c), ptr(ctx.maps), scale, ptr(add_in),
                                                  add_scale, ptr(v), _window_taps(), ptr(grad), stream()))
         ctx.maps = ctx.g1 = None
-        return grad, None, None, None, None
+        return grad, None, None, None, None, None
 
 
-def ssim(pred: torch.Tensor, target: torch.Tensor, *, background: torch.Tensor = None, min_rgb_level: float = 0.0) -> torch.Tensor:
+def ssim(pred: torch.Tensor, target: torch.Tensor, *, background: torch.Tensor = None, min_rgb_level: float = 0.0,
+         downscale: int = 1) -> torch.Tensor:
     """pytorch_msssim.SSIM(data_range=1, size_average=True, channel=C) of two (H, W, C) images (splatfacto.py:260,958);
-    differentiable w.r.t. `pred`.  A uint8 target is prepared as in `l1_loss`."""
-    return _Photometric.apply(pred, target, None, background, min_rgb_level)
+    differentiable w.r.t. `pred`.  A uint8 target is prepared as in `l1_loss`, `downscale` included."""
+    return _Photometric.apply(pred, target, None, background, min_rgb_level, downscale)
 
 
 def photometric_loss(pred: torch.Tensor, target: torch.Tensor, ssim_lambda: float = 0.2, *, background: torch.Tensor = None,
-                     min_rgb_level: float = 0.0) -> torch.Tensor:
+                     min_rgb_level: float = 0.0, downscale: int = 1) -> torch.Tensor:
     """Splatfacto's main loss (splatfacto.py:943-975): (1 - ssim_lambda) * mean|target - pred| + ssim_lambda *
     (1 - SSIM(target, pred)); differentiable w.r.t. `pred`.  `target` is the prepared float image or the dataset's uint8
     image, (H, W, 3) or (H, W, 4): then / 255, compositing over `background` and clamp(min=min_rgb_level / 255) run inside
     the L1 kernel, which hands the prepared target to the SSIM kernels.  (A mask multiplies BOTH images in the reference,
-    :957-964: apply it to `pred` and to a float target before the call.)"""
-    return _Photometric.apply(pred, target, float(ssim_lambda), background, min_rgb_level)
+    :957-964: apply it to `pred` and to a float target before the call.)  `downscale` as in `l1_loss`: the L1 kernel pools
+    the full-resolution uint8 image and the SSIM term is taken against that pooled target."""
+    return _Photometric.apply(pred, target, float(ssim_lambda), background, min_rgb_level, downscale)
 
 
 photometric_loss.accepts_uint8 = True
+photometric_loss.accepts_downscale = True
+ssim.accepts_downscale = True

@@ -593,6 +593,26 @@ B200_API int b200_l1_loss_gamma(long long numel, const float *pred_linear, const
 B200_API int b200_l1_loss_u8(long long n_pixels, int channels, const float *pred, const unsigned char *target_u8,
                              const float *background, float min_level, float gamma, const float *mask, float *loss,
                              float *grad, float *target_out, void *ws, int ws_is_zeroed, void *stream);
+/* b200_l1_loss_u8 for a render at 1/d of the target's resolution (Splatfacto's resolution schedule, splatfacto.py:660-667):
+ * the target's area downscale (`resize_image`, :83-95: conv2d with a d x d box of weight 1/d^2 at stride d) rides in the
+ * same pass, which reads the full-resolution image once.  target_u8 is (in_h, in_w, channels) bytes with rows of
+ * in_w * channels bytes (no alignment asked); mask is in_h * in_w floats or null; pred, grad and target_out are
+ * (in_h / d) * (in_w / d) * 3 floats (floored sizes; rows and columns past d * (in / d) are ignored, as by the strided conv2d).
+ * d = 2, 4, 8 or 16.  Per output pixel, in the reference's order: every channel (alpha included) and the mask are pooled
+ * from k / 255.0f, summed in float32 in one fixed order (rows top to bottom, pixels left to right) and scaled by 1/d^2
+ * (exact); RGBA is composited over background with the POOLED alpha; clamp(min = min_level); both images times the pooled
+ * mask; the gamma step on pred; L1 mean over 3 * (in_h / d) * (in_w / d).  grad is the cotangent w.r.t. the linear render.
+ * Error bound (first order, u = 2^-24, one rounding per operation; torch's conv2d sums in an order of its own, so equality
+ * with it bit for bit is not available; tests/downscale_f64.py restates this in float64 and evaluates it per element):
+ *   pooled channel / alpha / mask p:  e_p = (d^2 - 1) u p   (d^2 non-negative terms; the mask bound uses its |values|)
+ *   composite t = a c + (1 - a) bg:    e_t = (|c| + |bg|) e_a + |a| e_c + u (|a c| + 2 |(1 - a) bg| + |t|);  RGB: e_t = e_c
+ *   clamp: e_t unchanged;  mask:       e_tm = |m| e_t + |t| e_m + u |t m|
+ *   pred side y (gamma-corrected or not): e_y = |y| e_m + u |y m| with a mask, plus 4 u |y m| with gamma (powf, not
+ *   correctly rounded);  loss: mean(e_tm + e_y) + the reduction's rounding, at most (depth) u L for its deepest chain.
+ * Where |pred_img - target| exceeds e_tm + e_y the cotangent's sign is the reference's.  Deterministic. */
+B200_API int b200_l1_loss_u8_area(int in_h, int in_w, int channels, int d, const float *pred, const unsigned char *target_u8,
+                                  const float *background, float min_level, float gamma, const float *mask, float *loss,
+                                  float *grad, float *target_out, void *ws, int ws_is_zeroed, void *stream);
 
 /* SSIM term of the photometric loss, (1 - lambda) * L1 + lambda * (1 - SSIM) (nerfstudio/models/splatfacto.py:957-975;
  * SSIM = pytorch_msssim.SSIM(data_range=1, size_average=True, channel=C): 11-tap Gaussian window sigma 1.5, separable,
