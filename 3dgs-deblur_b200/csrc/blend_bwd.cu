@@ -38,6 +38,10 @@ struct BlendBwdParams {
     int views;     // images of the launch, laid out as in BlendFwdParams (tile v * tbx * tby + t, rows v * H + i)
 };
 
+struct BlendBwdReplayParams : BlendBwdParams {
+    const uint16_t *visit_mask;  // the recording forward's (list position, warp) masks (b200_blend_forward_record)
+};
+
 // CTA -> (image, tile within the image)
 __device__ __forceinline__ void cta_tile(const int32_t *tile_order, const BlendGeom &g, int &view, int &tile) {
     const int t = tile_order ? __ldg(tile_order + blockIdx.x) : (int)blockIdx.x;
@@ -279,10 +283,18 @@ __global__ void __launch_bounds__(BLEND_THREADS, 3) blend_backward_kernel(const 
 //     algebra when no lane passes (launch_bwd).
 // Visit epilogue: the 13 per-Gaussian sums are reduced over the warp through a shared-memory transposition.  DET as in
 // blend_backward_kernel.
+// REPLAY (b200_blend_backward_replay): the warp's visits and their samples are the recording forward's mask of (list
+// position, warp) instead of the cull and the per-sample last-contributor skip.  Per pixel-sample, the sigma, alpha and
+// idx <= final_idx tests below pass exactly where the forward blended (same ex2.approx of the same sigma, the same cut,
+// both clamps above 1/255, final_idx = the last entry blended before the stop), so the visits and samples it leaves out
+// are the ones whose every pixel is masked: their terms are exact zeros, which leave every nonzero sum unchanged and
+// every +0 sum at +0 (a skipped DET slot keeps its cleared +0; a stored -0 adds to +0 the same).  Every recorded sample
+// has a passing lane, so no per-sample vote is needed with rolling shutter either.
 constexpr int RED_STRIDE = 36;  // floats per row: 32 lanes + 4 of padding (rows stay 16-byte aligned, halves hit distinct banks)
 constexpr int BWD_MIN_CTAS = 5;  // 96 registers
-template <int S, bool VOTE, bool DET>
-__global__ void __launch_bounds__(128, BWD_MIN_CTAS) blend_backward_kernel2(const BlendBwdParams p) {
+template <int S, bool VOTE, bool DET, bool REPLAY>
+__global__ void __launch_bounds__(128, BWD_MIN_CTAS)
+    blend_backward_kernel2(const std::conditional_t<REPLAY, BlendBwdReplayParams, BlendBwdParams> p) {
     constexpr int NT = 128;
     __shared__ __align__(128) PackedGaussian s_rec[BLEND_STAGES][BLEND_BATCH];
     __shared__ __align__(8) uint64_t s_bar[BLEND_STAGES];
@@ -394,11 +406,23 @@ __global__ void __launch_bounds__(128, BWD_MIN_CTAS) blend_backward_kernel2(cons
         }
     };
 
+    // REPLAY: the recorded mask of entry c0 + lane of this batch, for the warp (0 beyond the warp's last contributor)
+    auto recorded = [&](int top, int cnt, int c0) -> unsigned {
+        const int e = c0 + lane;
+        if constexpr (REPLAY)
+            return ((e < cnt) && (top - e <= wmax)) ? (unsigned)__ldg(p.visit_mask + (size_t)(top - e) * (NT / 32) + warp) : 0u;
+        return 0u;
+    };
+
     B200_COUNT_DECL;
     if (nb > 0) issue(0);
     for (int b = 0; b < nb; ++b) {
         const int st = b & 1;
         if (b + 1 < nb) issue(b + 1);
+        unsigned next_mask = 0u;  // REPLAY: loaded one chunk ahead (the first before the batch wait)
+        if constexpr (REPLAY) {
+            if (wmax >= range.x) next_mask = recorded(hi - b * BLEND_BATCH, min(BLEND_BATCH, hi - b * BLEND_BATCH - range.x + 1), 0);
+        }
         wait_batch(s_bar, b);
         const int top = hi - b * BLEND_BATCH;
         const int cnt = min(BLEND_BATCH, top - range.x + 1);
@@ -406,8 +430,13 @@ __global__ void __launch_bounds__(128, BWD_MIN_CTAS) blend_backward_kernel2(cons
         if (wmax >= range.x) {
             for (int c0 = 0; c0 < cnt; c0 += 32) {
                 const int e = c0 + lane;
-                const unsigned my_mask =
-                    ((e < cnt) && (top - e <= wmax)) ? sample_mask_exact<S>(s_rec[st][e], win, p.g.exposure) : 0u;
+                unsigned my_mask;
+                if constexpr (REPLAY) {
+                    my_mask = next_mask;
+                    if (c0 + 32 < cnt) next_mask = recorded(top, cnt, c0 + 32);
+                } else {
+                    my_mask = ((e < cnt) && (top - e <= wmax)) ? sample_mask_exact<S>(s_rec[st][e], win, p.g.exposure) : 0u;
+                }
                 unsigned m = __ballot_sync(0xffffffffu, my_mask != 0u);
                 if ((e < cnt) && (top - e <= wmax)) B200_COUNT(0, 1);
                 while (m) {
@@ -433,7 +462,7 @@ __global__ void __launch_bounds__(128, BWD_MIN_CTAS) blend_backward_kernel2(cons
                     bool any = false;
 #pragma unroll
                     for (int s = 0; s < S; ++s) {
-                        if (!(smask & (1u << s)) || idx > smax[s]) continue;  // warp-uniform
+                        if (!(smask & (1u << s)) || (!REPLAY && idx > smax[s])) continue;  // warp-uniform
                         const f2 tau = f2_add(f2_splat(blur[s]), ROLL);
                         const f2 dx = f2_fma(tau, VX, dx0), dy = f2_fma(tau, VY, dy0);
                         const f2 u0 = f2_fma(HA, dx, f2_mul(CB, dy));
@@ -532,16 +561,18 @@ static bool paired_bwd(unsigned block_width) { return block_width == 16 && !blen
 static int bwd_warps(unsigned block_width) { return paired_bwd(block_width) ? BLEND_THREADS / 2 / 32 : BLEND_THREADS / 32; }
 
 template <int S, bool DET>
-static int launch_bwd(const BlendBwdParams &p, cudaStream_t st) {
+static int launch_bwd(const BlendBwdReplayParams &p, cudaStream_t st) {
     const int ctas = p.views * p.g.tbx * p.g.tby;
-    if (paired_bwd(p.g.bw)) {
+    if (p.visit_mask) {
+        blend_backward_kernel2<S, false, DET, true><<<ctas, BLEND_THREADS / 2, 0, st>>>(p);
+    } else if (paired_bwd(p.g.bw)) {
         // per-sample votes ("does any lane hold a contributing pixel", then skip the gradient algebra): without rolling
         // shutter the exact cull leaves 4 % of the entered sample blocks empty and the vote + branch costs more than the
         // masked arithmetic; with it the warp's time window widens the cull and the skip pays
         if (p.g.rs_time != 0.f)
-            blend_backward_kernel2<S, true, DET><<<ctas, BLEND_THREADS / 2, 0, st>>>(p);
+            blend_backward_kernel2<S, true, DET, false><<<ctas, BLEND_THREADS / 2, 0, st>>>(p);
         else
-            blend_backward_kernel2<S, false, DET><<<ctas, BLEND_THREADS / 2, 0, st>>>(p);
+            blend_backward_kernel2<S, false, DET, false><<<ctas, BLEND_THREADS / 2, 0, st>>>(p);
     } else {
         blend_backward_kernel<S, DET><<<ctas, BLEND_THREADS, 0, st>>>(p);
     }
@@ -809,7 +840,7 @@ static int run_blend_backward(int num_points, unsigned img_height, unsigned img_
                               const float *v_output, const float *v_output_alpha, float *v_xy, float *v_xy_abs,
                               float *v_pix_vels, float *v_conic, float *v_colors, float *v_opacity, bool outputs_are_zero,
                               cudaStream_t st, const int32_t *tile_order = nullptr, float *slots = nullptr,
-                              int views = 1) {
+                              int views = 1, const uint16_t *visit_mask = nullptr) {
     B200_REQUIRE(n_blur_samples > 0 && n_blur_samples <= B200_MAX_BLUR_SAMPLES, "unsupported blur size");
     B200_REQUIRE(num_points >= 1, "num_points must be >= 1");
     B200_REQUIRE(block_width > 1 && block_width <= 16, "block_width must be between 2 and 16");
@@ -826,7 +857,7 @@ static int run_blend_backward(int num_points, unsigned img_height, unsigned img_
         B200_CUDA(cudaMemsetAsync(v_colors, 0, n * 3 * sizeof(float), st));
         B200_CUDA(cudaMemsetAsync(v_opacity, 0, n * sizeof(float), st));
     }
-    BlendBwdParams p;
+    BlendBwdReplayParams p;
     p.g = blend_geom(img_height, img_width, block_width, rolling_shutter_time, exposure_time);
     p.ids_sorted = gaussian_ids_sorted;
     p.tile_bins = reinterpret_cast<const int2 *>(tile_bins);
@@ -838,6 +869,7 @@ static int run_blend_backward(int num_points, unsigned img_height, unsigned img_
     p.v_opac = v_opacity;
     p.slots = slots;
     p.views = views;
+    p.visit_mask = visit_mask;
     return with_blur_samples(n_blur_samples, [&](auto s) {
         return slots ? launch_bwd<decltype(s)::value, true>(p, st) : launch_bwd<decltype(s)::value, false>(p, st);
     });
@@ -887,7 +919,7 @@ static int run_blend_backward_deterministic(int views, int num_points, int num_e
                                             const float *v_output, const float *v_output_alpha, const int32_t *status,
                                             const int32_t *tile_order, void *ws, size_t ws_bytes, float *v_xy,
                                             float *v_xy_abs, float *v_pix_vels, float *v_conic, float *v_colors,
-                                            float *v_opacity, void *stream) {
+                                            float *v_opacity, void *stream, const uint16_t *visit_mask = nullptr) {
     B200_REQUIRE(num_points >= 1, "num_points must be >= 1");
     B200_REQUIRE(num_entries >= 0, "num_entries must be >= 0");
     B200_REQUIRE(num_entries == 0 || gaussian_ids_sorted, "null gaussian_ids_sorted");
@@ -908,7 +940,7 @@ static int run_blend_backward_deterministic(int views, int num_points, int num_e
         int rc = run_blend_backward(num_points, img_height, img_width, block_width, n_blur_samples, gaussian_ids_sorted,
                                     tile_bins, packed, rolling_shutter_time, exposure_time, background, final_Ts,
                                     final_idx, v_output, v_output_alpha, v_xy, v_xy_abs, v_pix_vels, v_conic, v_colors,
-                                    v_opacity, true, st, tile_order, slots, views);
+                                    v_opacity, true, st, tile_order, slots, views, visit_mask);
         if (rc) return rc;
         uint32_t *keys_a = reinterpret_cast<uint32_t *>(base + L.keys_a);
         int32_t *pos_a = reinterpret_cast<int32_t *>(base + L.pos_a);
@@ -986,6 +1018,53 @@ extern "C" int b200_blend_backward_views_deterministic(int num_views, int num_re
                                             exposure_time, background, final_Ts, final_idx, v_output, v_output_alpha,
                                             nullptr, tile_order, ws, ws_bytes, v_xy, v_xy_abs, v_pix_vels, v_conic,
                                             v_colors, v_opacity, stream);
+}
+
+static int check_replay(int num_views, unsigned img_height, unsigned img_width, unsigned block_width,
+                        const int32_t *tile_order, const void *visit_mask) {
+    int rc = check_views_bwd(num_views, img_height, img_width, block_width, tile_order);
+    if (rc) return rc;
+    B200_REQUIRE(visit_mask, "null visit_mask");
+    B200_REQUIRE(b200_blend_records_visits(block_width), "visit records need the paired kernels (block_width 16)");
+    return B200_OK;
+}
+
+extern "C" int b200_blend_backward_replay(int num_views, int num_records, unsigned img_height, unsigned img_width,
+                                          unsigned block_width, unsigned n_blur_samples,
+                                          const int32_t *gaussian_ids_sorted, const int32_t *tile_bins,
+                                          const void *packed, float rolling_shutter_time, float exposure_time,
+                                          const float *background, const float *final_Ts, const int32_t *final_idx,
+                                          const float *v_output, const float *v_output_alpha, const void *visit_mask,
+                                          const int32_t *tile_order, float *v_xy, float *v_xy_abs, float *v_pix_vels,
+                                          float *v_conic, float *v_colors, float *v_opacity, int outputs_are_zero,
+                                          void *stream) {
+    int rc = check_replay(num_views, img_height, img_width, block_width, tile_order, visit_mask);
+    if (rc) return rc;
+    return run_blend_backward(num_records, img_height, img_width, block_width, n_blur_samples, gaussian_ids_sorted,
+                              tile_bins, packed, rolling_shutter_time, exposure_time, background, final_Ts, final_idx,
+                              v_output, v_output_alpha, v_xy, v_xy_abs, v_pix_vels, v_conic, v_colors, v_opacity,
+                              outputs_are_zero != 0, as_stream(stream), tile_order, nullptr, num_views,
+                              static_cast<const uint16_t *>(visit_mask));
+}
+
+extern "C" int b200_blend_backward_replay_deterministic(int num_views, int num_records, int num_entries,
+                                                        unsigned img_height, unsigned img_width, unsigned block_width,
+                                                        unsigned n_blur_samples, const int32_t *gaussian_ids_sorted,
+                                                        const int32_t *tile_bins, const void *packed,
+                                                        float rolling_shutter_time, float exposure_time,
+                                                        const float *background, const float *final_Ts,
+                                                        const int32_t *final_idx, const float *v_output,
+                                                        const float *v_output_alpha, const int32_t *status,
+                                                        const void *visit_mask, const int32_t *tile_order, void *ws,
+                                                        size_t ws_bytes, float *v_xy, float *v_xy_abs, float *v_pix_vels,
+                                                        float *v_conic, float *v_colors, float *v_opacity, void *stream) {
+    int rc = check_replay(num_views, img_height, img_width, block_width, tile_order, visit_mask);
+    if (rc) return rc;
+    return run_blend_backward_deterministic(num_views, num_records, num_entries, img_height, img_width, block_width,
+                                            n_blur_samples, gaussian_ids_sorted, tile_bins, packed, rolling_shutter_time,
+                                            exposure_time, background, final_Ts, final_idx, v_output, v_output_alpha,
+                                            status, tile_order, ws, ws_bytes, v_xy, v_xy_abs, v_pix_vels, v_conic,
+                                            v_colors, v_opacity, stream, static_cast<const uint16_t *>(visit_mask));
 }
 
 extern "C" int b200_rasterize_backward(int num_points, unsigned img_height, unsigned img_width, unsigned block_width,

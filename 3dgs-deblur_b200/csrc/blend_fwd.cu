@@ -35,6 +35,12 @@ struct BlendFwdParams {
                                // its pixels are rows v * H .. v * H + H - 1 of the (views * H, W) outputs
 };
 
+// what the recording forward writes besides the blend (b200_blend_forward_record)
+struct BlendFwdRecParams : BlendFwdParams {
+    uint16_t *visit_mask;  // (list position, warp) -> samples some lane of the warp blended the entry at
+    int32_t *tile_cost;    // per tile of the lists: the blended (warp visit, sample) pairs
+};
+
 // CTA -> (image, tile within the image)
 __device__ __forceinline__ void cta_tile(const int32_t *tile_order, const BlendGeom &g, int &view, int &tile) {
     const int t = tile_order ? __ldg(tile_order + blockIdx.x) : (int)blockIdx.x;
@@ -197,14 +203,24 @@ __global__ void __launch_bounds__(BLEND_THREADS, 1) blend_forward_kernel(const B
 // (alpha = 0 leaves T, the colour sums and `last` untouched).  There is no per-sample "does any lane pass" vote: with
 // the exact cull in front, 96 % of the sample blocks a warp enters at config 2 have a passing lane (execution counters,
 // -DB200_BLEND_COUNTERS), so the vote + branch would cost more than the masked arithmetic it skips.
+//
+// REC (the recording forward, b200_blend_forward_record): each warp also writes, for every list position it walks, the
+// samples at which some lane of the warp blended the entry (the lane's `ok` after the stop test, OR-reduced once per
+// visit, stored once per 32 entries as uint16 at (position, warp); 0 for culled and skipped entries), and the CTA
+// writes how many (visit, sample) pairs it blended to tile_cost.  The replaying backward walks exactly those visits
+// and samples (blend_bwd.cu); a warp's walk reaches at least its last blended entry, so every position the backward
+// reads is written.  The blend itself is the same instruction stream: outputs are bit-identical to REC = false.
 constexpr int FWD_MIN_CTAS = 6;  // 80 registers
-template <int S>
-__global__ void __launch_bounds__(128, FWD_MIN_CTAS) blend_forward_kernel2(const BlendFwdParams p) {
+template <int S, bool REC>
+__global__ void __launch_bounds__(128, FWD_MIN_CTAS)
+    blend_forward_kernel2(const std::conditional_t<REC, BlendFwdRecParams, BlendFwdParams> p) {
     constexpr int NT = 128;
+    static_assert(S <= 16, "the visit mask is 16 bits");
     __shared__ __align__(128) PackedGaussian s_rec[BLEND_STAGES][BLEND_BATCH];
     __shared__ __align__(8) uint64_t s_bar[BLEND_STAGES];
+    __shared__ int s_cost[NT / 32];
 
-    const int tid = threadIdx.x, lane = tid & 31;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     int view, tile;
     cta_tile(p.tile_order, p.g, view, tile);
     const int tile_x = tile % p.g.tbx, tile_y = tile / p.g.tbx;
@@ -224,6 +240,9 @@ __global__ void __launch_bounds__(128, FWD_MIN_CTAS) blend_forward_kernel2(const
     if (p.ref_isect && __ldg(p.ref_isect + view) < 1) {  // block-uniform
 #pragma unroll
         for (int q = 0; q < 2; ++q) write_empty_render<S>(p, inside[q], pi[q], pj[q]);
+        if constexpr (REC) {  // (the image's lists are empty, so the backward reads no visit mask of it)
+            if (tid == 0) p.tile_cost[view * (p.g.tbx * p.g.tby) + tile] = 0;
+        }
         return;
     }
     float blur[S];
@@ -252,6 +271,7 @@ __global__ void __launch_bounds__(128, FWD_MIN_CTAS) blend_forward_kernel2(const
 #pragma unroll
     for (int q = 0; q < 2; ++q) alive[q] = inside[q] ? ((1u << S) - 1u) : 0u;
     unsigned walive = __reduce_or_sync(0xffffffffu, alive[0] | alive[1]);  // samples some lane of the warp still blends
+    int cost = 0;  // REC: the warp's blended (visit, sample) pairs
 
     B200_COUNT_DECL;
     int b = 0;
@@ -272,6 +292,7 @@ __global__ void __launch_bounds__(128, FWD_MIN_CTAS) blend_forward_kernel2(const
                 unsigned m = __ballot_sync(0xffffffffu, my_mask != 0u);
                 if (e < cnt) B200_COUNT(0, 1);
                 const unsigned alive_chunk = alive[0] + alive[1];  // (bits only ever clear: the sum drops iff one did)
+                unsigned rec = 0u;  // REC: the warp's blended samples of entry c0 + lane
                 while (m) {
                     const int src = __ffs(m) - 1;
                     const int k = c0 + src;
@@ -288,6 +309,7 @@ __global__ void __launch_bounds__(128, FWD_MIN_CTAS) blend_forward_kernel2(const
                     const f2 CR = f2_splat(C.x * inv_s), CG = f2_splat(C.y * inv_s), CBl = f2_splat(C.z * inv_s);
                     const f2 dx0 = f2_sub(f2_splat(A.x), PX), dy0 = f2_sub(f2_splat(A.y), PY);
                     const int idx = start + k;
+                    unsigned blended = 0u;  // REC: samples this lane blended the entry at
 #ifdef B200_BLEND_COUNTERS
                     bool blended_ = false;
 #endif
@@ -329,10 +351,19 @@ __global__ void __launch_bounds__(128, FWD_MIN_CTAS) blend_forward_kernel2(const
                         T[s] = f2_make(ok0 ? f2_lo(nT) : f2_lo(T[s]), ok1 ? f2_hi(nT) : f2_hi(T[s]));
                         last[0][s] = ok0 ? idx : last[0][s];
                         last[1][s] = ok1 ? idx : last[1][s];
+                        if (REC && (ok0 || ok1)) blended |= 1u << s;
                     }
 #ifdef B200_BLEND_COUNTERS
                     if (__any_sync(0xffffffffu, blended_) && lane == 0) B200_COUNT(5, 1);
 #endif
+                    if constexpr (REC) {
+                        const unsigned wm = __reduce_or_sync(0xffffffffu, blended);
+                        rec = lane == src ? wm : rec;
+                        cost += __popc(wm);
+                    }
+                }
+                if constexpr (REC) {
+                    if (e < cnt) p.visit_mask[(size_t)(start + e) * (NT / 32) + warp] = (uint16_t)rec;
                 }
                 // the warp's live-sample set is refreshed once per 32 entries instead of after every visit (a vote + compare
                 // per visit for an event that happens S times per pixel): until then a sample that just finished for every
@@ -348,6 +379,11 @@ __global__ void __launch_bounds__(128, FWD_MIN_CTAS) blend_forward_kernel2(const
     }
     if (pending && b < nb) wait_batch(s_bar, b);  // drain the prefetch before exit
     B200_COUNT_FLUSH(0);
+    if constexpr (REC) {
+        if (lane == 0) s_cost[warp] = cost;
+        __syncthreads();
+        if (tid == 0) p.tile_cost[view * (p.g.tbx * p.g.tby) + tile] = s_cost[0] + s_cost[1] + s_cost[2] + s_cost[3];
+    }
 
     const float bg0 = __ldg(p.background), bg1 = __ldg(p.background + 1), bg2 = __ldg(p.background + 2);
 #pragma unroll
@@ -372,11 +408,13 @@ __global__ void __launch_bounds__(128, FWD_MIN_CTAS) blend_forward_kernel2(const
 }
 
 template <int S>
-static int launch_fwd(const BlendFwdParams &p, cudaStream_t st) {
+static int launch_fwd(const BlendFwdRecParams &p, cudaStream_t st) {
     // two pixels per lane when the tile is the full 16x16 (the only size Splatfacto uses, splatfacto.py:815)
     const int ctas = p.views * p.g.tbx * p.g.tby;
-    if (p.g.bw == 16 && !blend_force_one_pixel(false))
-        blend_forward_kernel2<S><<<ctas, BLEND_THREADS / 2, 0, st>>>(p);
+    if (p.visit_mask)
+        blend_forward_kernel2<S, true><<<ctas, BLEND_THREADS / 2, 0, st>>>(p);
+    else if (p.g.bw == 16 && !blend_force_one_pixel(false))
+        blend_forward_kernel2<S, false><<<ctas, BLEND_THREADS / 2, 0, st>>>(p);
     else
         blend_forward_kernel<S><<<ctas, BLEND_THREADS, 0, st>>>(p);
     B200_LAUNCH_CHECK();
@@ -388,13 +426,18 @@ static int launch_fwd(const BlendFwdParams &p, cudaStream_t st) {
 // One CTA counting-sorts the tiles by list length into ORDER_BUCKETS buckets spanning [0, longest]: exact for lists
 // shorter than ORDER_BUCKETS entries, and within a bucket the order is whatever the atomics give.  The result is a
 // permutation of [0, num_tiles) whatever tile_bins holds, so the blend covers every tile exactly once.
+// COST: the key is tile_cost (the recording forward's blended (visit, sample) pairs per tile) instead of the list length:
+// the order of the replaying backward, whose work those pairs are.
 constexpr int ORDER_THREADS = 1024, ORDER_BUCKETS = 2048;
+template <bool COST>
 static __global__ void __launch_bounds__(ORDER_THREADS) tile_order_kernel(int n, const int2 *__restrict__ bins,
+                                                                        const int32_t *__restrict__ cost,
                                                                         int32_t *__restrict__ order) {
     __shared__ int s_off[ORDER_BUCKETS];
     __shared__ int s_warp[ORDER_THREADS / 32];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     auto len = [&](int t) {
+        if constexpr (COST) return max(__ldg(cost + t), 0);
         const int2 r = bins[t];
         return (int)min(max((long long)r.y - (long long)r.x, 0ll), 0x7fffffffll);
     };
@@ -564,10 +607,22 @@ using namespace b200;
 extern "C" int b200_blend_tile_order(int num_tiles, const int32_t *tile_bins, int32_t *tile_order, void *stream) {
     B200_REQUIRE(num_tiles >= 1, "num_tiles must be >= 1");
     B200_REQUIRE(tile_bins && tile_order, "null pointer");
-    tile_order_kernel<<<1, ORDER_THREADS, 0, as_stream(stream)>>>(num_tiles, reinterpret_cast<const int2 *>(tile_bins),
-                                                                   tile_order);
+    tile_order_kernel<false><<<1, ORDER_THREADS, 0, as_stream(stream)>>>(
+        num_tiles, reinterpret_cast<const int2 *>(tile_bins), nullptr, tile_order);
     B200_LAUNCH_CHECK();
     return B200_OK;
+}
+
+extern "C" int b200_blend_tile_order_cost(int num_tiles, const int32_t *tile_cost, int32_t *tile_order, void *stream) {
+    B200_REQUIRE(num_tiles >= 1, "num_tiles must be >= 1");
+    B200_REQUIRE(tile_cost && tile_order, "null pointer");
+    tile_order_kernel<true><<<1, ORDER_THREADS, 0, as_stream(stream)>>>(num_tiles, nullptr, tile_cost, tile_order);
+    B200_LAUNCH_CHECK();
+    return B200_OK;
+}
+
+extern "C" int b200_blend_records_visits(unsigned block_width) {
+    return block_width == 16 && !blend_force_one_pixel(false) && !blend_force_one_pixel(true);
 }
 
 extern "C" size_t b200_packed_record_bytes(void) { return sizeof(PackedGaussian); }
@@ -576,14 +631,15 @@ static int run_blend_forward(unsigned img_height, unsigned img_width, unsigned b
                              const int32_t *gaussian_ids_sorted, const int32_t *tile_bins, const void *packed,
                              float rolling_shutter_time, float exposure_time, const float *background, float *out_img,
                              float *final_Ts, int32_t *final_idx, float *out_alpha, cudaStream_t st,
-                             const int32_t *ref_isect = nullptr, const int32_t *tile_order = nullptr, int views = 1) {
+                             const int32_t *ref_isect = nullptr, const int32_t *tile_order = nullptr, int views = 1,
+                             uint16_t *visit_mask = nullptr, int32_t *tile_cost = nullptr) {
     B200_REQUIRE(n_blur_samples > 0 && n_blur_samples <= B200_MAX_BLUR_SAMPLES, "unsupported blur size");  // bindings.cu:450-452
     B200_REQUIRE(block_width > 1 && block_width <= 16, "block_width must be between 2 and 16");
     B200_REQUIRE(img_height > 0 && img_width > 0, "image size must be positive");
     B200_REQUIRE(tile_bins && background && packed, "null input pointer");
     B200_REQUIRE(aligned16(packed), "packed records must be 16-byte aligned");
     B200_REQUIRE(out_img && final_Ts && final_idx, "null output pointer");
-    BlendFwdParams p;
+    BlendFwdRecParams p;
     p.g = blend_geom(img_height, img_width, block_width, rolling_shutter_time, exposure_time);
     p.ids_sorted = gaussian_ids_sorted;
     p.tile_bins = reinterpret_cast<const int2 *>(tile_bins);
@@ -593,6 +649,7 @@ static int run_blend_forward(unsigned img_height, unsigned img_width, unsigned b
     p.out_img = out_img; p.final_Ts = final_Ts; p.final_idx = final_idx; p.out_alpha = out_alpha;
     p.ref_isect = ref_isect;
     p.views = views;
+    p.visit_mask = visit_mask; p.tile_cost = tile_cost;
     return with_blur_samples(n_blur_samples, [&](auto s) { return launch_fwd<decltype(s)::value>(p, st); });
 }
 
@@ -668,6 +725,24 @@ extern "C" int b200_blend_forward_views(int num_views, unsigned img_height, unsi
     return run_blend_forward(img_height, img_width, block_width, n_blur_samples, gaussian_ids_sorted, tile_bins, packed,
                              rolling_shutter_time, exposure_time, background, out_img, final_Ts, final_idx, out_alpha,
                              as_stream(stream), view_isect, tile_order, num_views);
+}
+
+extern "C" int b200_blend_forward_record(int num_views, unsigned img_height, unsigned img_width, unsigned block_width,
+                                         unsigned n_blur_samples, const int32_t *gaussian_ids_sorted,
+                                         const int32_t *tile_bins, const void *packed, float rolling_shutter_time,
+                                         float exposure_time, const float *background, const int32_t *view_isect,
+                                         const int32_t *tile_order, float *out_img, float *final_Ts, int32_t *final_idx,
+                                         float *out_alpha, void *visit_mask, int32_t *tile_cost, void *stream) {
+    B200_REQUIRE(num_views >= 1, "num_views must be >= 1");
+    B200_REQUIRE(b200_blend_records_visits(block_width), "visit records need the paired kernels (block_width 16)");
+    B200_REQUIRE(tile_order && visit_mask && tile_cost, "null tile_order / visit_mask / tile_cost");
+    const long long tiles = (long long)((img_width + block_width - 1) / block_width) * ((img_height + block_width - 1) / block_width);
+    B200_REQUIRE((long long)num_views * tiles < 0x7fffffffll && (long long)num_views * img_height < 0x7fffffffll,
+                 "num_views * tiles exceeds int32");
+    return run_blend_forward(img_height, img_width, block_width, n_blur_samples, gaussian_ids_sorted, tile_bins, packed,
+                             rolling_shutter_time, exposure_time, background, out_img, final_Ts, final_idx, out_alpha,
+                             as_stream(stream), view_isect, tile_order, num_views, static_cast<uint16_t *>(visit_mask),
+                             tile_cost);
 }
 
 extern "C" int b200_blend_forward_packed_ordered(unsigned img_height, unsigned img_width, unsigned block_width,

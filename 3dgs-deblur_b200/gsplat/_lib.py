@@ -117,6 +117,13 @@ SIGNATURES = {
                                                                       _p, _p, _f, _f, _u, _u, _u, _f, _p, _p, _p, _p,
                                                                       _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p,
                                                                       _p, _p, _sz, _p]),
+    "b200_blend_records_visits": (_i, [_u]),
+    "b200_blend_forward_record": (_i, [_i, _u, _u, _u, _u, _p, _p, _p, _f, _f, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "b200_blend_tile_order_cost": (_i, [_i, _p, _p, _p]),
+    "b200_blend_backward_replay": (_i, [_i, _i, _u, _u, _u, _u, _p, _p, _p, _f, _f, _p, _p, _p, _p, _p, _p, _p,
+                                        _p, _p, _p, _p, _p, _p, _i, _p]),
+    "b200_blend_backward_replay_deterministic": (_i, [_i, _i, _i, _u, _u, _u, _u, _p, _p, _p, _f, _f, _p, _p, _p, _p, _p,
+                                                      _p, _p, _p, _p, _sz, _p, _p, _p, _p, _p, _p, _p]),
     "b200_nd_rasterize_forward": (_i, [_i, _u, _u, _u, _u, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
     "b200_nd_rasterize_backward": (_i, [_i, _u, _u, _u, _u, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p,
                                         _p, _p, _p, _p, _p, _p]),

@@ -6,6 +6,7 @@ code and tests that do `import gsplat.cuda as _C` keep working.  Tensors are all
 PyTorch and handed to the C ABI (include/b200splat.h) as raw device pointers on the current stream.
 """
 import functools
+from typing import NamedTuple
 
 import torch
 
@@ -328,36 +329,76 @@ def set_record_colors(packed, colors):
     return packed
 
 
+class VisitRecord(NamedTuple):
+    """What the recording blend forward (b200_blend_forward_record) saw, for its backward to replay: `mask` (uint16 bits
+    in int16 storage, 4 per list position) and `tile_cost` (int32 per tile).  Valid only with the forward's lists,
+    records and final_Ts / final_idx."""
+    mask: torch.Tensor
+    tile_cost: torch.Tensor
+
+
+def _record_visits(views, H, W, bw, gaussian_ids_sorted, tile_bins, packed, rs, ex, background, view_isect, out):
+    """Recording forward into `out` = (out_img, final_Ts, final_idx, alpha or None) -> (tile_order, VisitRecord).  When
+    the paired kernels do not run for this tile size nothing is launched but the order: -> (tile_order, None)."""
+    lib = _lib.load()
+    S = out[1].shape[-1]
+    order = _tile_order(tile_bins, H, W, bw, views)
+    if not lib.b200_blend_records_visits(bw):
+        return order, None
+    dev = packed.device
+    # sized from the list capacity, so the buffer is the same on every replay of a captured step
+    rec = VisitRecord(torch.empty((4 * max(gaussian_ids_sorted.numel(), 1),), dtype=torch.int16, device=dev),
+                      torch.empty((order.numel(),), dtype=torch.int32, device=dev))
+    check(lib.b200_blend_forward_record(
+        views, H, W, bw, S, ptr(gaussian_ids_sorted), ptr(tile_bins), ptr(packed), float(rs), float(ex),
+        ptr(_f32(background)), ptr(view_isect), ptr(order), *[ptr(t) for t in out], ptr(rec.mask), ptr(rec.tile_cost),
+        stream()))
+    return order, rec
+
+
 def blend_forward_packed(img_height, img_width, block_width, n_blur_samples, gaussian_ids_sorted, tile_bins, packed,
-                         rolling_shutter_time, exposure_time, background, want_alpha=False, *, status=None):
+                         rolling_shutter_time, exposure_time, background, want_alpha=False, *, status=None, record=False):
     """Extension: blend forward on prepacked records -> (out_img, final_Ts, final_idx[, alpha]); alpha = 1 - mean_s
-    final_Ts written by the same kernel (rasterize.py:161-163 computes it with two torch passes)."""
+    final_Ts written by the same kernel (rasterize.py:161-163 computes it with two torch passes).  record=True: one more
+    element, the VisitRecord to pass to blend_backward_packed(record=...) (None on tiles other than 16x16), written by
+    the same launch; the outputs are the same bit for bit."""
     require_cuda(gaussian_ids_sorted, tile_bins, packed, background)
     dev = packed.device
-    H, W, S = int(img_height), int(img_width), int(n_blur_samples)
+    H, W, S, bw = int(img_height), int(img_width), int(n_blur_samples), int(block_width)
+    rec = None
     with on_device(dev):
         out_img = torch.empty((H, W, 3), dtype=torch.float32, device=dev)
         final_Ts = torch.empty((H, W, S), dtype=torch.float32, device=dev)
         final_idx = torch.empty((H, W, S), dtype=torch.int32, device=dev)
         alpha = torch.empty((H, W), dtype=torch.float32, device=dev) if want_alpha else None
         # with `status` (capacity-mode lists) the reference's empty-render branch is taken on the device
-        order = _tile_order(tile_bins, H, W, int(block_width))
-        check(_lib.load().b200_blend_forward_packed_ordered(
-            H, W, int(block_width), S, ptr(gaussian_ids_sorted), ptr(tile_bins), ptr(packed), float(rolling_shutter_time),
-            float(exposure_time), ptr(_f32(background)), ptr(status), ptr(order), ptr(out_img), ptr(final_Ts), ptr(final_idx),
-            ptr(alpha), stream()))
-    if want_alpha:
-        return out_img, final_Ts, final_idx, alpha
-    return out_img, final_Ts, final_idx
+        outs = (out_img, final_Ts, final_idx, alpha)
+        if record:
+            order, rec = _record_visits(1, H, W, bw, gaussian_ids_sorted, tile_bins, packed, rolling_shutter_time,
+                                        exposure_time, background, status[3:] if status is not None else None, outs)
+        else:
+            order = _tile_order(tile_bins, H, W, bw)
+        if rec is None:
+            check(_lib.load().b200_blend_forward_packed_ordered(
+                H, W, bw, S, ptr(gaussian_ids_sorted), ptr(tile_bins), ptr(packed), float(rolling_shutter_time),
+                float(exposure_time), ptr(_f32(background)), ptr(status), ptr(order), *[ptr(t) for t in outs], stream()))
+    out = (out_img, final_Ts, final_idx, alpha) if want_alpha else (out_img, final_Ts, final_idx)
+    return out + (rec,) if record else out
 
 
 def blend_backward_packed(num_points, img_height, img_width, block_width, n_blur_samples, gaussian_ids_sorted, tile_bins,
                           packed, rolling_shutter_time, exposure_time, background, final_Ts, final_idx, v_output,
-                          v_output_alpha, *, status=None):
+                          v_output_alpha, *, status=None, record=None):
     """Extension: blend backward on prepacked records -> (v_xy, v_xy_abs, v_pix_vels, v_conic, v_colors, v_opacity).
     Under torch.use_deterministic_algorithms(True) the per-Gaussian sums are added in a fixed order
     (b200_blend_backward_packed_deterministic): bit-identical from call to call.  `status`: the capacity-mode status
-    block the lists were built with (its entry count marks where the padding starts); only read in that mode."""
+    block the lists were built with (its entry count marks where the padding starts); only read in that mode.
+    `record`: the VisitRecord of the forward that produced final_Ts / final_idx: the backward then visits only what
+    that forward blended, costliest tiles first (b200_blend_backward_replay); same gradients."""
+    if record is not None:
+        return _blend_backward_replay(1, num_points, img_height, img_width, block_width, n_blur_samples,
+                                      gaussian_ids_sorted, tile_bins, packed, rolling_shutter_time, exposure_time,
+                                      background, final_Ts, final_idx, v_output, v_output_alpha, status, record)
     require_cuda(gaussian_ids_sorted, tile_bins, packed, background)
     dev = packed.device
     n, H, W, bw, S = int(num_points), int(img_height), int(img_width), int(block_width), int(n_blur_samples)
@@ -379,6 +420,31 @@ def blend_backward_packed(num_points, img_height, img_width, block_width, n_blur
                 n, H, W, bw, S, ptr(gaussian_ids_sorted), ptr(tile_bins), ptr(packed), rs, ex, ptr(_f32(background)),
                 ptr(_f32(final_Ts)), ptr(final_idx), ptr(v_output), ptr(v_output_alpha), ptr(order),
                 *[ptr(t) for t in outs], 1, stream()))
+    return outs
+
+
+def _blend_backward_replay(views, n, H, W, bw, S, gaussian_ids_sorted, tile_bins, packed, rs, ex, background, final_Ts,
+                           final_idx, v_output, v_output_alpha, status, record):
+    require_cuda(gaussian_ids_sorted, tile_bins, packed, background, final_Ts, final_idx, record.mask)
+    dev = packed.device
+    views, n, H, W, bw, S, rs, ex = int(views), int(n), int(H), int(W), int(bw), int(S), float(rs), float(ex)
+    lib = _lib.load()
+    with on_device(dev):
+        v_output = _f32(v_output).contiguous()
+        v_output_alpha = _f32(v_output_alpha).contiguous() if v_output_alpha is not None else None
+        m = gaussian_ids_sorted.numel()
+        outs, ws, nbytes = _blend_backward_outputs(n, m, bw, dev)
+        order = torch.empty_like(record.tile_cost)
+        check(lib.b200_blend_tile_order_cost(order.numel(), ptr(record.tile_cost), ptr(order), stream()))
+        common = (H, W, bw, S, ptr(gaussian_ids_sorted), ptr(tile_bins), ptr(packed), rs, ex, ptr(_f32(background)),
+                  ptr(_f32(final_Ts)), ptr(final_idx), ptr(v_output), ptr(v_output_alpha))
+        if ws is not None:
+            check(lib.b200_blend_backward_replay_deterministic(views, n, m, *common, ptr(status), ptr(record.mask),
+                                                               ptr(order), ptr(ws), nbytes, *[ptr(t) for t in outs],
+                                                               stream()))
+        else:
+            check(lib.b200_blend_backward_replay(views, n, *common, ptr(record.mask), ptr(order),
+                                                 *[ptr(t) for t in outs], 1, stream()))
     return outs
 
 
@@ -471,32 +537,44 @@ def bin_cull_views(views, packed, depths, radii, num_tiles_hit, img_height, img_
 
 
 def blend_forward_views(views, img_height, img_width, block_width, n_blur_samples, gaussian_ids_sorted, tile_bins, packed,
-                        rolling_shutter_time, exposure_time, background, view_isect, want_alpha=True):
+                        rolling_shutter_time, exposure_time, background, view_isect, want_alpha=True, *, record=False):
     """Extension: blend forward of a view batch -> (out_img (B,H,W,3), final_Ts (B,H,W,S), final_idx (B,H,W,S)[, alpha
-    (B,H,W)]); a view whose view_isect is < 1 gets the reference's empty render."""
+    (B,H,W)]); a view whose view_isect is < 1 gets the reference's empty render.  record=True: one more element, the
+    VisitRecord for blend_backward_views(record=...), as in blend_forward_packed."""
     require_cuda(gaussian_ids_sorted, tile_bins, packed, background, view_isect)
     dev = packed.device
     B, H, W, bw, S = int(views), int(img_height), int(img_width), int(block_width), int(n_blur_samples)
+    rec = None
     with on_device(dev):
         out_img = torch.empty((B, H, W, 3), dtype=torch.float32, device=dev)
         final_Ts = torch.empty((B, H, W, S), dtype=torch.float32, device=dev)
         final_idx = torch.empty((B, H, W, S), dtype=torch.int32, device=dev)
         alpha = torch.empty((B, H, W), dtype=torch.float32, device=dev) if want_alpha else None
-        order = _tile_order(tile_bins, H, W, bw, B)
-        check(_lib.load().b200_blend_forward_views(
-            B, H, W, bw, S, ptr(gaussian_ids_sorted), ptr(tile_bins), ptr(packed), float(rolling_shutter_time),
-            float(exposure_time), ptr(_f32(background)), ptr(view_isect), ptr(order), ptr(out_img), ptr(final_Ts),
-            ptr(final_idx), ptr(alpha), stream()))
-    if want_alpha:
-        return out_img, final_Ts, final_idx, alpha
-    return out_img, final_Ts, final_idx
+        outs = (out_img, final_Ts, final_idx, alpha)
+        if record:
+            order, rec = _record_visits(B, H, W, bw, gaussian_ids_sorted, tile_bins, packed, rolling_shutter_time,
+                                        exposure_time, background, view_isect, outs)
+        else:
+            order = _tile_order(tile_bins, H, W, bw, B)
+        if rec is None:
+            check(_lib.load().b200_blend_forward_views(
+                B, H, W, bw, S, ptr(gaussian_ids_sorted), ptr(tile_bins), ptr(packed), float(rolling_shutter_time),
+                float(exposure_time), ptr(_f32(background)), ptr(view_isect), ptr(order), *[ptr(t) for t in outs],
+                stream()))
+    out = (out_img, final_Ts, final_idx, alpha) if want_alpha else (out_img, final_Ts, final_idx)
+    return out + (rec,) if record else out
 
 
 def blend_backward_views(views, num_records, img_height, img_width, block_width, n_blur_samples, gaussian_ids_sorted,
                          tile_bins, packed, rolling_shutter_time, exposure_time, background, final_Ts, final_idx, v_output,
-                         v_output_alpha):
+                         v_output_alpha, *, record=None):
     """Extension: blend backward of a view batch -> per-record (views * N rows) (v_xy, v_xy_abs, v_pix_vels, v_conic,
-    v_colors, v_opacity); deterministic under torch.use_deterministic_algorithms(True) like blend_backward_packed."""
+    v_colors, v_opacity); deterministic under torch.use_deterministic_algorithms(True) like blend_backward_packed.
+    `record`: the forward's VisitRecord, as in blend_backward_packed."""
+    if record is not None:
+        return _blend_backward_replay(views, num_records, img_height, img_width, block_width, n_blur_samples,
+                                      gaussian_ids_sorted, tile_bins, packed, rolling_shutter_time, exposure_time,
+                                      background, final_Ts, final_idx, v_output, v_output_alpha, None, record)
     require_cuda(gaussian_ids_sorted, tile_bins, packed, background, final_Ts, final_idx)
     dev = packed.device
     B, n, H, W, bw, S = int(views), int(num_records), int(img_height), int(img_width), int(block_width), int(n_blur_samples)

@@ -479,7 +479,8 @@ def fused_shading_phase(model: FlatGaussians, geo: Dict, scene: Dict, target: to
             check(lib.b200_fused_colors_forward_mode(mode, *args))
         else:
             check(lib.b200_fused_colors_forward(*args))
-        rgb, Ts, fi = _C.blend_forward_packed(H, W, bw, S, geo["ids"], geo["bins"], packed, rs, ex, bg, status=geo["status"])
+        rgb, Ts, fi, visits = _C.blend_forward_packed(H, W, bw, S, geo["ids"], geo["bins"], packed, rs, ex, bg,
+                                                      status=geo["status"], record=True)
     from gsplat.losses import l1_loss, l1_loss_and_grad
     ds = scene.get("target_downscale", 1)  # (as in shading_phase)
     kw = {} if ds == 1 else dict(downscale=ds)
@@ -492,7 +493,8 @@ def fused_shading_phase(model: FlatGaussians, geo: Dict, scene: Dict, target: to
         (v_rgb,) = torch.autograd.grad(loss, rgb)
     with torch.no_grad(), _lib.on_device(dev):
         v_xy, v_abs, v_pix, v_conic, v_col, v_op = _C.blend_backward_packed(
-            n, H, W, bw, S, geo["ids"], geo["bins"], packed, rs, ex, bg, Ts, fi, v_rgb, None, status=geo["status"])
+            n, H, W, bw, S, geo["ids"], geo["bins"], packed, rs, ex, bg, Ts, fi, v_rgb, None, status=geo["status"],
+            record=visits)
         g = {name: model.flat_grad[a:b_] for name, (a, b_) in model.slices.items()}
         g_vel = torch.empty(6, dtype=torch.float32, device=dev) if model.cam_vel is not None else None
         _C.fused_preprocess_backward(

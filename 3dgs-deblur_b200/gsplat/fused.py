@@ -206,7 +206,8 @@ class _FusedRender(Function):
             else:
                 check(lib.b200_fused_preprocess_forward_views(*args))
             view_isect, ids, bins = _C.bin_cull_views(B, packed, depths, radii, nth, H, W, bw, S, rs, ex)
-            rgb, Ts, fi, alpha = _C.blend_forward_views(B, H, W, bw, S, ids, bins, packed, rs, ex, bg, view_isect)
+            rgb, Ts, fi, alpha, ctx.visits = _C.blend_forward_views(B, H, W, bw, S, ids, bins, packed, rs, ex, bg, view_isect,
+                                                                    record=True)
             D = d_ids = d_bins = d_T = d_idx = None
             if depth:
                 d_isect, d_ids, d_bins = view_isect, ids, bins
@@ -241,7 +242,7 @@ class _FusedRender(Function):
         sink = ctx.grad_sink or {}
         with _lib.on_device(dev):
             v_xy, v_abs, v_pix, v_conic, v_col, v_op = _C.blend_backward_views(
-                B, B * n, H, W, bw, S, ids, bins, packed, rs, ex, bg, Ts, fi, v_rgb.contiguous(), v_alpha)
+                B, B * n, H, W, bw, S, ids, bins, packed, rs, ex, bg, Ts, fi, v_rgb.contiguous(), v_alpha, record=ctx.visits)
             ctx.info["absgrad"] = v_abs.view(*ctx.rows, 2)
             out = {}
             for name, like in zip(_RAW, (means, log_scales, quats, opacity_logit, sh_dc, sh_rest)):

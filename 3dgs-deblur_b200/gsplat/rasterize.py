@@ -147,9 +147,9 @@ class _RasterizeGaussians(Function):
             # records and blend; the list length, an overflow and the empty-render case are all decided on the device
             packed = _C.set_record_colors(prepared.packed, colors)
             ids_sorted, tile_bins = prepared.ids, prepared.bins
-            img, final_Ts, final_idx, alpha = _C.blend_forward_packed(H, W, bw, blur_samples, ids_sorted, tile_bins, packed,
-                                                                      rolling_shutter_time, exposure_time, background,
-                                                                      want_alpha=True, status=prepared.status)
+            img, final_Ts, final_idx, alpha, ctx.visits = _C.blend_forward_packed(
+                H, W, bw, blur_samples, ids_sorted, tile_bins, packed, rolling_shutter_time, exposure_time, background,
+                want_alpha=True, status=prepared.status, record=True)
             ctx.cfg = (H, W, bw, blur_samples, rolling_shutter_time, exposure_time, 1, True)
             ctx.status = prepared.status  # where the capacity-sized lists' padding starts (deterministic backward)
             ctx.save_for_backward(ids_sorted, tile_bins, xys, pix_vels, conics, colors, opacity, background, final_Ts,
@@ -182,9 +182,12 @@ class _RasterizeGaussians(Function):
             img, ids_sorted, tile_bins, final_Ts, final_idx = _empty_render(H, W, colors.shape[-1], blur_samples, background,
                                                                             xys.device)
         elif rgb:
-            img, final_Ts, final_idx, alpha = _C.blend_forward_packed(H, W, bw, blur_samples, ids_sorted, tile_bins, packed,
-                                                                      rolling_shutter_time, exposure_time, background,
-                                                                      want_alpha=True)
+            # a record of the blended visits for the backward to replay (device tensors only: the kernels record it)
+            out = _C.blend_forward_packed(H, W, bw, blur_samples, ids_sorted, tile_bins, packed, rolling_shutter_time,
+                                          exposure_time, background, want_alpha=True,
+                                          **({"record": True} if packed.is_cuda else {}))
+            img, final_Ts, final_idx, alpha = out[:4]
+            ctx.visits = out[4] if len(out) > 4 else None
         else:  # N-channel kernels (fp16 accumulators, no blur): un-culled two-level binning
             tile_bounds = ((W + bw - 1) // bw, (H + bw - 1) // bw, 1)
             ids_sorted, tile_bins = _C.bin_tiles(n_isect, xys, depths, radii, num_tiles_hit, tile_bounds, bw)
@@ -217,10 +220,12 @@ class _RasterizeGaussians(Function):
                 torch.zeros_like(t) for t in (xys, xys, pix_vels, conics, colors, opacity))
         elif has_packed:
             # grad_alpha None = zero alpha cotangent: the kernel then reads no (H, W) buffer for it
-            capacity_lists = {"status": ctx.status} if hasattr(ctx, "status") else {}
+            kw = {"status": ctx.status} if hasattr(ctx, "status") else {}
+            if getattr(ctx, "visits", None) is not None:
+                kw["record"] = ctx.visits
             v_xy, v_xy_abs, v_pix_vels, v_conic, v_colors, v_opacity = _C.blend_backward_packed(
                 xys.size(0), H, W, bw, n_samples, ids_sorted, tile_bins, packed, rs_time, exposure, background, final_Ts,
-                final_idx, grad_img.contiguous(), grad_alpha, **capacity_lists)
+                final_idx, grad_img.contiguous(), grad_alpha, **kw)
             v_opacity = v_opacity.reshape(opacity.shape)
         else:
             v_xy, v_xy_abs, v_pix_vels, v_conic, v_colors, v_opacity = _C.nd_rasterize_backward(

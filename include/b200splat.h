@@ -435,6 +435,50 @@ B200_API int b200_blend_backward_views_deterministic(int num_views, int num_reco
                                                      size_t ws_bytes, float *v_xy, float *v_xy_abs, float *v_pix_vels,
                                                      float *v_conic, float *v_colors, float *v_opacity, void *stream);
 
+/* ---- visit records: a backward that replays what its forward blended ------------------------------------------------
+ * b200_blend_records_visits(block_width): 1 when the three calls below run for that tile size (16x16 tiles, the paired
+ *   two-pixel kernels), else 0; callers then take the entry points above.
+ * b200_blend_forward_record = b200_blend_forward_views (num_views >= 1, one view = the single-image lists; view_isect
+ *   may be null: no empty-render branch; tile_order required) with the same outputs bit for bit, and in addition:
+ *   visit_mask, uint16[num_entries * 4] for the num_entries positions of gaussian_ids_sorted (the capacity in capacity
+ *   mode): at (list position, warp of the tile's CTA) the blur samples at which some pixel of that warp blended the
+ *   entry; tile_cost, int32[num_views * tiles]: per tile, the number of blended (warp, entry, sample) triples.
+ * b200_blend_tile_order_cost: b200_blend_tile_order keyed on tile_cost instead of the list length (costliest first).
+ * b200_blend_backward_replay(_deterministic) = b200_blend_backward_views(_deterministic) with the same results (the
+ *   deterministic ones bit for bit), but each warp visits only the entries and samples visit_mask records; status as
+ *   in b200_blend_backward_packed_deterministic (may be null); ws: b200_blend_backward_deterministic_ws_bytes.
+ * Between the forward and the backward the caller keeps alive, unchanged: gaussian_ids_sorted, tile_bins, packed,
+ *   final_Ts, final_idx and visit_mask (tile_cost only until b200_blend_tile_order_cost has run).  The backward reads a
+ *   mask only at positions up to its warp's last contributor, all of which the forward wrote; a mask from other lists,
+ *   records or outputs gives wrong gradients. */
+B200_API int b200_blend_records_visits(unsigned block_width);
+B200_API int b200_blend_forward_record(int num_views, unsigned img_height, unsigned img_width, unsigned block_width,
+                                       unsigned n_blur_samples, const int32_t *gaussian_ids_sorted,
+                                       const int32_t *tile_bins, const void *packed, float rolling_shutter_time,
+                                       float exposure_time, const float *background, const int32_t *view_isect,
+                                       const int32_t *tile_order, float *out_img, float *final_Ts, int32_t *final_idx,
+                                       float *out_alpha, void *visit_mask, int32_t *tile_cost, void *stream);
+B200_API int b200_blend_tile_order_cost(int num_tiles, const int32_t *tile_cost, int32_t *tile_order, void *stream);
+B200_API int b200_blend_backward_replay(int num_views, int num_records, unsigned img_height, unsigned img_width,
+                                        unsigned block_width, unsigned n_blur_samples, const int32_t *gaussian_ids_sorted,
+                                        const int32_t *tile_bins, const void *packed, float rolling_shutter_time,
+                                        float exposure_time, const float *background, const float *final_Ts,
+                                        const int32_t *final_idx, const float *v_output, const float *v_output_alpha,
+                                        const void *visit_mask, const int32_t *tile_order, float *v_xy, float *v_xy_abs,
+                                        float *v_pix_vels, float *v_conic, float *v_colors, float *v_opacity,
+                                        int outputs_are_zero, void *stream);
+B200_API int b200_blend_backward_replay_deterministic(int num_views, int num_records, int num_entries,
+                                                      unsigned img_height, unsigned img_width, unsigned block_width,
+                                                      unsigned n_blur_samples, const int32_t *gaussian_ids_sorted,
+                                                      const int32_t *tile_bins, const void *packed,
+                                                      float rolling_shutter_time, float exposure_time,
+                                                      const float *background, const float *final_Ts,
+                                                      const int32_t *final_idx, const float *v_output,
+                                                      const float *v_output_alpha, const int32_t *status,
+                                                      const void *visit_mask, const int32_t *tile_order, void *ws,
+                                                      size_t ws_bytes, float *v_xy, float *v_xy_abs, float *v_pix_vels,
+                                                      float *v_conic, float *v_colors, float *v_opacity, void *stream);
+
 /* ---- differentiable depth (splatfacto.py:881-897) ---------------------------------------------------------------------
  * D = the static blend (S = 1, no rolling shutter, zero background) of the records' view-space depths: the second
  * rasterize call Splatfacto makes with the depths as colours.  The records must come from the fused forward entry points
