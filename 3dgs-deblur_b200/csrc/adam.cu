@@ -110,6 +110,156 @@ __global__ void adam_head_kernel(int n, float *p, float *g, float *m, float *v, 
     if ((int)threadIdx.x < n) adam_one(p[threadIdx.x], g[threadIdx.x], m[threadIdx.x], v[threadIdx.x], a);
 }
 
+// ---- per-group learning rates ----------------------------------------------------------------------------------------
+// Splatfacto steps one Adam per parameter group, each with its own rate and scheduler (nerfstudio/configs/
+// method_configs.py: the splatfacto optimizers table).  Here one pass still updates any slice of the flat buffers: a
+// segment table maps each GLOBAL flat index to its group, and the prepare kernel leaves lr_g(s) / bc1 of every group in
+// a small device buffer.  Both tables travel by value in the kernel parameters (no copy, capturable).
+
+struct LrGroup {  // nerfstudio's ExponentialDecayScheduler (engine/schedulers.py), or a constant rate
+    double lr_init, lr_final, lr_pre_warmup, warmup_steps, max_steps;
+    int kind;  // 0 constant (lr_init exactly), 1 exponential decay
+    int ramp;  // 0 cosine, 1 linear
+};
+struct LrTable { int n; LrGroup g[B200_ADAM_MAX_GROUPS]; };
+
+struct Segment {  // [begin, end) global flat indices; period > 0: (i - begin) % period < split -> ga, else gb
+    long long begin, end;
+    int period, split, ga, gb;
+};
+struct SegTable { int n; Segment s[B200_ADAM_MAX_SEGMENTS]; };
+
+// nerfstudio's func(step) times LambdaLR's base rate, in double and in the Python expression's order
+__device__ double scheduled_lr(const LrGroup &G, long long s) {
+    if (G.kind == 0) return G.lr_init;  // exp(log(lr)) is not lr: a constant group never evaluates the formula
+    const double init = G.lr_init, pre = G.lr_pre_warmup, wu = G.warmup_steps, step = (double)s;
+    double lr;
+    if (step < wu) {
+        lr = G.ramp == 0 ? pre + (init - pre) * sin(0.5 * M_PI * fmin(fmax(step / wu, 0.0), 1.0))
+                         : pre + (init - pre) * step / wu;
+    } else {
+        const double t = fmin(fmax((step - wu) / (G.max_steps - wu), 0.0), 1.0);
+        lr = exp(log(init) * (1.0 - t) + log(G.lr_final) * t);
+    }
+    return init * (lr / init);  // LambdaLR: base_lr * (func_lr(step) / lr_init)
+}
+
+// adam_prepare_kernel's state update (AdamState.lr_over_bc1 takes group 0's constant), then one thread per group writes
+// (float)(lr_g(s) / bc1) with s = the index of the step being prepared (vetoed steps included).  A vetoed step leaves
+// the group constants as they were, as adam_prepare_kernel leaves lr_over_bc1.
+__global__ void adam_prepare_groups_kernel(AdamState *st, int32_t *veto_flag, double beta1, double beta2, LrTable tab,
+                                           float *group_lr) {
+    const int t = threadIdx.x;
+    const bool veto = veto_flag && *veto_flag != 0;
+    const int idx = st->seen, step = st->step + 1;
+    __syncthreads();  // every thread has read the state before thread 0 advances it
+    if (veto) {
+        if (t == 0) {
+            *veto_flag = 0;
+            st->seen = idx + 1;
+            st->skip = 1;
+            st->ring[st->vetoed % 10] = idx;
+            st->vetoed += 1;
+        }
+        return;
+    }
+    const double bc1 = 1.0 - pow(beta1, (double)step);
+    if (t < tab.n) group_lr[t] = (float)(scheduled_lr(tab.g[t], idx) / bc1);
+    if (t == 0) {
+        if (veto_flag) *veto_flag = 0;
+        st->seen = idx + 1;
+        st->skip = 0;
+        st->step = step;
+        const double bc2 = 1.0 - pow(beta2, (double)step);
+        st->lr_over_bc1 = (float)(scheduled_lr(tab.g[0], idx) / bc1);
+        st->inv_sqrt_bc2 = (float)(1.0 / sqrt(bc2));
+    }
+}
+
+__device__ __forceinline__ int segment_of(const SegTable &T, long long e) {
+    int j = -1;
+    for (int k = 0; k < T.n; ++k)
+        if (e >= T.s[k].begin && e < T.s[k].end) j = k;
+    return j;
+}
+
+__device__ __forceinline__ unsigned period_offset(const Segment &S, long long e) {
+    const unsigned long long off = (unsigned long long)(e - S.begin);
+    return off < (1ull << 32) ? (unsigned)off % (unsigned)S.period : (unsigned)(off % (unsigned long long)S.period);
+}
+
+__device__ __forceinline__ int group_at(const SegTable &T, long long e) {
+    const int j = segment_of(T, e);
+    if (j < 0) return -1;
+    const Segment &S = T.s[j];
+    if (S.period == 0) return S.ga;
+    return (int)period_offset(S, e) < S.split ? S.ga : S.gb;
+}
+
+// one element of group gi (-1: in no segment -- parameter and moments stay, the gradient is still cleared)
+__device__ __forceinline__ void adam_group_one(float &p, float &g, float &m, float &v, int gi, AdamArgs a,
+                                               const float *__restrict__ group_lr) {
+    if (gi < 0) {
+        if (a.zero_grad) g = 0.f;
+        return;
+    }
+    a.lr_over_bc1 = __ldg(group_lr + gi);
+    adam_one(p, g, m, v, a);
+}
+
+// adam_state_kernel with each element's lr / bc1 taken from its group.  `goff` = global flat index of slice element 0.
+__global__ void __launch_bounds__(ADAM_THREADS) adam_groups_kernel(long long n, long long goff, float *__restrict__ p,
+                                                                   float *__restrict__ g, float *__restrict__ m,
+                                                                   float *__restrict__ v, AdamArgs a,
+                                                                   const AdamState *__restrict__ st,
+                                                                   const float *__restrict__ group_lr, SegTable segs) {
+    a.inv_sqrt_bc2 = st->inv_sqrt_bc2;
+    const bool skip = st->skip != 0;
+    const long long n4 = n >> 2;
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    float4 *p4 = reinterpret_cast<float4 *>(p), *g4 = reinterpret_cast<float4 *>(g);
+    float4 *m4 = reinterpret_cast<float4 *>(m), *v4 = reinterpret_cast<float4 *>(v);
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride) {
+        if (skip) {
+            if (a.zero_grad) g4[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+            continue;
+        }
+        const long long e0 = goff + (i << 2);
+        float4 P = p4[i], G = g4[i], M = m4[i], V = v4[i];
+        const int j = segment_of(segs, e0);
+        int gi[4];
+        if (j >= 0 && e0 + 4 <= segs.s[j].end) {  // the whole vector lies in one segment
+            const Segment &S = segs.s[j];
+            if (S.period == 0) {  // fast path: one group, one constant
+                a.lr_over_bc1 = __ldg(group_lr + S.ga);
+                adam_one(P.x, G.x, M.x, V.x, a); adam_one(P.y, G.y, M.y, V.y, a);
+                adam_one(P.z, G.z, M.z, V.z, a); adam_one(P.w, G.w, M.w, V.w, a);
+                p4[i] = P; m4[i] = M; v4[i] = V;
+                if (a.zero_grad) g4[i] = G;
+                continue;
+            }
+            unsigned r = period_offset(S, e0);  // one division per vector, then step through the period
+#pragma unroll
+            for (int c = 0; c < 4; ++c) {
+                gi[c] = (int)r < S.split ? S.ga : S.gb;
+                r = r + 1 == (unsigned)S.period ? 0u : r + 1;
+            }
+        } else {
+#pragma unroll
+            for (int c = 0; c < 4; ++c) gi[c] = group_at(segs, e0 + c);
+        }
+        adam_group_one(P.x, G.x, M.x, V.x, gi[0], a, group_lr); adam_group_one(P.y, G.y, M.y, V.y, gi[1], a, group_lr);
+        adam_group_one(P.z, G.z, M.z, V.z, gi[2], a, group_lr); adam_group_one(P.w, G.w, M.w, V.w, gi[3], a, group_lr);
+        p4[i] = P; m4[i] = M; v4[i] = V;
+        if (a.zero_grad) g4[i] = G;
+    }
+    if (blockIdx.x == 0 && threadIdx.x < (int)(n & 3)) {
+        const long long i = (n4 << 2) + threadIdx.x;
+        if (skip) { if (a.zero_grad) g[i] = 0.f; }
+        else adam_group_one(p[i], g[i], m[i], v[i], group_at(segs, goff + i), a, group_lr);
+    }
+}
+
 }  // namespace b200
 
 using namespace b200;
@@ -209,4 +359,91 @@ extern "C" int b200_adam_step_state_background(long long numel, float *param, fl
     B200_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     return adam_state_launch(numel, param, grad, exp_avg, exp_avg_sq, state, beta1, beta2, eps, grad_scale, zero_grad,
                              (long long)sms * ctas_per_sm, stream);
+}
+
+// ---- per-group learning rates: host side ---------------------------------------------------------------------------
+extern "C" int b200_adam_prepare_groups(void *state, int32_t *veto_flag, int n_groups, const double *groups, double beta1,
+                                        double beta2, float *group_lr, void *stream) {
+    B200_REQUIRE(state && group_lr, "null state or group_lr");
+    B200_REQUIRE(n_groups >= 1 && n_groups <= B200_ADAM_MAX_GROUPS, "n_groups must be in [1, B200_ADAM_MAX_GROUPS]");
+    B200_REQUIRE(groups, "null group table");
+    B200_REQUIRE(beta1 >= 0.0 && beta1 < 1.0 && beta2 >= 0.0 && beta2 < 1.0, "betas must lie in [0, 1)");
+    LrTable tab{};
+    tab.n = n_groups;
+    for (int k = 0; k < n_groups; ++k) {
+        const double *w = groups + (size_t)k * B200_LR_GROUP_DOUBLES;
+        LrGroup &G = tab.g[k];
+        G.kind = (int)w[0]; G.lr_init = w[1]; G.lr_final = w[2]; G.lr_pre_warmup = w[3]; G.warmup_steps = w[4];
+        G.max_steps = w[5]; G.ramp = (int)w[6];
+        B200_REQUIRE(w[0] == 0.0 || w[0] == 1.0, "group kind must be 0 (constant) or 1 (exponential decay)");
+        B200_REQUIRE(w[1] >= 0.0, "learning rates must be >= 0");
+        if (G.kind == 1) {
+            B200_REQUIRE(w[1] > 0.0 && w[2] > 0.0, "an exponential decay needs lr_init > 0 and lr_final > 0");
+            B200_REQUIRE(w[3] >= 0.0 && w[4] >= 0.0 && w[5] > w[4], "need lr_pre_warmup >= 0, 0 <= warmup_steps < max_steps");
+            B200_REQUIRE(w[6] == 0.0 || w[6] == 1.0, "ramp must be 0 (cosine) or 1 (linear)");
+        }
+    }
+    adam_prepare_groups_kernel<<<1, 32, 0, as_stream(stream)>>>(static_cast<AdamState *>(state), veto_flag, beta1, beta2,
+                                                                tab, group_lr);
+    B200_LAUNCH_CHECK();
+    return B200_OK;
+}
+
+static int adam_groups_launch(long long numel, long long offset, float *param, float *grad, float *exp_avg, float *exp_avg_sq,
+                              int n_segments, const long long *segments, const void *state, const float *group_lr,
+                              double beta1, double beta2, double eps, double grad_scale, int zero_grad, long long max_blocks,
+                              void *stream) {
+    B200_REQUIRE(numel >= 0 && offset >= 0, "numel and offset must be >= 0");
+    B200_REQUIRE(n_segments >= 0 && n_segments <= B200_ADAM_MAX_SEGMENTS, "n_segments must be in [0, B200_ADAM_MAX_SEGMENTS]");
+    B200_REQUIRE(n_segments == 0 || segments, "null segment table");
+    SegTable segs{};
+    long long prev_end = -1;
+    for (int k = 0; k < n_segments; ++k) {
+        const long long *w = segments + (size_t)k * B200_ADAM_SEGMENT_WORDS;
+        B200_REQUIRE(w[0] >= 0 && w[0] < w[1] && w[0] >= prev_end, "segments must be non-empty, sorted and disjoint");
+        B200_REQUIRE(w[2] >= 0 && w[2] <= 0x7fffffff && w[3] >= 0 && w[3] <= w[2], "need 0 <= split <= period < 2^31");
+        B200_REQUIRE(w[4] >= 0 && w[4] < B200_ADAM_MAX_GROUPS && w[5] >= 0 && w[5] < B200_ADAM_MAX_GROUPS,
+                     "group indices must be in [0, B200_ADAM_MAX_GROUPS)");
+        prev_end = w[1];
+        if (w[1] <= offset || w[0] >= offset + numel) continue;  // only the segments this slice touches travel
+        Segment &S = segs.s[segs.n++];
+        S.begin = w[0]; S.end = w[1]; S.period = (int)w[2]; S.split = (int)w[3]; S.ga = (int)w[4]; S.gb = (int)w[5];
+    }
+    if (numel == 0) return B200_OK;
+    B200_REQUIRE(param && grad && exp_avg && exp_avg_sq && state && group_lr, "null pointer");
+    B200_REQUIRE(((reinterpret_cast<uintptr_t>(param) | reinterpret_cast<uintptr_t>(grad) | reinterpret_cast<uintptr_t>(exp_avg) |
+                   reinterpret_cast<uintptr_t>(exp_avg_sq)) & 15u) == 0,
+                 "the slice must start on a 16-byte boundary of the four buffers");
+    AdamArgs a;
+    a.lr_over_bc1 = 0.f; a.inv_sqrt_bc2 = 0.f;
+    a.one_minus_beta1 = (float)(1.0 - beta1); a.beta2 = (float)beta2; a.one_minus_beta2 = (float)(1.0 - beta2);
+    a.eps = (float)eps; a.grad_scale = (float)grad_scale; a.zero_grad = zero_grad ? 1 : 0;
+    const long long n4 = numel >> 2;
+    long long want = (n4 + ADAM_THREADS - 1) / ADAM_THREADS;
+    const int blocks = (int)(want < 1 ? 1 : (want > max_blocks ? max_blocks : want));
+    adam_groups_kernel<<<blocks, ADAM_THREADS, 0, as_stream(stream)>>>(numel, offset, param, grad, exp_avg, exp_avg_sq, a,
+                                                                      static_cast<const AdamState *>(state), group_lr, segs);
+    B200_LAUNCH_CHECK();
+    return B200_OK;
+}
+
+extern "C" int b200_adam_step_state_groups(long long numel, long long offset, float *param, float *grad, float *exp_avg,
+                                           float *exp_avg_sq, int n_segments, const long long *segments, const void *state,
+                                           const float *group_lr, double beta1, double beta2, double eps, double grad_scale,
+                                           int zero_grad, void *stream) {
+    return adam_groups_launch(numel, offset, param, grad, exp_avg, exp_avg_sq, n_segments, segments, state, group_lr, beta1,
+                              beta2, eps, grad_scale, zero_grad, 1ll << 30, stream);
+}
+
+extern "C" int b200_adam_step_state_groups_background(long long numel, long long offset, float *param, float *grad,
+                                                      float *exp_avg, float *exp_avg_sq, int n_segments,
+                                                      const long long *segments, const void *state, const float *group_lr,
+                                                      double beta1, double beta2, double eps, double grad_scale, int zero_grad,
+                                                      int ctas_per_sm, void *stream) {
+    B200_REQUIRE(ctas_per_sm >= 1 && ctas_per_sm <= 32, "ctas_per_sm must be in [1, 32]");
+    int dev = 0, sms = 0;
+    B200_CUDA(cudaGetDevice(&dev));
+    B200_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    return adam_groups_launch(numel, offset, param, grad, exp_avg, exp_avg_sq, n_segments, segments, state, group_lr, beta1,
+                              beta2, eps, grad_scale, zero_grad, (long long)sms * ctas_per_sm, stream);
 }

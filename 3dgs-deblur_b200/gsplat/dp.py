@@ -231,8 +231,8 @@ class ImageShardedTrainer:
         # when backward returns.  Exchange and update are pipelined over contiguous CHUNKS of the flat buffers (the
         # geometry block + `sh_chunks` pieces of the SH block): chunk i is updated as soon as its allreduce has landed,
         # while the allreduce of chunk i+1 is still on the wire.  Adam is per-element and every chunk sees the same step
-        # count and learning rate, so this is the same update as one optimizer over all parameters (a per-group
-        # learning rate would need chunk boundaries on parameter boundaries).  Every extra collective costs fixed latency on
+        # count and learning rate, so this is the same update as one optimizer over all parameters (this trainer keeps
+        # one rate; PipelinedTrainer's per-group rates map elements to groups by global index, independent of chunks).  Every extra collective costs fixed latency on
         # the NCCL stream that its pipelining has to hide, hence the default of one SH chunk + the geometry chunk.
         # optimizer = "b200": gsplat.optim.FlatAdam (one kernel per slice, clears the gradient slice in the same pass);
         # "torch": torch.optim.Adam per chunk (what the CPU/gloo tests of this host logic inject).
@@ -558,19 +558,30 @@ class PipelinedTrainer:
     Resolution schedule (`num_downscales` > 0, Splatfacto's splatfacto.py:660-667): image k (k = the step that trains on
     it) renders at 1/d_k of the scene's size, d_k = 2 ** max(num_downscales - k // resolution_schedule, 0), with fx, fy,
     cx, cy scaled by 1/d_k (Cameras.rescale_output_resolution, floor rounding); the loss still gets the full-resolution
-    target (see `_as_target`).  `render_size` = (H, W) of the image whose backward just ran, valid in `after_backward`."""
+    target (see `_as_target`).  `render_size` = (H, W) of the image whose backward just ran, valid in `after_backward`.
 
-    def __init__(self, model: FlatGaussians, scene: Dict, lr: float = 1e-3, group=None, loss_fn=None, use_graphs: bool = True,
+    Per-group learning rates (`lr` a dict or "splatfacto"; gsplat.optim.splatfacto_lr, method_configs.py:609-662): every
+    slice update gives each element its own group's rate, with the group's schedule evaluated on the device at the index
+    of the step being prepared (= `steps`, vetoed steps included).  `learning_rates()` reads them on the host.
+
+    SH degree ramp (`sh_degree_interval` > 0, Splatfacto's splatfacto.py:844): image k renders at SH degree
+    min(k // sh_degree_interval, sh_degree_to_use); the degree is part of the graph key and graphs of a lower degree are
+    dropped once the next degree starts."""
+
+    def __init__(self, model: FlatGaussians, scene: Dict, lr=1e-3, group=None, loss_fn=None, use_graphs: bool = True,
                  capacity: Optional[int] = None, sh_degree_to_use: int = 3, geometry_fn=None, shading_fn=None,
                  optimizer: str = "b200", sh_chunks: int = 1, operators: Optional[str] = None,
                  rasterize_mode: str = "antialiased", color_mode: str = "sh", num_downscales: int = 0,
-                 resolution_schedule: int = 3000):
+                 resolution_schedule: int = 3000, sh_degree_interval: int = 0):
         """operators: "dropin" = the two phases on the reference-compatible operators under autograd (`geometry_phase` /
         `shading_phase`); "fused" = on the fused raw-parameter kernels (`fused_geometry_phase` / `fused_shading_phase`:
         same numbers, ~45 fewer launches per step); None = fused where it applies (CUDA, sh_layout "split"), else drop-in.
         rasterize_mode ("antialiased" / "classic") and color_mode ("sh" / "sigmoid"): Splatfacto's two render switches, as
         in gsplat.fused.render_gaussians; both operator sets serve them (injected phases are called as they are).
-        num_downscales / resolution_schedule: Splatfacto's resolution schedule (class docstring); 0 trains at full size."""
+        num_downscales / resolution_schedule: Splatfacto's resolution schedule (class docstring); 0 trains at full size.
+        lr: a float (one rate for every parameter), or a dict of per-group rates keyed by gsplat.optim.GROUPS names (float
+        = constant, gsplat.optim.ExponentialDecay = scheduled), or "splatfacto" for gsplat.optim.splatfacto_lr().
+        sh_degree_interval: 0 = SH degree fixed at sh_degree_to_use; > 0 = Splatfacto's degree ramp (class docstring)."""
         self.model, self.scene = model, dict(scene)
         if int(num_downscales) != num_downscales or not 0 <= num_downscales <= 4:
             raise ValueError("num_downscales must be an integer from 0 to 4 (factors up to 16)")
@@ -585,10 +596,17 @@ class PipelinedTrainer:
         if loss_fn is None:
             from gsplat.losses import l1_loss as loss_fn
         self.loss_fn = loss_fn
-        self.sh_degree = sh_degree_to_use
+        if int(sh_degree_interval) != sh_degree_interval or sh_degree_interval < 0:
+            raise ValueError("sh_degree_interval must be a non-negative integer")
+        self.sh_degree_to_use, self.sh_degree_interval = sh_degree_to_use, int(sh_degree_interval)
+        self.sh_degree = sh_degree_to_use   # degree of the image the scene is currently set up for
         from gsplat._lib import render_mode
         render_mode(rasterize_mode, color_mode, "PipelinedTrainer")  # ValueError for an unknown mode
         self.rasterize_mode, self.color_mode = rasterize_mode, color_mode
+        if color_mode == "sigmoid":  # sigmoid(sh_dc) reads no SH basis: nothing to ramp
+            self.sh_degree_interval = 0
+        if self.sh_degree_interval:
+            self.sh_degree = self.sh_degree_at(0)
         fusable = model.flat.device.type == "cuda" and model.sh_layout == "split"
         if operators is None:
             operators = "fused" if fusable else "dropin"
@@ -635,9 +653,23 @@ class PipelinedTrainer:
         n_sh = max(1, int(sh_chunks)) if self.distributed else 1
         cuts = [lo + ((total - lo) * k // n_sh) // 4 * 4 for k in range(n_sh)] + [total]
         self._sh_bounds = [(cuts[k], cuts[k + 1]) for k in range(n_sh) if cuts[k + 1] > cuts[k]]
+        # per-group rates: None = one rate for the whole buffer (the float path, unchanged)
+        if isinstance(lr, str):
+            if lr != "splatfacto":
+                raise ValueError(f"lr must be a float, a dict of per-group rates or 'splatfacto', got {lr!r}")
+            from gsplat.optim import splatfacto_lr
+            lr = splatfacto_lr()
+        self.lr_groups = dict(lr) if isinstance(lr, dict) else None
+        if self.lr_groups is not None and optimizer != "b200":
+            raise ValueError("per-group learning rates need optimizer='b200' (the grouped device-state Adam)")
         if optimizer == "b200":
-            from gsplat.optim import FlatAdam
-            self.adam = FlatAdam(model.flat, model.flat_grad, lr=lr, eps=1e-15).use_device_state()
+            from gsplat.optim import FlatAdam, group_segments
+            if self.lr_groups is None:
+                self.adam = FlatAdam(model.flat, model.flat_grad, lr=lr, eps=1e-15).use_device_state()
+            else:
+                self.lr_group_names, scheds, segs = group_segments(model, self.lr_groups)
+                self.adam = FlatAdam(model.flat, model.flat_grad, lr=0.0, eps=1e-15).use_device_state(groups=scheds)
+                self.adam.set_groups(segs)
         elif optimizer == "torch":  # CPU / gloo tests of this host logic: same slices, torch's Adam, host-side veto
             self.adam = None
             lo, total = model.sh_start, model.flat.numel()
@@ -682,6 +714,19 @@ class PipelinedTrainer:
         """Splatfacto's _get_downscale_factor (splatfacto.py:660-667) for the image trained at step `image`."""
         return 2 ** max(self.num_downscales - int(image) // self.resolution_schedule, 0)
 
+    def sh_degree_at(self, image: int) -> int:
+        """Splatfacto's SH degree ramp (splatfacto.py:844) for the image trained at step `image`."""
+        if not self.sh_degree_interval:
+            return self.sh_degree_to_use
+        return min(int(image) // self.sh_degree_interval, self.sh_degree_to_use)
+
+    def learning_rates(self, step: Optional[int] = None):
+        """{group: rate} of step `step` (default: the next step, `steps`), computed on the host without a device sync;
+        None with a single float rate."""
+        if self.lr_groups is None or self.adam is None:
+            return None
+        return dict(zip(self.lr_group_names, self.adam.learning_rates(self.steps if step is None else step)))
+
     def _set_resolution(self, image):
         d = self._d = self.downscale_factor(image)
         f, s = self._full, self.scene
@@ -724,14 +769,15 @@ class PipelinedTrainer:
         key = self._key() + (target_shape_dtype,)
         e = self._graphs.get(key)
         if e is None:
-            e = self._graphs[key] = dict(gA=None, gB=None, geo=None, target=None, warm=0, d=self._d)
+            e = self._graphs[key] = dict(gA=None, gB=None, geo=None, target=None, warm=0, d=self._d, deg=self.sh_degree)
         return e
 
     def _drop_coarser_graphs(self):
-        """The schedule only ever lowers d: entries of a coarser stage never replay again.  Called at the start of a step,
-        when the last of them (phase B of the previous image) is already queued: the stream is drained first (once per
-        stage change) so that no graph or graph-pool memory is released while a replay still uses it."""
-        stale = [k for k, e in self._graphs.items() if e["d"] > self._d]
+        """The schedules only ever lower d and raise the SH degree: entries of an earlier stage never replay again.  Called
+        at the start of a step, when the last of them (phase B of the previous image) is already queued: the stream is
+        drained first (once per stage change) so that no graph or graph-pool memory is released while a replay still
+        uses it."""
+        stale = [k for k, e in self._graphs.items() if e["d"] > self._d or e["deg"] < self.sh_degree]
         if stale and self.cuda:
             torch.cuda.current_stream().synchronize()
         for key in stale:
@@ -840,6 +886,8 @@ class PipelinedTrainer:
         self._set_camera(cam, cam_index)
         if self._full is not None:  # the scene takes this image's resolution: A(image) and B(image) read it
             self._set_resolution(image)
+        if self.sh_degree_interval:  # and its SH degree (B(image) reads it; part of the graph key)
+            self.sh_degree = self.sh_degree_at(image)
         self._size_capacity()
         self._prepared = True
         self._A_done = False
@@ -860,7 +908,7 @@ class PipelinedTrainer:
 
     def _train_step(self, target, next_cam, next_index):
         m = self.model
-        if self._full is not None:
+        if self._full is not None or self.sh_degree_interval:
             self._drop_coarser_graphs()
         e = self._entry((tuple(target.shape), target.dtype))
         self._ensure_A(e)
@@ -943,7 +991,8 @@ class PipelinedTrainer:
 
     def on_resize(self):
         """The model's buffers were reallocated (gsplat.densify.Densifier.refine): drop the captured graphs (they address
-        the old buffers), recompute the exchange slices, put the new leaves on this trainer's stream.  The next step
+        the old buffers), recompute the exchange slices and the per-group segment table, put the new leaves on this
+        trainer's stream.  The next step
         re-sizes nothing else: the list capacity follows the polled high-water mark as before."""
         self.finish()
         self._graphs.clear()
@@ -954,6 +1003,9 @@ class PipelinedTrainer:
         n_sh = len(self._sh_bounds)
         cuts = [lo + ((total - lo) * k // n_sh) // 4 * 4 for k in range(n_sh)] + [total]
         self._sh_bounds = [(cuts[k], cuts[k + 1]) for k in range(n_sh) if cuts[k + 1] > cuts[k]]
+        if self.lr_groups is not None and self.adam is not None:  # every group boundary moved with N
+            from gsplat.optim import group_segments
+            self.adam.set_groups(group_segments(m, self.lr_groups)[2])
         if self.cuda:
             with torch.cuda.stream(self.main):
                 m.rebind_leaves()

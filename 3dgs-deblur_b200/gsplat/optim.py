@@ -5,11 +5,136 @@ The reference builds one `torch.optim.Adam(eps=1e-15)` per Splatfacto parameter 
 to the flat parameter / gradient buffers of `gsplat.dp.FlatGaussians`, and updates any `[begin, end)` slice with one
 kernel (`b200_adam_step`): a data-parallel trainer can update slice i while the gradient exchange of slice i+1 is still
 in flight, the gradient slice is cleared in the same pass (no separate zero_grad fill), and a step costs one C call
-instead of a Python optimizer round trip per slice.  CUDA only."""
+instead of a Python optimizer round trip per slice.  CUDA only.
+
+Per-group learning rates: Splatfacto gives every parameter group its own rate, and the means and camera-velocity groups a
+schedule (`splatfacto_lr`).  `group_segments` maps the flat layout to those groups, and `FlatAdam.use_device_state(groups=
+...)` + `set_groups(segments)` switch to the grouped device-state kernels (b200_adam_prepare_groups,
+b200_adam_step_state_groups), which give every element its own group's rate in the same single pass."""
+import math
+
+import numpy as np
 import torch
 
 from . import _lib
 from ._lib import check, stream
+
+
+class ExponentialDecay:
+    """nerfstudio's ExponentialDecayScheduler (engine/schedulers.py:92-141) with the config's defaults: from `lr_pre_warmup`
+    up to `lr_init` over `warmup_steps` (cosine or linear ramp), then exponentially down to `lr_final` at `max_steps`, and
+    flat after.  nerfstudio wraps it in LambdaLR (base rate times func(step) / lr_init); `lr_at(step)` is that product,
+    the rate iteration `step` of nerfstudio's trainer runs with (its schedulers step after the optimizers)."""
+
+    def __init__(self, lr_init: float, lr_final: float = None, warmup_steps: int = 0, lr_pre_warmup: float = 1e-8,
+                 max_steps: int = 100000, ramp: str = "cosine"):
+        if ramp not in ("cosine", "linear"):
+            raise ValueError("ExponentialDecay: ramp must be 'cosine' or 'linear'")
+        self.lr_init = float(lr_init)
+        self.lr_final = self.lr_init if lr_final is None else float(lr_final)
+        self.warmup_steps, self.max_steps = int(warmup_steps), int(max_steps)
+        self.lr_pre_warmup, self.ramp = float(lr_pre_warmup), ramp
+        if not (self.lr_init > 0 and self.lr_final > 0 and self.lr_pre_warmup >= 0
+                and 0 <= self.warmup_steps < self.max_steps):
+            raise ValueError("ExponentialDecay: need lr_init, lr_final > 0, lr_pre_warmup >= 0, 0 <= warmup_steps < max_steps")
+
+    def lr_at(self, step: int) -> float:
+        """Host value (float64) for logging; the device evaluates the same expression in double."""
+        init, pre, wu = self.lr_init, self.lr_pre_warmup, self.warmup_steps
+        if step < wu:
+            if self.ramp == "cosine":
+                lr = pre + (init - pre) * np.sin(0.5 * np.pi * np.clip(step / wu, 0, 1))
+            else:
+                lr = pre + (init - pre) * step / wu
+        else:
+            t = np.clip((step - wu) / (self.max_steps - wu), 0, 1)
+            lr = np.exp(np.log(init) * (1 - t) + np.log(self.lr_final) * t)
+        return float(init * (lr / init))
+
+    def row(self):
+        return [1.0, self.lr_init, self.lr_final, self.lr_pre_warmup, float(self.warmup_steps), float(self.max_steps),
+                0.0 if self.ramp == "cosine" else 1.0]
+
+    def __repr__(self):
+        return (f"ExponentialDecay(lr_init={self.lr_init}, lr_final={self.lr_final}, warmup_steps={self.warmup_steps}, "
+                f"lr_pre_warmup={self.lr_pre_warmup}, max_steps={self.max_steps}, ramp={self.ramp!r})")
+
+
+def lr_at(schedule, step: int) -> float:
+    """A group's rate at schedule position `step`: a float is constant, an ExponentialDecay is evaluated."""
+    return schedule.lr_at(step) if isinstance(schedule, ExponentialDecay) else float(schedule)
+
+
+def _group_row(schedule):
+    if isinstance(schedule, ExponentialDecay):
+        return schedule.row()
+    lr = float(schedule)
+    if not (math.isfinite(lr) and lr >= 0):
+        raise ValueError(f"learning rates must be finite and >= 0, got {schedule!r}")
+    return [0.0, lr, lr, 0.0, 0.0, 1.0, 0.0]
+
+
+# FlatGaussians field -> group, in group-index order.  The camera-velocity rows (n_cameras, 6) hold two groups:
+# columns 0-2 (linear) and 3-5 (angular)
+GROUPS = ("means", "log_scales", "quats", "opacity_logit", "sh_dc", "sh_rest", "cam_vel_linear", "cam_vel_angular")
+
+
+def splatfacto_lr():
+    """Splatfacto's per-group Adam rates and schedules (nerfstudio/configs/method_configs.py:609-662, every group with
+    eps 1e-15), keyed by FlatGaussians names: scales -> log_scales, opacities -> opacity_logit, features_dc / _rest ->
+    sh_dc / sh_rest, camera_velocity_opt_linear / _angular -> columns 0-2 / 3-5 of cam_vel."""
+    return dict(
+        means=ExponentialDecay(1.6e-4, lr_final=1.6e-6, max_steps=30000),
+        log_scales=0.005,
+        quats=0.001,
+        opacity_logit=0.05,
+        sh_dc=0.0025,
+        sh_rest=0.0025 / 20,
+        cam_vel_linear=ExponentialDecay(1e-3, lr_final=1e-6, max_steps=30000, warmup_steps=1000, lr_pre_warmup=0),
+        cam_vel_angular=ExponentialDecay(2e-4, lr_final=1e-7, max_steps=30000, warmup_steps=1000, lr_pre_warmup=0),
+    )
+
+
+def group_segments(model, lr):
+    """The group table and the segment table of a gsplat.dp.FlatGaussians for the rates `lr` (a dict keyed by GROUPS
+    names: float = constant rate, or an ExponentialDecay) -> (names, schedules, segments).  `names` / `schedules` are the
+    groups the model has, in GROUPS order (group index = position); `segments` are (begin, end, period, split, group_a,
+    group_b) rows over global flat indices, sorted.  Split SH layout: one segment per field; block layout: one periodic
+    segment over the (N, K, 3) block, the first 3 floats of each row sh_dc.  The camera rows are one periodic segment
+    (period 6, split 3).  The alignment pad belongs to no group.  ValueError for an unknown name and for a group the model
+    has without a rate; velocity rates for a model without camera rows are ignored, as nerfstudio ignores configured groups
+    that have no parameters."""
+    unknown = sorted(set(lr) - set(GROUPS))
+    if unknown:
+        raise ValueError(f"group_segments: unknown parameter group(s) {unknown}; known: {list(GROUPS)}")
+    sl = model.slices
+    present = [n for n in GROUPS[:4] if sl[n][1] > sl[n][0]]
+    if model.sh_layout == "block":
+        present += ["sh_dc"] + (["sh_rest"] if model.K > 1 else [])
+    else:
+        present += [n for n in ("sh_dc", "sh_rest") if sl[n][1] > sl[n][0]]
+    if model.cam_vel is not None:
+        present += ["cam_vel_linear", "cam_vel_angular"]
+    missing = [n for n in present if n not in lr]
+    if missing:
+        raise ValueError(f"group_segments: no learning rate for the model's group(s) {missing}")
+    idx = {n: i for i, n in enumerate(present)}
+    segs = []
+    for n in present[:4]:
+        segs.append((sl[n][0], sl[n][1], 0, 0, idx[n], idx[n]))
+    if model.cam_vel is not None:
+        a, b = sl["cam_vel"]
+        segs.append((a, b, 6, 3, idx["cam_vel_linear"], idx["cam_vel_angular"]))
+    if model.sh_layout == "block":
+        a, b = sl["sh"]
+        g_dc = idx["sh_dc"]
+        segs.append((a, b, 3 * model.K, 3, g_dc, idx.get("sh_rest", g_dc)))
+    else:
+        for n in ("sh_dc", "sh_rest"):
+            if n in idx:
+                segs.append((sl[n][0], sl[n][1], 0, 0, idx[n], idx[n]))
+    segs.sort()
+    return present, [lr[n] for n in present], segs
 
 
 class FlatAdam:
@@ -26,20 +151,57 @@ class FlatAdam:
         self._lib = _lib.load()
 
     # ---- device-resident step state (no host sync, CUDA-graph friendly) ------------------------------------------
-    def use_device_state(self):
+    def use_device_state(self, groups=None):
         """Switch to the device-resident step count / bias corrections / veto (b200_adam_prepare,
-        b200_adam_step_state): `prepare(veto_flag)` once per step, then `update_state(begin, end)` per slice."""
+        b200_adam_step_state): `prepare(veto_flag)` once per step, then `update_state(begin, end)` per slice.
+        groups: a list of per-group rates (float = constant, or ExponentialDecay; group index = position) for the grouped
+        kernels; `set_groups(segments)` then says which flat elements belong to which group.  `group_lr` (device
+        float32[groups]) holds each group's lr / (1 - beta1^step) of the last prepared step."""
         if getattr(self, "state", None) is None:
             nbytes = self._lib.b200_adam_state_bytes()
             self.state = torch.zeros(nbytes // 4, dtype=torch.int32, device=self.flat.device)
+        self.groups = None
+        if groups is not None:
+            groups = list(groups)
+            if not 1 <= len(groups) <= 16:
+                raise ValueError("FlatAdam: between 1 and 16 learning-rate groups (B200_ADAM_MAX_GROUPS)")
+            self._group_table = torch.tensor([_group_row(g) for g in groups], dtype=torch.float64)
+            self.groups = groups
+            self.group_lr = torch.zeros(len(groups), dtype=torch.float32, device=self.flat.device)
+            self._segments = torch.zeros((0, 6), dtype=torch.int64)
         return self
+
+    def set_groups(self, segments):
+        """The segment table of the grouped update: (begin, end, period, split, group_a, group_b) rows over GLOBAL flat
+        indices, sorted and disjoint (group_segments builds it from a model).  Elements in no segment are not updated."""
+        if getattr(self, "groups", None) is None:
+            raise ValueError("FlatAdam.set_groups: call use_device_state(groups=...) first")
+        segs = torch.tensor([list(map(int, s)) for s in segments], dtype=torch.int64).reshape(-1, 6)
+        if segs.shape[0] > 16:
+            raise ValueError("FlatAdam.set_groups: at most 16 segments (B200_ADAM_MAX_SEGMENTS)")
+        if segs.numel() and (int(segs[:, 4:].max()) >= len(self.groups) or int(segs[:, 4:].min()) < 0):
+            raise ValueError("FlatAdam.set_groups: a segment names a group index outside the group table")
+        self._segments = segs.contiguous()
+
+    def learning_rates(self, step: int):
+        """Each group's rate (float64) at schedule position `step` -- the index of a prepared step, vetoed ones included
+        (PipelinedTrainer.steps) -- computed on the host, no device sync.  None without groups."""
+        if getattr(self, "groups", None) is None:
+            return None
+        return [lr_at(g, int(step)) for g in self.groups]
 
     def prepare(self, veto_flag=None):
         """Once per step, before the first `update_state`.  veto_flag: device int32[1] (or None); non-zero skips this step's
         update on the device (gradients are still cleared) and is reset to zero."""
+        veto = None if veto_flag is None else veto_flag.data_ptr()
         with _lib.on_device(self.flat.device):
-            check(self._lib.b200_adam_prepare(self.state.data_ptr(), None if veto_flag is None else veto_flag.data_ptr(),
-                                              self.lr, self.betas[0], self.betas[1], stream()))
+            if getattr(self, "groups", None) is not None:
+                check(self._lib.b200_adam_prepare_groups(self.state.data_ptr(), veto, len(self.groups),
+                                                         self._group_table.data_ptr(), self.betas[0], self.betas[1],
+                                                         self.group_lr.data_ptr(), stream()))
+            else:
+                check(self._lib.b200_adam_prepare(self.state.data_ptr(), veto, self.lr, self.betas[0], self.betas[1],
+                                                  stream()))
 
     def update_state(self, begin: int = 0, end: int = None, grad_scale: float = 1.0, zero_grad: bool = True,
                      background_ctas: int = 0):
@@ -50,6 +212,17 @@ class FlatAdam:
             raise ValueError(f"FlatAdam.update_state: bad slice [{begin}, {end}) (must start on a 16-byte boundary)")
         off = 4 * begin
         p, g, m, v = self._ptrs
+        if getattr(self, "groups", None) is not None:  # every element at its own group's rate
+            segs = self._segments
+            with _lib.on_device(self.flat.device):
+                args = (end - begin, begin, p + off, g + off, m + off, v + off, segs.shape[0], segs.data_ptr(),
+                        self.state.data_ptr(), self.group_lr.data_ptr(), self.betas[0], self.betas[1], self.eps,
+                        float(grad_scale), 1 if zero_grad else 0)
+                if background_ctas > 0:
+                    check(self._lib.b200_adam_step_state_groups_background(*args, int(background_ctas), stream()))
+                else:
+                    check(self._lib.b200_adam_step_state_groups(*args, stream()))
+            return
         with _lib.on_device(self.flat.device):
             if background_ctas > 0:
                 check(self._lib.b200_adam_step_state_background(

@@ -712,6 +712,39 @@ B200_API int b200_adam_step_state_background(long long numel, float *param, floa
                                              const void *state, double beta1, double beta2, double eps, double grad_scale,
                                              int zero_grad, int ctas_per_sm, void *stream);
 
+/* Per-group learning rates (Splatfacto steps one Adam per parameter group, each with its own rate and scheduler:
+ * nerfstudio/configs/method_configs.py, the splatfacto optimizers).  Same state, same arithmetic; only lr differs.
+ *   groups: HOST double[n_groups][B200_LR_GROUP_DOUBLES], read during the call and passed to the kernel by value (so it
+ *       can be captured): {kind (0 constant, 1 exponential decay), lr_init, lr_final, lr_pre_warmup, warmup_steps,
+ *       max_steps, ramp (0 cosine, 1 linear)}.  Kind 1 is nerfstudio's ExponentialDecayScheduler (engine/schedulers.py)
+ *       under LambdaLR: lr_g(s) = lr_init * (func_lr(s) / lr_init), in double.  Kind 0 uses lr_init exactly.
+ *   b200_adam_prepare_groups: b200_adam_prepare's state update (AdamState's lr_over_bc1 takes group 0's value), then
+ *       group_lr[g] = (float)(lr_g(s) / (1 - beta1^step)) for every group: group_lr is DEVICE float[n_groups].  The
+ *       schedule position s is the index of the step being prepared, vetoed steps included: `steps prepared` (word [4])
+ *       before the increment.  Bias corrections count applied steps, as before.  A vetoed step leaves group_lr as it was.
+ *   b200_adam_step_state_groups: b200_adam_step_state over numel floats whose first one is GLOBAL flat index `offset`;
+ *       every element uses its own group's group_lr.  segments: HOST long long[n_segments][B200_ADAM_SEGMENT_WORDS],
+ *       sorted and disjoint, by value like `groups`: {begin, end, period, split, group_a, group_b}.  Global index i in
+ *       [begin, end) belongs to group_a when period == 0 or (i - begin) % period < split, else to group_b.  An element in
+ *       no segment keeps its parameter and moments bit-unchanged; its gradient is still cleared.  A vetoed step moves
+ *       nothing and clears the gradient slice.  The slice must start 16-byte aligned; it need not start or end on a
+ *       segment boundary. */
+#define B200_ADAM_MAX_GROUPS 16
+#define B200_ADAM_MAX_SEGMENTS 16
+#define B200_LR_GROUP_DOUBLES 7
+#define B200_ADAM_SEGMENT_WORDS 6
+B200_API int b200_adam_prepare_groups(void *state, int32_t *veto_flag, int n_groups, const double *groups, double beta1,
+                                      double beta2, float *group_lr, void *stream);
+B200_API int b200_adam_step_state_groups(long long numel, long long offset, float *param, float *grad, float *exp_avg,
+                                         float *exp_avg_sq, int n_segments, const long long *segments, const void *state,
+                                         const float *group_lr, double beta1, double beta2, double eps, double grad_scale,
+                                         int zero_grad, void *stream);
+B200_API int b200_adam_step_state_groups_background(long long numel, long long offset, float *param, float *grad,
+                                                    float *exp_avg, float *exp_avg_sq, int n_segments,
+                                                    const long long *segments, const void *state, const float *group_lr,
+                                                    double beta1, double beta2, double eps, double grad_scale, int zero_grad,
+                                                    int ctas_per_sm, void *stream);
+
 /* ---- rasterization without a host sync ---------------------------------------------------------------------------
  * The reference reads the intersection count back to size its lists (gsplat/utils.py:123-124 `.item()`); the two-phase
  * culled binning above reads the culled count.  In CAPACITY mode the caller sizes the lists from a running high-water
