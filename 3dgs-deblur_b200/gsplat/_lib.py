@@ -132,6 +132,9 @@ SIGNATURES = {
     "b200_nd_rasterize_forward": (_i, [_i, _u, _u, _u, _u, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
     "b200_nd_rasterize_backward": (_i, [_i, _u, _u, _u, _u, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p,
                                         _p, _p, _p, _p, _p, _p]),
+    "b200_camera_pose_apply": (_i, [_i, _i, _p, _p, _p, _p, _p]),
+    "b200_camera_pose_backward": (_i, [_i, _i, _p, _p, _p, _p, _p, _p]),
+    "b200_camera_l2": (_i, [_i, _p, _f, _f, _p, _p, _p]),
 }
 # render modes: each *_mode entry point is its base entry point behind a leading mode word (the view-batch backward's base
 # is the _depth one: v_depth is nullable there)

@@ -138,7 +138,7 @@ class Densifier:
             if n_splits:
                 z = (normal_samples or (lambda k: torch.randn((k, 3), device=dev)))(samps * n_splits).to(dev).float().contiguous()
             old = {k: v.detach() for k, v in p.items()}
-            old_cam = None if m.cam_vel is None else m.cam_vel.detach().clone()
+            old_cam = {k: getattr(m, k).detach().clone() for k in ("cam_vel", "cam_pose") if getattr(m, k) is not None}
             old_slices = dict(m.slices)
             old_flat = m.flat
             old_avg = old_sq = None
@@ -159,11 +159,11 @@ class Densifier:
                     for src_buf, dst_buf in ((old_avg, self.adam.exp_avg), (old_sq, self.adam.exp_avg_sq)):
                         check(lib.b200_densify_gather(n, samps, 3, width, src_buf.data_ptr() + 4 * a0, dst_buf.data_ptr() + 4 * a1,
                                                       ptr(ws), ptr(counts), None, None, None, stream()))
-            if old_cam is not None:  # camera rows are not Gaussians: carried over with their moments
-                m.cam_vel.data.copy_(old_cam)
+            for name, rows in old_cam.items():  # camera rows are not Gaussians: carried over with their moments
+                getattr(m, name).data.copy_(rows)
                 if self.adam is not None:
-                    a0, b0 = old_slices["cam_vel"]
-                    a1, b1 = m.slices["cam_vel"]
+                    a0, b0 = old_slices[name]
+                    a1, b1 = m.slices[name]
                     self.adam.exp_avg[a1:b1].copy_(old_avg[a0:b0])
                     self.adam.exp_avg_sq[a1:b1].copy_(old_sq[a0:b0])
             del old_flat

@@ -34,20 +34,27 @@ FIELDS = ("means", "log_scales", "quats", "opacity_logit", "sh_dc", "sh_rest")
 class FlatGaussians:
     """Gaussian parameters as views into one flat buffer (+ a flat gradient buffer of the same layout)."""
 
-    def __init__(self, scene: Dict, device, n_cameras: int = 0, optimize_velocities: bool = False, sh_layout: str = "split"):
+    def __init__(self, scene: Dict, device, n_cameras: int = 0, optimize_velocities: bool = False, sh_layout: str = "split",
+                 optimize_poses: bool = False):
         """sh_layout "split": sh_dc (N,1,3) and sh_rest (N,K-1,3) are two parameters like Splatfacto's features_dc /
         features_rest (the render block concatenates them every step, splatfacto.py:840-842; gsplat.fused reads them
         separately).  "block": ONE (N,K,3) parameter `sh` in the layout spherical_harmonics consumes -- no per-step
-        torch.cat (a 57 MB copy at 300k Gaussians) and no cat backward; `sh_dc` / `sh_rest` remain readable as views."""
+        torch.cat (a 57 MB copy at 300k Gaussians) and no cat backward; `sh_dc` / `sh_rest` remain readable as views.
+        optimize_poses: `cam_pose` (n_cameras, 6), one zero-initialised [trans | rot] SO3xR3 correction per training camera
+        (Splatfacto's camera optimiser, gsplat.camera_opt), placed after the velocity rows."""
         if sh_layout not in ("split", "block"):
             raise ValueError("sh_layout must be 'split' or 'block'")
+        if optimize_poses and n_cameras < 1:
+            raise ValueError("optimize_poses needs n_cameras >= 1")
         N = scene["means"].shape[0]
         K = scene["sh_rest"].shape[1] + 1
         self.N, self.K, self.sh_layout = N, K, sh_layout
+        self._n_vel = n_cameras if optimize_velocities else 0
+        self._n_pose = n_cameras if optimize_poses else 0
         widths = dict(means=3, log_scales=3, quats=4, opacity_logit=1, sh_dc=3, sh_rest=3 * (K - 1))
         shapes = dict(means=(N, 3), log_scales=(N, 3), quats=(N, 4), opacity_logit=(N, 1), sh_dc=(N, 1, 3),
                       sh_rest=(N, K - 1, 3))
-        extra = 6 * n_cameras if optimize_velocities else 0
+        extra = 6 * (self._n_vel + self._n_pose)
         # pad the camera rows so the SH coefficients start on a 16-byte boundary (the slice-wise device-state Adam and
         # the SH kernels' vector accesses want that)
         pad = (-(N * 11 + extra)) % 4
@@ -57,6 +64,7 @@ class FlatGaussians:
         self.params: Dict[str, torch.Tensor] = {}
         self.slices: Dict[str, tuple] = {}
         self.cam_vel: Optional[torch.Tensor] = None
+        self.cam_pose: Optional[torch.Tensor] = None
 
         def take(name, off, numel, shape):
             view = self.flat[off:off + numel].view(shape)
@@ -68,9 +76,8 @@ class FlatGaussians:
         off = 0
         for name in FIELDS:
             if name == "sh_dc":  # camera rows (+ alignment padding) sit between the geometry block and the SH block
-                if extra:
-                    self.cam_vel = take("cam_vel", off, extra, (n_cameras, 6))
-                off += extra + pad
+                off = self._take_camera_rows(take, off)
+                off += pad
                 if sh_layout == "block":
                     blk = self.flat[off:off + N * 3 * K].view(N, K, 3)
                     blk[:, :1].copy_(scene["sh_dc"].to(device).reshape(N, 1, 3))
@@ -92,6 +99,16 @@ class FlatGaussians:
         sh = self.params["sh"].detach()
         return {"sh_dc": sh[:, :1], "sh_rest": sh[:, 1:]}
 
+    def _take_camera_rows(self, take, off):
+        """The velocity rows, then the pose rows, from flat offset `off`; returns the offset after them."""
+        if self._n_vel:
+            self.cam_vel = take("cam_vel", off, 6 * self._n_vel, (self._n_vel, 6))
+            off += 6 * self._n_vel
+        if self._n_pose:
+            self.cam_pose = take("cam_pose", off, 6 * self._n_pose, (self._n_pose, 6))
+            off += 6 * self._n_pose
+        return off
+
     def rebind_leaves(self):
         """Replace every parameter by a fresh leaf tensor over the same storage (same .grad views).  Autograd ties a
         leaf's gradient accumulator to the stream that is current when the accumulator is first created; a trainer that
@@ -106,14 +123,17 @@ class FlatGaussians:
             new = self.cam_vel.detach().requires_grad_(True)
             new.grad = self.cam_vel.grad
             self.cam_vel = new
+        if self.cam_pose is not None:
+            new = self.cam_pose.detach().requires_grad_(True)
+            new.grad = self.cam_pose.grad
+            self.cam_pose = new
 
     def _reallocate(self, new_n: int):
         """New flat / gradient buffers for `new_n` Gaussians with the same field order, camera rows and layout rules; the
         parameter views are rebuilt (contents uninitialised: gsplat.densify.Densifier fills them).  Anything that cached
         pointers into the old buffers (optimizer, captured graphs) must be rebound by the caller."""
         K, dev = self.K, self.flat.device
-        n_cam = 0 if self.cam_vel is None else self.cam_vel.shape[0]
-        extra = 6 * n_cam
+        extra = 6 * (self._n_vel + self._n_pose)
         pad = (-(new_n * 11 + extra)) % 4
         widths = dict(means=3, log_scales=3, quats=4, opacity_logit=1, sh_dc=3, sh_rest=3 * (K - 1))
         shapes = dict(means=(new_n, 3), log_scales=(new_n, 3), quats=(new_n, 4), opacity_logit=(new_n, 1), sh_dc=(new_n, 1, 3),
@@ -121,7 +141,7 @@ class FlatGaussians:
         total = new_n * sum(widths.values()) + extra + pad
         self.flat = torch.zeros(total, dtype=torch.float32, device=dev)
         self.flat_grad = torch.zeros_like(self.flat)
-        self.params, self.slices, self.cam_vel, self.N = {}, {}, None, new_n
+        self.params, self.slices, self.cam_vel, self.cam_pose, self.N = {}, {}, None, None, new_n
 
         def take(name, off, numel, shape):
             pr = self.flat[off:off + numel].view(shape).requires_grad_(True)
@@ -132,9 +152,8 @@ class FlatGaussians:
         off = 0
         for name in FIELDS:
             if name == "sh_dc":
-                if extra:
-                    self.cam_vel = take("cam_vel", off, extra, (n_cam, 6))
-                off += extra + pad
+                off = self._take_camera_rows(take, off)
+                off += pad
                 if self.sh_layout == "block":
                     self.params["sh"] = take("sh", off, new_n * 3 * K, (new_n, K, 3))
                     self.slices["sh_dc"] = self.slices["sh_rest"] = self.slices["sh"]
@@ -155,16 +174,34 @@ class FlatGaussians:
         ps = list(self.params.values())
         if self.cam_vel is not None:
             ps.append(self.cam_vel)
+        if self.cam_pose is not None:
+            ps.append(self.cam_pose)
         return ps
 
     def zero_grad(self):
         self.flat_grad.zero_()
 
 
+def _posed_camera(model: FlatGaussians, cam: Dict, cam_index: int) -> Dict:
+    """`cam` at the optimised pose of camera `cam_index` (gsplat.camera_opt.apply_pose) when the model has pose rows: the
+    view matrix differentiable in model.cam_pose, cam_pos detached."""
+    if model.cam_pose is None:
+        return cam
+    from gsplat.camera_opt import apply_pose
+
+    dev = model.flat.device
+    row = torch.cat([cam["viewmat"].reshape(-1)[:12].to(dev), torch.zeros(6, device=dev),
+                     cam["cam_pos"].reshape(-1)[:3].to(dev)]).float()
+    viewmat, cam_pos = apply_pose(row, model.cam_pose, cam_index)
+    return dict(cam, viewmat=viewmat[0], cam_pos=cam_pos[0])
+
+
 def render(model: FlatGaussians, cam: Dict, scene: Dict, cam_index: int = 0, sh_degree_to_use: int = 3):
-    """The Splatfacto render block (splatfacto.py:816-880) on the public operators.  Returns (rgb, alpha, xys)."""
+    """The Splatfacto render block (splatfacto.py:816-880) on the public operators.  Returns (rgb, alpha, xys).  A model
+    with pose rows renders camera `cam_index` at its optimised pose."""
     from gsplat import project_gaussians, rasterize_gaussians, spherical_harmonics
 
+    cam = _posed_camera(model, cam, cam_index)
     p = model.params
     if model.cam_vel is not None:
         vel = model.cam_vel[cam_index] + cam["vel0"]
@@ -191,9 +228,11 @@ def render(model: FlatGaussians, cam: Dict, scene: Dict, cam_index: int = 0, sh_
 def render_fused(model: FlatGaussians, cam: Dict, scene: Dict, cam_index: int = 0, sh_degree_to_use: int = 3,
                  write_grads_in_place: bool = True):
     """Same render through gsplat.fused.render_gaussians (raw parameters in, one operator; SURVEY 8f-1).  With
-    `write_grads_in_place` the backward kernel overwrites the model's flat gradient buffer directly."""
+    `write_grads_in_place` the backward kernel overwrites the model's flat gradient buffer directly.  A model with pose
+    rows renders camera `cam_index` at its optimised pose; the pose gradient is accumulated into cam_pose.grad."""
     from gsplat.fused import render_gaussians
 
+    cam = _posed_camera(model, cam, cam_index)
     p = model.params
     if model.cam_vel is not None:
         vel = model.cam_vel[cam_index] + cam["vel0"]
@@ -216,6 +255,8 @@ class ImageShardedTrainer:
     def __init__(self, model: FlatGaussians, scene: Dict, lr: float = 1e-3, group=None, overlap_sh: bool = True,
                  fused: bool = False, loss_fn=None, sh_chunks: int = 1, optimizer: str = "b200"):
         self.model, self.scene = model, scene
+        if model.cam_pose is not None:
+            raise ValueError("ImageShardedTrainer does not optimise camera poses: use PipelinedTrainer(operators='fused')")
         if loss_fn is None:  # fused L1 (value + cotangent in one kernel); CUDA only, like the operators themselves
             from gsplat.losses import l1_loss as loss_fn
         self.loss_fn = loss_fn
@@ -417,7 +458,7 @@ def fused_geometry_phase(model: FlatGaussians, st: Dict, scene: Dict, capacity: 
     from gsplat._lib import check, ptr, stream
 
     p = model.params
-    cam = st["cam"]
+    cam = cam_in = st["cam"]
     with torch.no_grad():
         if model.cam_vel is not None:  # per-camera velocity rows (disjoint across images): row cam_index + dataset value
             vel = model.cam_vel.detach().index_select(0, st["cam_index"])[0] + cam[12:18]
@@ -429,6 +470,10 @@ def fused_geometry_phase(model: FlatGaussians, st: Dict, scene: Dict, capacity: 
         n, dev = model.N, model.flat.device
         lib = _lib.load()
         with _lib.on_device(dev):
+            if model.cam_pose is not None:  # the camera at its optimised pose: viewmat and cam_pos of the row adjusted
+                from gsplat.camera_opt import pose_apply_
+                cam = torch.empty_like(cam_in)
+                pose_apply_(cam_in, model.cam_pose.detach(), st["cam_index"], cam)
             packed = torch.empty((n * lib.b200_packed_record_bytes(),), dtype=torch.uint8, device=dev)
             depths = torch.empty((n,), dtype=torch.float32, device=dev)
             radii = torch.empty((n,), dtype=torch.int32, device=dev)
@@ -443,7 +488,7 @@ def fused_geometry_phase(model: FlatGaussians, st: Dict, scene: Dict, capacity: 
                 check(lib.b200_fused_geometry_forward(*args))
             ids, bins = _C.bin_cull_capacity(packed, depths, radii, nth, H, W, bw, blur, rs, ex, capacity, status)
     return dict(packed=packed, depths=depths, radii=radii, num_tiles_hit=nth, ids=ids, bins=bins, vel=vel, cam=cam,
-                cam_index=st["cam_index"], status=status, blur=blur, absgrad=None)
+                cam_in=cam_in, cam_index=st["cam_index"], status=status, blur=blur, absgrad=None)
 
 
 def fused_shading_phase(model: FlatGaussians, geo: Dict, scene: Dict, target: torch.Tensor, loss_fn, sh_degree_to_use: int = 3,
@@ -497,19 +542,25 @@ def fused_shading_phase(model: FlatGaussians, geo: Dict, scene: Dict, target: to
             record=visits)
         g = {name: model.flat_grad[a:b_] for name, (a, b_) in model.slices.items()}
         g_vel = torch.empty(6, dtype=torch.float32, device=dev) if model.cam_vel is not None else None
+        g_vm = torch.empty(12, dtype=torch.float32, device=dev) if model.cam_pose is not None else None
         _C.fused_preprocess_backward(
             dev, n, ptr(p["means"]), ptr(p["log_scales"]), ptr(p["quats"]), ptr(p["opacity_logit"]), ptr(p["sh_dc"]),
             ptr(p["sh_rest"]), K, sh_degree_to_use, ptr(cam), ptr(cam_pos), ptr(vel[:3]), ptr(vel[3:]), rs, ex, fx, fy, cx, cy,
             H, W, bw, _CLIP_THRESH, ptr(packed), ptr(radii), ptr(v_xy), ptr(v_pix), ptr(v_conic), ptr(v_col), ptr(v_op),
             ptr(g["means"]), ptr(g["log_scales"]), ptr(g["quats"]), ptr(g["opacity_logit"]), ptr(g["sh_dc"]), ptr(g["sh_rest"]),
-            ptr(g_vel[:3]) if g_vel is not None else None, ptr(g_vel[3:]) if g_vel is not None else None, None, mode=mode)
+            ptr(g_vel[:3]) if g_vel is not None else None, ptr(g_vel[3:]) if g_vel is not None else None, ptr(g_vm),
+            mode=mode)
         if g_vel is not None:
             g["cam_vel"].view(-1, 6).index_add_(0, geo["cam_index"], g_vel.view(1, 6))
+        if g_vm is not None:  # the view-matrix gradient through the pose correction into the camera's pose row
+            from gsplat.camera_opt import pose_backward_
+            pose_backward_(geo["cam_in"], model.cam_pose.detach(), geo["cam_index"], g_vm, g["cam_pose"])
     geo["absgrad"] = v_abs   # the `xys.absgrad` side channel of the drop-in operator (densification statistic)
     return loss.detach()
 
 
 _CLIP_THRESH = 0.01  # project_gaussians' default near plane (gsplat/gsplat/project_gaussians.py:31)
+
 
 
 def balanced_assignment(costs, world: int):
@@ -572,7 +623,7 @@ class PipelinedTrainer:
                  capacity: Optional[int] = None, sh_degree_to_use: int = 3, geometry_fn=None, shading_fn=None,
                  optimizer: str = "b200", sh_chunks: int = 1, operators: Optional[str] = None,
                  rasterize_mode: str = "antialiased", color_mode: str = "sh", num_downscales: int = 0,
-                 resolution_schedule: int = 3000, sh_degree_interval: int = 0):
+                 resolution_schedule: int = 3000, sh_degree_interval: int = 0, camera_l2=None):
         """operators: "dropin" = the two phases on the reference-compatible operators under autograd (`geometry_phase` /
         `shading_phase`); "fused" = on the fused raw-parameter kernels (`fused_geometry_phase` / `fused_shading_phase`:
         same numbers, ~45 fewer launches per step); None = fused where it applies (CUDA, sh_layout "split"), else drop-in.
@@ -581,7 +632,13 @@ class PipelinedTrainer:
         num_downscales / resolution_schedule: Splatfacto's resolution schedule (class docstring); 0 trains at full size.
         lr: a float (one rate for every parameter), or a dict of per-group rates keyed by gsplat.optim.GROUPS names (float
         = constant, gsplat.optim.ExponentialDecay = scheduled), or "splatfacto" for gsplat.optim.splatfacto_lr().
-        sh_degree_interval: 0 = SH degree fixed at sh_degree_to_use; > 0 = Splatfacto's degree ramp (class docstring)."""
+        sh_degree_interval: 0 = SH degree fixed at sh_degree_to_use; > 0 = Splatfacto's degree ramp (class docstring).
+        Camera pose rows (FlatGaussians(optimize_poses=True)): phase A renders each image at its camera's optimised pose
+        and phase B adds the pose-row gradient (gsplat.camera_opt); fused operators only.  lr="splatfacto" then includes
+        gsplat.optim.splatfacto_pose_lr(); a dict needs the two POSE_GROUPS rates.
+        camera_l2: None (default), "splatfacto" or a dict of weights trans / rot / linear / angular: Splatfacto's camera
+        regularisers (camera_optimizers.py:189-195, :267-273) over all pose rows (trans / rot) and all velocity rows
+        (linear / angular) every step, added to the returned loss and to the rows' gradients."""
         self.model, self.scene = model, dict(scene)
         if int(num_downscales) != num_downscales or not 0 <= num_downscales <= 4:
             raise ValueError("num_downscales must be an integer from 0 to 4 (factors up to 16)")
@@ -614,6 +671,13 @@ class PipelinedTrainer:
             raise ValueError("operators must be 'fused', 'dropin' or None")
         if operators == "fused" and not fusable and geometry_fn is None:
             raise ValueError("operators='fused' needs a CUDA model with sh_layout='split'")
+        if operators == "dropin" and getattr(model, "cam_pose", None) is not None:
+            raise ValueError("camera pose rows need operators='fused' (the drop-in path gets pose optimisation from "
+                             "nerfstudio's own CameraOptimizer)")
+        from gsplat.camera_opt import camera_l2_weights
+        self.camera_l2 = camera_l2_weights(camera_l2)
+        if self.camera_l2 is not None and model.flat.device.type != "cuda":
+            raise ValueError("camera_l2 needs a CUDA model (b200_camera_l2)")
         self.operators = operators
         phases = (fused_geometry_phase, fused_shading_phase) if operators == "fused" else (geometry_phase, shading_phase)
         modes = dict(rasterize_mode=rasterize_mode, color_mode=color_mode)
@@ -657,8 +721,10 @@ class PipelinedTrainer:
         if isinstance(lr, str):
             if lr != "splatfacto":
                 raise ValueError(f"lr must be a float, a dict of per-group rates or 'splatfacto', got {lr!r}")
-            from gsplat.optim import splatfacto_lr
+            from gsplat.optim import splatfacto_lr, splatfacto_pose_lr
             lr = splatfacto_lr()
+            if getattr(model, "cam_pose", None) is not None:
+                lr.update(splatfacto_pose_lr())
         self.lr_groups = dict(lr) if isinstance(lr, dict) else None
         if self.lr_groups is not None and optimizer != "b200":
             raise ValueError("per-group learning rates need optimizer='b200' (the grouped device-state Adam)")
@@ -824,12 +890,26 @@ class PipelinedTrainer:
             with torch.cuda.graph(g, stream=self.main):
                 tgt = self._as_target(e["target"])
                 self.loss.copy_(self.shading_fn(self.model, e["geo"], self.scene, tgt, self.loss_fn, self.sh_degree))
+                self._camera_regularisers()
             e["gB"], e["nB"] = g, self._lib_launches() - n0
             g.replay()
             return
         tgt = self._as_target(target)
         self.loss.copy_(self.shading_fn(self.model, self._geo, self.scene, tgt, self.loss_fn, self.sh_degree))
+        self._camera_regularisers()
         e["warm"] += 1
+
+    def _camera_regularisers(self):
+        """camera_l2: the regulariser values added to the step's loss, their gradients to the camera rows' gradients."""
+        w, m = self.camera_l2, self.model
+        if w is None:
+            return
+        from gsplat import _lib
+        from gsplat.camera_opt import camera_l2_
+        with _lib.on_device(m.flat.device):
+            for rows, a, b_ in ((m.cam_pose, w["trans"], w["rot"]), (m.cam_vel, w["linear"], w["angular"])):
+                if rows is not None:
+                    camera_l2_(rows.detach(), a, b_, rows.grad, self.loss)
 
     def _as_target(self, target):
         """The dataset's uint8 image goes to the loss as it is when the loss converts it in its own kernel

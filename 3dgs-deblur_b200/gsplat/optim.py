@@ -95,18 +95,32 @@ def splatfacto_lr():
     )
 
 
+# The camera pose rows (n_cameras, 6) of a model built with optimize_poses: columns 0-2 (translation) and 3-5 (rotation),
+# nerfstudio's camera_opt_trans / camera_opt_rot groups.  Their group indices follow the GROUPS the model has.
+POSE_GROUPS = ("cam_pose_trans", "cam_pose_rot")
+
+
+def splatfacto_pose_lr():
+    """Splatfacto's camera-optimiser rates (method_configs.py:634-645, eps 1e-15), keyed by POSE_GROUPS names:
+    camera_opt_trans -> columns 0-2 of cam_pose, camera_opt_rot -> columns 3-5."""
+    return dict(
+        cam_pose_trans=ExponentialDecay(2e-4, lr_final=1e-7, max_steps=30000, warmup_steps=500, lr_pre_warmup=0),
+        cam_pose_rot=ExponentialDecay(5e-5, lr_final=1e-7, max_steps=30000, warmup_steps=500, lr_pre_warmup=0),
+    )
+
+
 def group_segments(model, lr):
-    """The group table and the segment table of a gsplat.dp.FlatGaussians for the rates `lr` (a dict keyed by GROUPS
-    names: float = constant rate, or an ExponentialDecay) -> (names, schedules, segments).  `names` / `schedules` are the
-    groups the model has, in GROUPS order (group index = position); `segments` are (begin, end, period, split, group_a,
-    group_b) rows over global flat indices, sorted.  Split SH layout: one segment per field; block layout: one periodic
-    segment over the (N, K, 3) block, the first 3 floats of each row sh_dc.  The camera rows are one periodic segment
-    (period 6, split 3).  The alignment pad belongs to no group.  ValueError for an unknown name and for a group the model
-    has without a rate; velocity rates for a model without camera rows are ignored, as nerfstudio ignores configured groups
-    that have no parameters."""
-    unknown = sorted(set(lr) - set(GROUPS))
+    """The group table and the segment table of a gsplat.dp.FlatGaussians for the rates `lr` (a dict keyed by GROUPS and
+    POSE_GROUPS names: float = constant rate, or an ExponentialDecay) -> (names, schedules, segments).  `names` /
+    `schedules` are the groups the model has, in GROUPS then POSE_GROUPS order (group index = position); `segments` are
+    (begin, end, period, split, group_a, group_b) rows over global flat indices, sorted.  Split SH layout: one segment per
+    field; block layout: one periodic segment over the (N, K, 3) block, the first 3 floats of each row sh_dc.  The velocity
+    rows and the pose rows are one periodic segment each (period 6, split 3).  The alignment pad belongs to no group.
+    ValueError for an unknown name and for a group the model has without a rate; velocity or pose rates for a model
+    without those rows are ignored, as nerfstudio ignores configured groups that have no parameters."""
+    unknown = sorted(set(lr) - set(GROUPS) - set(POSE_GROUPS))
     if unknown:
-        raise ValueError(f"group_segments: unknown parameter group(s) {unknown}; known: {list(GROUPS)}")
+        raise ValueError(f"group_segments: unknown parameter group(s) {unknown}; known: {list(GROUPS + POSE_GROUPS)}")
     sl = model.slices
     present = [n for n in GROUPS[:4] if sl[n][1] > sl[n][0]]
     if model.sh_layout == "block":
@@ -115,6 +129,9 @@ def group_segments(model, lr):
         present += [n for n in ("sh_dc", "sh_rest") if sl[n][1] > sl[n][0]]
     if model.cam_vel is not None:
         present += ["cam_vel_linear", "cam_vel_angular"]
+    cam_pose = getattr(model, "cam_pose", None)
+    if cam_pose is not None:
+        present += list(POSE_GROUPS)
     missing = [n for n in present if n not in lr]
     if missing:
         raise ValueError(f"group_segments: no learning rate for the model's group(s) {missing}")
@@ -125,6 +142,9 @@ def group_segments(model, lr):
     if model.cam_vel is not None:
         a, b = sl["cam_vel"]
         segs.append((a, b, 6, 3, idx["cam_vel_linear"], idx["cam_vel_angular"]))
+    if cam_pose is not None:
+        a, b = sl["cam_pose"]
+        segs.append((a, b, 6, 3, idx["cam_pose_trans"], idx["cam_pose_rot"]))
     if model.sh_layout == "block":
         a, b = sl["sh"]
         g_dc = idx["sh_dc"]

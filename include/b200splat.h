@@ -796,6 +796,28 @@ B200_API int b200_densify_gather(int num_points, int n_split_samples, int field,
                                  const void *ws, const int32_t *counts, const float *log_scales, const float *quats,
                                  const float *randn, void *stream);
 
+/* ---- camera pose optimisation (Splatfacto's SO3xR3 camera optimiser) ---------------------------------------------------
+ * A camera row is 21 floats: viewmat (3x4 row major) 12 | lin_vel 3 | ang_vel 3 | cam_pos 3, as built from an OpenGL c2w by
+ * gsplat.data.to_gsplat_camera (viewmat = [R^T | -R^T t] with R = c2w's rotation times diag(1,-1,-1), cam_pos = t).  A
+ * pose row is 6 floats [trans 3 | rot 3], zero = no correction; pose is (num_cameras, 6), index DEVICE int64[num_views]
+ * names each view's pose row.  Nothing is read from the host, so all three may be captured in a CUDA graph.
+ *   b200_camera_pose_apply: out_rows[v] = row v with c2w' = c2w [exp_map_SO3xR3(pose[index[v]])] (cameras/lie_groups.py:
+ *       24-59, camera_optimizers.py:175-187) turned into viewmat and cam_pos as above (splatfacto.py:734-745, :843); the
+ *       velocities are copied.  A view whose index is outside [0, num_cameras) gets a row of NaNs.  out_rows must not alias rows.
+ *   b200_camera_pose_backward: g_viewmat (num_views, 12), the gradient of the ADJUSTED viewmats, becomes the pose-row
+ *       gradient, ADDED into g_pose (num_cameras, 6) at each view's index.  One CTA; views that share a pose row are added in
+ *       view order with separately rounded adds, so the result is deterministic and equals num_views sequential calls.
+ *       cam_pos carries no gradient (the reference detaches it).  Views with an out-of-range index add nothing.
+ *   b200_camera_l2: the camera regulariser (camera_optimizers.py:189-195, :267-273) of an (num_rows, 6) block split 3 | 3:
+ *       value[0] += w_a * mean_i |rows_i[0:3]| + w_b * mean_i |rows_i[3:6]|, and its gradient ADDED into g_rows (zero for
+ *       a zero-norm half, as torch gives it).  One CTA, a fixed summation order, no atomics. */
+B200_API int b200_camera_pose_apply(int num_views, int num_cameras, const float *rows, const float *pose,
+                                    const int64_t *index, float *out_rows, void *stream);
+B200_API int b200_camera_pose_backward(int num_views, int num_cameras, const float *rows, const float *pose,
+                                       const int64_t *index, const float *g_viewmat, float *g_pose, void *stream);
+B200_API int b200_camera_l2(int num_rows, const float *rows, float w_a, float w_b, float *g_rows, float *value,
+                            void *stream);
+
 #ifdef __cplusplus
 }
 #endif
