@@ -49,6 +49,7 @@ class Densifier:
         self.num_train_data = int(num_train_data)
         self.lib = _lib.load()
         self.grad_norm = self.vis_counts = self.max_2d = None
+        self.first_visible = None  # radii > 0 of the first image since the last refinement (reduce_stats reads it)
         self.last_size = None
         self.log = []
 
@@ -66,6 +67,7 @@ class Densifier:
             self.grad_norm = torch.empty(n, dtype=torch.float32, device=dev)
             self.vis_counts = torch.empty(n, dtype=torch.float32, device=dev)
             self.max_2d = torch.empty(n, dtype=torch.float32, device=dev)
+            self.first_visible = (radii.reshape(-1) > 0).float()
         self.last_size = (int(img_height), int(img_width))
         with _lib.on_device(dev):
             check(self.lib.b200_densify_accumulate(n, ptr(absgrad.contiguous().float()), ptr(radii.contiguous()),
@@ -74,15 +76,18 @@ class Densifier:
 
     def reduce_stats(self, group=None):
         """Data-parallel training: sum / sum / max of the statistics over the ranks, so every rank takes the same
-        decisions (the count that the first image sets to one on every rank is corrected for)."""
+        decisions -- those of one process that saw the ranks' images interleaved (rank 0's first image, rank 1's first
+        image, ..., rank 0's second image, ...).  The first image of a rank sets every count to one (:417-419), visible
+        or not; only rank 0's is the first of that sequence, so every other rank replaces that one by its first image's
+        visibility before the sum."""
         import torch.distributed as dist
 
         if self.grad_norm is None or not (dist.is_available() and dist.is_initialized()) or dist.get_world_size(group) == 1:
             return
-        world = dist.get_world_size(group)
         dist.all_reduce(self.grad_norm, op=dist.ReduceOp.SUM, group=group)
+        if dist.get_rank(group) > 0:
+            self.vis_counts += self.first_visible - 1.0
         dist.all_reduce(self.vis_counts, op=dist.ReduceOp.SUM, group=group)
-        self.vis_counts -= float(world - 1)
         dist.all_reduce(self.max_2d, op=dist.ReduceOp.MAX, group=group)
 
     # ---- refinement_after (:443-531)
@@ -111,7 +116,7 @@ class Densifier:
                     self.adam.exp_avg[a:b].zero_()
                     self.adam.exp_avg_sq[a:b].zero_()
             info = dict(info or {}, opacity_reset=True)
-        self.grad_norm = self.vis_counts = self.max_2d = None  # :523-525
+        self.grad_norm = self.vis_counts = self.max_2d = self.first_visible = None  # :523-525
         return info
 
     def _rebuild(self, step, do_densify, normal_samples):

@@ -312,22 +312,27 @@ def adam_constants(step, lr, betas=BETAS, eps=EPS):
     return dict(lrb=f(lr / bc1), isb=f(1.0 / np.sqrt(bc2)), omb1=f(1.0 - b1), b2=f(b2), omb2=f(1.0 - b2), eps=f(eps))
 
 
-def adam(p, g, m, v, step, lr, betas=BETAS, eps=EPS):
+def adam(p, g, m, v, step, lr, betas=BETAS, eps=EPS, g_err=None):
     """adam_one in float64 on fp32 inputs with the kernel's fp32 constants -> dict(p, m, v) of (value, bound) and
     `still`, the elements whose gradient and moments are all zero (their parameter stays bit-unchanged).  Every
     operation adds one rounding of its result (U |x| + the subnormal spacing), so the bound holds with or without FMA
-    contraction."""
+    contraction.  g_err: the gradient the kernel reads is not known exactly (a cross-rank sum in an unknown order, see
+    `exchanged`): `g` is then its float64 value and g_err its bound, carried through g - m and g * g."""
     k = adam_constants(step, lr, betas, eps)
-    p, g, m, v = (np.asarray(x, np.float32).astype(np.float64) for x in (p, g, m, v))
+    p, m, v = (np.asarray(x, np.float32).astype(np.float64) for x in (p, m, v))
+    if g_err is None:
+        g, ge = np.asarray(g, np.float32).astype(np.float64), 0.0
+    else:
+        g, ge = np.asarray(g, np.float64), np.asarray(g_err, np.float64)
     r = lambda x: U * np.abs(x) + TINY  # noqa: E731
     dlt = g - m
     t = k["omb1"] * dlt
     m1 = m + t
-    em = k["omb1"] * r(dlt) + r(t) + r(m1)
+    em = k["omb1"] * (r(dlt) + ge) + r(t) + r(m1)
     gg = g * g
     a_, b_ = k["b2"] * v, k["omb2"] * gg
     v1 = a_ + b_
-    ev = r(a_) + k["omb2"] * r(gg) + r(b_) + r(v1)
+    ev = r(a_) + k["omb2"] * (r(gg) + 2 * np.abs(g) * ge + ge * ge) + r(b_) + r(v1)
     s = np.sqrt(v1)
     with np.errstate(divide="ignore", invalid="ignore"):
         es = np.where(s > 0, np.minimum(np.sqrt(ev), ev / np.where(s > 0, s, 1.0)), np.sqrt(ev)) + r(s)
@@ -340,8 +345,22 @@ def adam(p, g, m, v, step, lr, betas=BETAS, eps=EPS):
     u = k["lrb"] * q
     p1 = p - u
     ep = k["lrb"] * eq + r(u) + r(p1)
-    still = (g == 0) & (m == 0) & (v == 0)
+    still = (g == 0) & (ge == 0) & (m == 0) & (v == 0)
     return dict(p=(p1, ep), m=(m1, em), v=(v1, ev), still=still)
+
+
+def exchanged(grads):
+    """The gradient FlatAdam reads after a data-parallel exchange of the fp32 per-rank gradients `grads` -> (value, bound).
+    gloo sums (in an order of its own) and the trainer folds grad_scale = fp32(1 / world) into Adam, which rounds the
+    product once; NCCL's AVG pre-multiplies every input by fp32(1 / world) (or divides the sum) in an order of its own,
+    and the scale is 1.  Either way: world - 1 additions and one scaling, each rounding at most U of the scaled sum of
+    |g_r|; the value is the exact sum times the exact 1 / world (fp32(1 / world) is within U of it)."""
+    gs = np.stack([np.asarray(x, np.float32).astype(np.float64) for x in grads])
+    world = gs.shape[0]
+    a = np.abs(gs).sum(0) / world
+    val = gs.sum(0) / world
+    err = (world + 2) * U * a + world * TINY * (a > 0)
+    return val, err
 
 
 def adam_fp32(p, g, m, v, step, lr, betas=BETAS, eps=EPS):

@@ -2,7 +2,9 @@
 
 The render itself needs the GPU library, so it is replaced by a differentiable stand-in with the same parameter
 interface; what is under test is the flat-buffer layout, the image -> rank assignment, the single gradient
-allreduce, replica equality after the optimizer step and the densification-statistic reductions."""
+allreduce, replica equality after the optimizer step and the densification-statistic reductions.  Also on the CPU:
+Densifier.reduce_stats against the reference's statistics over the ranks' images interleaved (world 2 and 3), and the
+cost-aware image grouping balanced_assignment."""
 import os
 import socket
 import sys
@@ -213,3 +215,115 @@ def test_pipelined_trainer_gloo(tmp_path, world):
     out = str(tmp_path / "flat2.pt")
     mp.spawn(_pipelined_worker, args=(world, _free_port(), out), nprocs=world, join=True)
     assert torch.isfinite(torch.load(out)).all()
+
+
+# ---- Densifier.reduce_stats: per-rank statistics -> those of the ranks' images interleaved ---------------------------
+
+def _rank_images(world, n_img, n=64, seed=0):
+    """images[k][r] = (absgrad (n, 2), radii (n,)) of rank r's k-th image; every Gaussian is invisible in some images,
+    visible in others, the first images included."""
+    g = torch.Generator().manual_seed(seed + world)
+    out = []
+    for _ in range(n_img):
+        row = []
+        for _ in range(world):
+            radii = torch.randint(0, 9, (n,), generator=g, dtype=torch.int32) * (torch.rand(n, generator=g) < 0.6)
+            absgrad = torch.rand(n, 2, generator=g) * (radii > 0)[:, None]
+            row.append((absgrad, radii.to(torch.int32)))
+        out.append(row)
+    return out
+
+
+def _reduce_worker(rank, world, port, out, n_img):
+    sys.path.insert(0, os.path.join(ROOT, "3dgs-deblur_b200"))
+    sys.path.insert(0, ROOT)
+    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
+    dist.init_process_group("gloo", rank=rank, world_size=world)
+    from gsplat.densify import Densifier
+    from oracle import densify_oracle as DO
+
+    images = _rank_images(world, n_img)
+    H, W = 48, 64
+    # this rank's statistics as the accumulate kernel leaves them (the reference's after_train over its own images)
+    # and its first image's visibility, which Densifier.accumulate records
+    own = {}
+    for k in range(n_img):
+        DO.accumulate(own, *images[k][rank], H, W)
+    den = Densifier(None)
+    den.grad_norm, den.vis_counts, den.max_2d = own["grad_norm"], own["vis_counts"], own["max_2d"]
+    den.first_visible = (images[0][rank][1] > 0).float()
+    den.reduce_stats()
+    want = {}
+    for k in range(n_img):
+        for r in range(world):
+            DO.accumulate(want, *images[k][r], H, W)
+    assert torch.equal(den.vis_counts, want["vis_counts"]), (den.vis_counts - want["vis_counts"]).abs().max()
+    assert torch.equal(den.max_2d, want["max_2d"])
+    torch.testing.assert_close(den.grad_norm, want["grad_norm"], rtol=1e-6, atol=0)  # (another summation order)
+    if rank == 0:
+        torch.save(den.vis_counts, out)
+    dist.destroy_process_group()
+
+
+@pytest.mark.parametrize("world", [2, 3])
+def test_densify_reduce_stats_is_the_interleaved_sequence(tmp_path, world):
+    """reduce_stats turns every rank's statistics into those of the interleaved sequence rank 0 image 0, rank 1 image 0,
+    ..., rank 0 image 1, ... as densify_oracle.accumulate (the reference's after_train) gives them: counts and max radii
+    exact.  Every rank's first image counts each Gaussian once; only the first image of the sequence may count an
+    invisible Gaussian."""
+    out = str(tmp_path / "vis.pt")
+    mp.spawn(_reduce_worker, args=(world, _free_port(), out, 3), nprocs=world, join=True)
+    assert torch.load(out).min() >= 1
+
+
+# ---- balanced_assignment ----------------------------------------------------------------------------------------------
+
+def _dp():
+    sys.path.insert(0, os.path.join(ROOT, "3dgs-deblur_b200"))
+    from gsplat import dp
+
+    return dp
+
+
+@pytest.mark.parametrize("world", [1, 2, 3, 4, 8])
+@pytest.mark.parametrize("n_steps", [1, 2, 3, 7, 16, 25])
+def test_balanced_assignment_groups_adjacent_costs(world, n_steps):
+    import random
+
+    dp = _dp()
+    rng = random.Random(world * 100 + n_steps)
+    costs = [rng.uniform(0.5, 1.5) for _ in range(world * n_steps)]
+    steps = dp.balanced_assignment(costs, world)
+    assert len(steps) == n_steps and all(len(s) == world for s in steps)
+    assert sorted(i for s in steps for i in s) == list(range(len(costs)))  # every image exactly once
+    # each step is a block of the cost order, and the steps are a permutation of those blocks
+    order = sorted(range(len(costs)), key=lambda i: -costs[i])
+    blocks = [order[j * world:(j + 1) * world] for j in range(n_steps)]
+    which = [next(j for j, b in enumerate(blocks) if sorted(b) == sorted(s)) for s in steps]
+    assert sorted(which) == list(range(n_steps))
+    assert dp.balanced_assignment(costs, world) == steps  # deterministic
+
+
+def test_balanced_assignment_ties_and_errors():
+    dp = _dp()
+    steps = dp.balanced_assignment([1.0] * 12, 4)
+    assert sorted(i for s in steps for i in s) == list(range(12))
+    assert sorted(tuple(sorted(s)) for s in steps) == [(0, 1, 2, 3), (4, 5, 6, 7), (8, 9, 10, 11)]  # ties: index order
+    for n, world in ((5, 2), (7, 3), (1, 2)):
+        with pytest.raises(ValueError):
+            dp.balanced_assignment([1.0] * n, world)
+
+
+@pytest.mark.parametrize("world", [2, 4, 8])
+def test_balanced_assignment_waits_no_longer_than_naive_groups(world):
+    """A synchronous step lasts as long as its costliest image: the sum over steps of max / mean (the idle share of the
+    step, + 1) is no larger than with the images grouped in index order, on random costs."""
+    import random
+
+    dp = _dp()
+    for seed in range(20):
+        rng = random.Random(seed)
+        costs = [rng.lognormvariate(0.0, 0.3) for _ in range(world * 24)]
+        ratio = lambda steps: sum(max(costs[i] for i in s) / (sum(costs[i] for i in s) / world) for s in steps)  # noqa: E731
+        naive = [list(range(j * world, (j + 1) * world)) for j in range(24)]
+        assert ratio(dp.balanced_assignment(costs, world)) <= ratio(naive)

@@ -38,8 +38,10 @@ def _within(name, actual, val, err):
                            f"{np.asarray(err)[bad][:3]}")
 
 
-def _trainer_inputs():
-    settings, rows, g, _ = SF.scene()
+def _trainer_inputs(scene=None):
+    """(settings, rows, gaussians, the trainer's scene dict, camera dicts) on the current device; `scene` = SF.scene()'s
+    result when the caller has it already (a worker process given it by its parent)."""
+    settings, rows, g, _ = SF.scene() if scene is None else scene
     cu = lambda a: torch.from_numpy(np.ascontiguousarray(a, np.float32)).cuda()  # noqa: E731
     n = len(g["means"])
     sc = dict(H=settings["H"], W=settings["W"], fx=settings["fx"], fy=settings["fy"], cx=settings["cx"], cy=settings["cy"],

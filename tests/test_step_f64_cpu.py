@@ -215,3 +215,47 @@ def test_adam_fp32_lies_within_the_f64_bound():
             assert np.median(out["p"][1] / ulp) < 4
         p, m, v = p1, m1, v1
     assert out["still"][:64].all()
+
+
+@pytest.mark.parametrize("world", [2, 3, 4])
+def test_adam_on_an_exchanged_gradient_lies_within_the_f64_bound(world):
+    """SF.exchanged + SF.adam(g_err=...): the fp32 exchanges the data-parallel trainer can see -- gloo's sum in any order
+    with grad_scale fp32(1 / world) folded into the update, NCCL's AVG as fp32(1 / world) pre-multiplied inputs summed in
+    any order, or the sum divided by world -- followed by adam_one in fp32 lie within the bound, down to subnormal
+    gradients; elements whose per-rank gradients and moments are all zero stay bit-unchanged."""
+    rng = np.random.default_rng(10 + world)
+    n = 1 << 14
+    p = (rng.normal(size=n) * 10.0 ** rng.uniform(-3, 1, n)).astype(np.float32)
+    m = (rng.normal(size=n) * 10.0 ** rng.uniform(-30, 0, n)).astype(np.float32)
+    v = (m.astype(np.float64) ** 2 * rng.uniform(1, 4, n)).astype(np.float32)
+    m[:64] = v[:64] = 0
+    gs = [(np.sign(rng.normal(size=n)) * 10.0 ** rng.uniform(-30, 2, n)).astype(np.float32) for _ in range(world)]
+    for g in gs:
+        g[rng.random(n) < 0.2] = 0
+        g[:64] = 0
+    gs[0][64:128] = -gs[1][64:128]  # exact cancellation
+    s = np.float32(1.0 / world)
+    with np.errstate(under="ignore"):
+        seen = []
+        for order in (list(range(world)), list(range(world))[::-1], list(rng.permutation(world))):
+            tot = gs[order[0]].copy()
+            for r in order[1:]:
+                tot = tot + gs[r]
+            seen += [tot, tot * s]  # gloo: the sum, scaled in the update; NCCL: the sum divided by world
+            pre = gs[order[0]] * s
+            for r in order[1:]:
+                pre = pre + gs[r] * s
+            seen.append(pre)        # NCCL: pre-multiplied inputs
+    val, err = SF.exchanged(gs)
+    assert (err[:64] == 0).all() and (val[:64] == 0).all()
+    for k, g in enumerate(seen):
+        out = SF.adam(p, val, m, v, 3, 1e-3, g_err=err)
+        # the gloo sum reaches the kernel unscaled: adam_one's first product is g * grad_scale
+        with np.errstate(under="ignore"):
+            gk = g * s if k % 3 == 0 else g
+        p1, m1, v1 = SF.adam_fp32(p, gk, m, v, 3, 1e-3)
+        _within("m", m1, *out["m"])
+        _within("v", v1, *out["v"])
+        _within("p", p1, *out["p"])
+        assert out["still"][:64].all() and not out["still"][64:].any()
+        assert np.array_equal(p1[:64].view(np.int32), p[:64].view(np.int32))
