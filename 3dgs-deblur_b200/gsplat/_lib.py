@@ -135,6 +135,10 @@ SIGNATURES = {
     "b200_camera_pose_apply": (_i, [_i, _i, _p, _p, _p, _p, _p]),
     "b200_camera_pose_backward": (_i, [_i, _i, _p, _p, _p, _p, _p, _p]),
     "b200_camera_l2": (_i, [_i, _p, _f, _f, _p, _p, _p]),
+    "b200_bg_scale_ws_bytes": (_sz, []),
+    "b200_background_forward": (_i, [_p, _p, _p]),
+    "b200_background_vjp": (_i, [C.c_longlong, _i, _p, _p, _p, _p, _p, _i, _p]),
+    "b200_scale_regularizer": (_i, [_i, _p, _f, _f, _i, _p, _p, _p, _p, _i, _p]),
 }
 # render modes: each *_mode entry point is its base entry point behind a leading mode word (the view-batch backward's base
 # is the _depth one: v_depth is nullable there)

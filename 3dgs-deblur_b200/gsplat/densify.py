@@ -143,7 +143,8 @@ class Densifier:
             if n_splits:
                 z = (normal_samples or (lambda k: torch.randn((k, 3), device=dev)))(samps * n_splits).to(dev).float().contiguous()
             old = {k: v.detach() for k, v in p.items()}
-            old_cam = {k: getattr(m, k).detach().clone() for k in ("cam_vel", "cam_pose") if getattr(m, k) is not None}
+            old_cam = {k: getattr(m, k).detach().clone() for k in ("cam_vel", "cam_pose", "learnable_bg")
+                       if getattr(m, k, None) is not None}
             old_slices = dict(m.slices)
             old_flat = m.flat
             old_avg = old_sq = None
@@ -164,7 +165,7 @@ class Densifier:
                     for src_buf, dst_buf in ((old_avg, self.adam.exp_avg), (old_sq, self.adam.exp_avg_sq)):
                         check(lib.b200_densify_gather(n, samps, 3, width, src_buf.data_ptr() + 4 * a0, dst_buf.data_ptr() + 4 * a1,
                                                       ptr(ws), ptr(counts), None, None, None, stream()))
-            for name, rows in old_cam.items():  # camera rows are not Gaussians: carried over with their moments
+            for name, rows in old_cam.items():  # camera rows and the background logit: carried over with their moments
                 getattr(m, name).data.copy_(rows)
                 if self.adam is not None:
                     a0, b0 = old_slices[name]

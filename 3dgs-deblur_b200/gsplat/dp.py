@@ -35,13 +35,15 @@ class FlatGaussians:
     """Gaussian parameters as views into one flat buffer (+ a flat gradient buffer of the same layout)."""
 
     def __init__(self, scene: Dict, device, n_cameras: int = 0, optimize_velocities: bool = False, sh_layout: str = "split",
-                 optimize_poses: bool = False):
+                 optimize_poses: bool = False, learnable_background: bool = False):
         """sh_layout "split": sh_dc (N,1,3) and sh_rest (N,K-1,3) are two parameters like Splatfacto's features_dc /
         features_rest (the render block concatenates them every step, splatfacto.py:840-842; gsplat.fused reads them
         separately).  "block": ONE (N,K,3) parameter `sh` in the layout spherical_harmonics consumes -- no per-step
         torch.cat (a 57 MB copy at 300k Gaussians) and no cat backward; `sh_dc` / `sh_rest` remain readable as views.
         optimize_poses: `cam_pose` (n_cameras, 6), one zero-initialised [trans | rot] SO3xR3 correction per training camera
-        (Splatfacto's camera optimiser, gsplat.camera_opt), placed after the velocity rows."""
+        (Splatfacto's camera optimiser, gsplat.camera_opt), placed after the velocity rows.
+        learnable_background: `learnable_bg` (3,), the zero-initialised logit of a learned background colour (Splatfacto's
+        background_color "auto": the blend's background is sigmoid(learnable_bg)), placed after the camera rows."""
         if sh_layout not in ("split", "block"):
             raise ValueError("sh_layout must be 'split' or 'block'")
         if optimize_poses and n_cameras < 1:
@@ -51,10 +53,11 @@ class FlatGaussians:
         self.N, self.K, self.sh_layout = N, K, sh_layout
         self._n_vel = n_cameras if optimize_velocities else 0
         self._n_pose = n_cameras if optimize_poses else 0
+        self._n_bg = 3 if learnable_background else 0
         widths = dict(means=3, log_scales=3, quats=4, opacity_logit=1, sh_dc=3, sh_rest=3 * (K - 1))
         shapes = dict(means=(N, 3), log_scales=(N, 3), quats=(N, 4), opacity_logit=(N, 1), sh_dc=(N, 1, 3),
                       sh_rest=(N, K - 1, 3))
-        extra = 6 * (self._n_vel + self._n_pose)
+        extra = 6 * (self._n_vel + self._n_pose) + self._n_bg
         # pad the camera rows so the SH coefficients start on a 16-byte boundary (the slice-wise device-state Adam and
         # the SH kernels' vector accesses want that)
         pad = (-(N * 11 + extra)) % 4
@@ -65,6 +68,7 @@ class FlatGaussians:
         self.slices: Dict[str, tuple] = {}
         self.cam_vel: Optional[torch.Tensor] = None
         self.cam_pose: Optional[torch.Tensor] = None
+        self.learnable_bg: Optional[torch.Tensor] = None
 
         def take(name, off, numel, shape):
             view = self.flat[off:off + numel].view(shape)
@@ -100,13 +104,17 @@ class FlatGaussians:
         return {"sh_dc": sh[:, :1], "sh_rest": sh[:, 1:]}
 
     def _take_camera_rows(self, take, off):
-        """The velocity rows, then the pose rows, from flat offset `off`; returns the offset after them."""
+        """The velocity rows, the pose rows, then the background logit, from flat offset `off`; returns the offset after
+        them."""
         if self._n_vel:
             self.cam_vel = take("cam_vel", off, 6 * self._n_vel, (self._n_vel, 6))
             off += 6 * self._n_vel
         if self._n_pose:
             self.cam_pose = take("cam_pose", off, 6 * self._n_pose, (self._n_pose, 6))
             off += 6 * self._n_pose
+        if self._n_bg:
+            self.learnable_bg = take("learnable_bg", off, 3, (3,))
+            off += 3
         return off
 
     def rebind_leaves(self):
@@ -127,13 +135,17 @@ class FlatGaussians:
             new = self.cam_pose.detach().requires_grad_(True)
             new.grad = self.cam_pose.grad
             self.cam_pose = new
+        if self.learnable_bg is not None:
+            new = self.learnable_bg.detach().requires_grad_(True)
+            new.grad = self.learnable_bg.grad
+            self.learnable_bg = new
 
     def _reallocate(self, new_n: int):
         """New flat / gradient buffers for `new_n` Gaussians with the same field order, camera rows and layout rules; the
         parameter views are rebuilt (contents uninitialised: gsplat.densify.Densifier fills them).  Anything that cached
         pointers into the old buffers (optimizer, captured graphs) must be rebound by the caller."""
         K, dev = self.K, self.flat.device
-        extra = 6 * (self._n_vel + self._n_pose)
+        extra = 6 * (self._n_vel + self._n_pose) + self._n_bg
         pad = (-(new_n * 11 + extra)) % 4
         widths = dict(means=3, log_scales=3, quats=4, opacity_logit=1, sh_dc=3, sh_rest=3 * (K - 1))
         shapes = dict(means=(new_n, 3), log_scales=(new_n, 3), quats=(new_n, 4), opacity_logit=(new_n, 1), sh_dc=(new_n, 1, 3),
@@ -141,7 +153,8 @@ class FlatGaussians:
         total = new_n * sum(widths.values()) + extra + pad
         self.flat = torch.zeros(total, dtype=torch.float32, device=dev)
         self.flat_grad = torch.zeros_like(self.flat)
-        self.params, self.slices, self.cam_vel, self.cam_pose, self.N = {}, {}, None, None, new_n
+        self.params, self.slices, self.cam_vel, self.cam_pose, self.learnable_bg = {}, {}, None, None, None
+        self.N = new_n
 
         def take(name, off, numel, shape):
             pr = self.flat[off:off + numel].view(shape).requires_grad_(True)
@@ -176,6 +189,8 @@ class FlatGaussians:
             ps.append(self.cam_vel)
         if self.cam_pose is not None:
             ps.append(self.cam_pose)
+        if self.learnable_bg is not None:
+            ps.append(self.learnable_bg)
         return ps
 
     def zero_grad(self):
@@ -196,9 +211,16 @@ def _posed_camera(model: FlatGaussians, cam: Dict, cam_index: int) -> Dict:
     return dict(cam, viewmat=viewmat[0], cam_pos=cam_pos[0])
 
 
+def _background(model: FlatGaussians, scene: Dict):
+    """The render's background: sigmoid(learnable_bg) (splatfacto.py:706-709), differentiable in the row, for a model
+    that learns it; scene["background"] otherwise."""
+    return torch.sigmoid(model.learnable_bg) if model.learnable_bg is not None else scene["background"]
+
+
 def render(model: FlatGaussians, cam: Dict, scene: Dict, cam_index: int = 0, sh_degree_to_use: int = 3):
     """The Splatfacto render block (splatfacto.py:816-880) on the public operators.  Returns (rgb, alpha, xys).  A model
-    with pose rows renders camera `cam_index` at its optimised pose."""
+    with pose rows renders camera `cam_index` at its optimised pose; a model with `learnable_bg` blends over
+    sigmoid(learnable_bg), whose gradient is accumulated into learnable_bg.grad."""
     from gsplat import project_gaussians, rasterize_gaussians, spherical_harmonics
 
     cam = _posed_camera(model, cam, cam_index)
@@ -221,7 +243,7 @@ def render(model: FlatGaussians, cam: Dict, scene: Dict, cam_index: int = 0, sh_
     rgb, alpha = rasterize_gaussians(xys, depths, pix_vels, radii, conics, num_tiles_hit, rgbs, opacities, H, W, bw,
                                      rolling_shutter_time=scene["rolling_shutter_time"],
                                      exposure_time=scene["exposure_time"], blur_samples=blur,
-                                     background=scene["background"], return_alpha=True)
+                                     background=_background(model, scene), return_alpha=True)
     return rgb, alpha, xys, radii
 
 
@@ -229,7 +251,8 @@ def render_fused(model: FlatGaussians, cam: Dict, scene: Dict, cam_index: int = 
                  write_grads_in_place: bool = True):
     """Same render through gsplat.fused.render_gaussians (raw parameters in, one operator; SURVEY 8f-1).  With
     `write_grads_in_place` the backward kernel overwrites the model's flat gradient buffer directly.  A model with pose
-    rows renders camera `cam_index` at its optimised pose; the pose gradient is accumulated into cam_pose.grad."""
+    rows renders camera `cam_index` at its optimised pose; the pose gradient is accumulated into cam_pose.grad.  A model
+    with `learnable_bg` blends over sigmoid(learnable_bg); its gradient is accumulated into learnable_bg.grad."""
     from gsplat.fused import render_gaussians
 
     cam = _posed_camera(model, cam, cam_index)
@@ -244,7 +267,7 @@ def render_fused(model: FlatGaussians, cam: Dict, scene: Dict, cam_index: int = 
     rgb, alpha, info = render_gaussians(
         p["means"], p["log_scales"], p["quats"], p["opacity_logit"], p["sh_dc"], p["sh_rest"], cam["viewmat"],
         cam["cam_pos"], lin, ang, cam["fx"], cam["fy"], cam["cx"], cam["cy"], scene["H"], scene["W"],
-        scene["block_width"], scene["background"], rolling_shutter_time=scene["rolling_shutter_time"],
+        scene["block_width"], _background(model, scene), rolling_shutter_time=scene["rolling_shutter_time"],
         exposure_time=scene["exposure_time"], blur_samples=blur, sh_degree_to_use=sh_degree_to_use, grad_sink=sink)
     return rgb, alpha, info
 
@@ -257,6 +280,8 @@ class ImageShardedTrainer:
         self.model, self.scene = model, scene
         if model.cam_pose is not None:
             raise ValueError("ImageShardedTrainer does not optimise camera poses: use PipelinedTrainer(operators='fused')")
+        if model.learnable_bg is not None:
+            raise ValueError("ImageShardedTrainer does not learn a background: use PipelinedTrainer(operators='fused')")
         if loss_fn is None:  # fused L1 (value + cotangent in one kernel); CUDA only, like the operators themselves
             from gsplat.losses import l1_loss as loss_fn
         self.loss_fn = loss_fn
@@ -498,7 +523,9 @@ def fused_shading_phase(model: FlatGaussians, geo: Dict, scene: Dict, target: to
     SH, clamp, sigmoid * compensation, projection VJP, exp, normalisation) that writes the model's flat gradient buffer
     row by row -- no accumulate passes, no memsets.  The gradient rows are OVERWRITTEN (the buffer is zero between steps:
     FlatAdam clears what it consumes); the camera-velocity row is accumulated.  The two render modes as in
-    `geometry_phase` / `shading_phase`, through the _mode entry points."""
+    `geometry_phase` / `shading_phase`, through the _mode entry points.  A model with `learnable_bg` blends over
+    sigmoid(learnable_bg) (geo["background"], written on the device) and writes the logit's gradient
+    (gsplat.background)."""
     import gsplat.cuda as _C
     from gsplat import _lib
     from gsplat._lib import check, ptr, stream
@@ -514,6 +541,12 @@ def fused_shading_phase(model: FlatGaussians, geo: Dict, scene: Dict, target: to
     cam_pos = cam[18:21]
     bg = scene["background"]
     lib = _lib.load()
+    if model.learnable_bg is not None:  # the blend's background is sigmoid(learnable_bg), computed on the device
+        from gsplat.background import background_forward_, background_vjp_
+        with _lib.on_device(dev):
+            bg = torch.empty(3, dtype=torch.float32, device=dev)
+            background_forward_(model.learnable_bg.detach(), bg)
+        geo["background"] = bg
     mode = _lib.render_mode(rasterize_mode, color_mode, "fused_shading_phase")
     if mode & _lib.COLOR_SIGMOID:
         sh_degree_to_use = 0  # sigmoid(sh_dc) reads no SH basis
@@ -555,6 +588,8 @@ def fused_shading_phase(model: FlatGaussians, geo: Dict, scene: Dict, target: to
         if g_vm is not None:  # the view-matrix gradient through the pose correction into the camera's pose row
             from gsplat.camera_opt import pose_backward_
             pose_backward_(geo["cam_in"], model.cam_pose.detach(), geo["cam_index"], g_vm, g["cam_pose"])
+        if model.learnable_bg is not None:
+            background_vjp_(v_rgb.contiguous(), Ts, bg, g["learnable_bg"])
     geo["absgrad"] = v_abs   # the `xys.absgrad` side channel of the drop-in operator (densification statistic)
     return loss.detach()
 
@@ -623,7 +658,8 @@ class PipelinedTrainer:
                  capacity: Optional[int] = None, sh_degree_to_use: int = 3, geometry_fn=None, shading_fn=None,
                  optimizer: str = "b200", sh_chunks: int = 1, operators: Optional[str] = None,
                  rasterize_mode: str = "antialiased", color_mode: str = "sh", num_downscales: int = 0,
-                 resolution_schedule: int = 3000, sh_degree_interval: int = 0, camera_l2=None):
+                 resolution_schedule: int = 3000, sh_degree_interval: int = 0, camera_l2=None,
+                 scale_regularization: bool = False, max_gauss_ratio: float = 10.0):
         """operators: "dropin" = the two phases on the reference-compatible operators under autograd (`geometry_phase` /
         `shading_phase`); "fused" = on the fused raw-parameter kernels (`fused_geometry_phase` / `fused_shading_phase`:
         same numbers, ~45 fewer launches per step); None = fused where it applies (CUDA, sh_layout "split"), else drop-in.
@@ -638,7 +674,14 @@ class PipelinedTrainer:
         gsplat.optim.splatfacto_pose_lr(); a dict needs the two POSE_GROUPS rates.
         camera_l2: None (default), "splatfacto" or a dict of weights trans / rot / linear / angular: Splatfacto's camera
         regularisers (camera_optimizers.py:189-195, :267-273) over all pose rows (trans / rot) and all velocity rows
-        (linear / angular) every step, added to the returned loss and to the rows' gradients."""
+        (linear / angular) every step, added to the returned loss and to the rows' gradients.
+        A learnable background (FlatGaussians(learnable_background=True), Splatfacto's background_color "auto"): phase B
+        blends over sigmoid(learnable_bg) and adds its gradient (gsplat.background); fused operators and RGB targets only.
+        lr="splatfacto" then includes gsplat.optim.splatfacto_background_lr(); a dict needs the "background_color" rate.
+        scale_regularization / max_gauss_ratio: Splatfacto's use_scale_regularization: at steps k with k % 10 == 0 (k =
+        `steps`, vetoed steps included, read on the device) 0.1 * mean(max(amax(e^s) / amin(e^s), max_gauss_ratio) -
+        max_gauss_ratio) over all Gaussians is added to the returned loss and its gradient to log_scales'.  Needs CUDA and
+        optimizer="b200"."""
         self.model, self.scene = model, dict(scene)
         if int(num_downscales) != num_downscales or not 0 <= num_downscales <= 4:
             raise ValueError("num_downscales must be an integer from 0 to 4 (factors up to 16)")
@@ -678,6 +721,14 @@ class PipelinedTrainer:
         self.camera_l2 = camera_l2_weights(camera_l2)
         if self.camera_l2 is not None and model.flat.device.type != "cuda":
             raise ValueError("camera_l2 needs a CUDA model (b200_camera_l2)")
+        self.learnable_bg = getattr(model, "learnable_bg", None) is not None
+        if self.learnable_bg and operators == "dropin":
+            raise ValueError("a learnable background needs operators='fused' (on the drop-in path Splatfacto's own "
+                             "learnable_bg gets its gradient through rasterize_gaussians)")
+        self.scale_regularization, self.max_gauss_ratio = bool(scale_regularization), float(max_gauss_ratio)
+        if self.scale_regularization and (model.flat.device.type != "cuda" or optimizer != "b200"):
+            raise ValueError("scale_regularization needs a CUDA model and optimizer='b200' (it reads the device step "
+                             "count of the Adam state)")
         self.operators = operators
         phases = (fused_geometry_phase, fused_shading_phase) if operators == "fused" else (geometry_phase, shading_phase)
         modes = dict(rasterize_mode=rasterize_mode, color_mode=color_mode)
@@ -721,10 +772,12 @@ class PipelinedTrainer:
         if isinstance(lr, str):
             if lr != "splatfacto":
                 raise ValueError(f"lr must be a float, a dict of per-group rates or 'splatfacto', got {lr!r}")
-            from gsplat.optim import splatfacto_lr, splatfacto_pose_lr
+            from gsplat.optim import splatfacto_background_lr, splatfacto_lr, splatfacto_pose_lr
             lr = splatfacto_lr()
             if getattr(model, "cam_pose", None) is not None:
                 lr.update(splatfacto_pose_lr())
+            if self.learnable_bg:
+                lr.update(splatfacto_background_lr())
         self.lr_groups = dict(lr) if isinstance(lr, dict) else None
         if self.lr_groups is not None and optimizer != "b200":
             raise ValueError("per-group learning rates need optimizer='b200' (the grouped device-state Adam)")
@@ -891,12 +944,14 @@ class PipelinedTrainer:
                 tgt = self._as_target(e["target"])
                 self.loss.copy_(self.shading_fn(self.model, e["geo"], self.scene, tgt, self.loss_fn, self.sh_degree))
                 self._camera_regularisers()
+                self._scale_regulariser()
             e["gB"], e["nB"] = g, self._lib_launches() - n0
             g.replay()
             return
         tgt = self._as_target(target)
         self.loss.copy_(self.shading_fn(self.model, self._geo, self.scene, tgt, self.loss_fn, self.sh_degree))
         self._camera_regularisers()
+        self._scale_regulariser()
         e["warm"] += 1
 
     def _camera_regularisers(self):
@@ -910,6 +965,17 @@ class PipelinedTrainer:
             for rows, a, b_ in ((m.cam_pose, w["trans"], w["rot"]), (m.cam_vel, w["linear"], w["angular"])):
                 if rows is not None:
                     camera_l2_(rows.detach(), a, b_, rows.grad, self.loss)
+
+    def _scale_regulariser(self):
+        """scale_regularization: at the steps the device clock selects, the regulariser's value added to the step's loss
+        and its gradient to the log_scales gradient."""
+        if not self.scale_regularization:
+            return
+        from gsplat import _lib
+        from gsplat.background import scale_regularizer_
+        p = self.model.params["log_scales"]
+        with _lib.on_device(self.device):
+            scale_regularizer_(p.detach(), self.adam.state, p.grad, self.loss, max_ratio=self.max_gauss_ratio)
 
     def _as_target(self, target):
         """The dataset's uint8 image goes to the loss as it is when the loss converts it in its own kernel
@@ -983,6 +1049,10 @@ class PipelinedTrainer:
         """Trains on the prepared image (B, exchange, update) and, given `next_cam`, runs A for the next image while the
         SH block is still being exchanged / updated.  Returns the device loss (a static tensor: copy it if you keep it)."""
         assert getattr(self, "_prepared", False), "call prepare(cam, cam_index) before the first train_step"
+        if self.learnable_bg and target.shape[-1] == 4:
+            # an RGBA target composited over the learned colour would give that colour a second gradient, through the
+            # target (composite_with_background, splatfacto.py:912-923), which this trainer does not compute
+            raise ValueError("a learnable background needs RGB targets: RGBA targets are composited over the background")
         with self._OnMain(self):
             return self._train_step(target, next_cam, next_index)
 

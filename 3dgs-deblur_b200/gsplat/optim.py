@@ -109,18 +109,31 @@ def splatfacto_pose_lr():
     )
 
 
+# The learned background logit (3,) of a model built with learnable_background: nerfstudio's background_color group.  Its
+# group index follows the pose groups.
+BACKGROUND_GROUP = "background_color"
+
+
+def splatfacto_background_lr():
+    """Splatfacto's background-colour rate (method_configs.py:658-661: constant 5e-3, eps 1e-15, no scheduler)."""
+    return dict(background_color=5e-3)
+
+
 def group_segments(model, lr):
-    """The group table and the segment table of a gsplat.dp.FlatGaussians for the rates `lr` (a dict keyed by GROUPS and
-    POSE_GROUPS names: float = constant rate, or an ExponentialDecay) -> (names, schedules, segments).  `names` /
-    `schedules` are the groups the model has, in GROUPS then POSE_GROUPS order (group index = position); `segments` are
+    """The group table and the segment table of a gsplat.dp.FlatGaussians for the rates `lr` (a dict keyed by GROUPS,
+    POSE_GROUPS and BACKGROUND_GROUP names: float = constant rate, or an ExponentialDecay) -> (names, schedules, segments).
+    `names` / `schedules` are the groups the model has, in GROUPS, POSE_GROUPS, BACKGROUND_GROUP order (group index =
+    position); `segments` are
     (begin, end, period, split, group_a, group_b) rows over global flat indices, sorted.  Split SH layout: one segment per
     field; block layout: one periodic segment over the (N, K, 3) block, the first 3 floats of each row sh_dc.  The velocity
-    rows and the pose rows are one periodic segment each (period 6, split 3).  The alignment pad belongs to no group.
-    ValueError for an unknown name and for a group the model has without a rate; velocity or pose rates for a model
-    without those rows are ignored, as nerfstudio ignores configured groups that have no parameters."""
-    unknown = sorted(set(lr) - set(GROUPS) - set(POSE_GROUPS))
+    rows and the pose rows are one periodic segment each (period 6, split 3), the background logit one plain segment.  The
+    alignment pad belongs to no group.  ValueError for an unknown name and for a group the model has without a rate;
+    velocity, pose or background rates for a model without those rows are ignored, as nerfstudio ignores configured groups
+    that have no parameters."""
+    known = GROUPS + POSE_GROUPS + (BACKGROUND_GROUP,)
+    unknown = sorted(set(lr) - set(known))
     if unknown:
-        raise ValueError(f"group_segments: unknown parameter group(s) {unknown}; known: {list(GROUPS + POSE_GROUPS)}")
+        raise ValueError(f"group_segments: unknown parameter group(s) {unknown}; known: {list(known)}")
     sl = model.slices
     present = [n for n in GROUPS[:4] if sl[n][1] > sl[n][0]]
     if model.sh_layout == "block":
@@ -132,6 +145,9 @@ def group_segments(model, lr):
     cam_pose = getattr(model, "cam_pose", None)
     if cam_pose is not None:
         present += list(POSE_GROUPS)
+    learnable_bg = getattr(model, "learnable_bg", None)
+    if learnable_bg is not None:
+        present.append(BACKGROUND_GROUP)
     missing = [n for n in present if n not in lr]
     if missing:
         raise ValueError(f"group_segments: no learning rate for the model's group(s) {missing}")
@@ -145,6 +161,9 @@ def group_segments(model, lr):
     if cam_pose is not None:
         a, b = sl["cam_pose"]
         segs.append((a, b, 6, 3, idx["cam_pose_trans"], idx["cam_pose_rot"]))
+    if learnable_bg is not None:
+        a, b = sl["learnable_bg"]
+        segs.append((a, b, 0, 0, idx[BACKGROUND_GROUP], idx[BACKGROUND_GROUP]))
     if model.sh_layout == "block":
         a, b = sl["sh"]
         g_dc = idx["sh_dc"]

@@ -818,6 +818,31 @@ B200_API int b200_camera_pose_backward(int num_views, int num_cameras, const flo
 B200_API int b200_camera_l2(int num_rows, const float *rows, float w_a, float w_b, float *g_rows, float *value,
                             void *stream);
 
+/* ---- learnable background and scale regulariser (Splatfacto's background_color "auto", use_scale_regularization) -------
+ * Nothing is read from the host, so all three may be captured in a CUDA graph.  b200_background_vjp and
+ * b200_scale_regularizer reduce in a fixed order (per-thread, warp, block, then the block partials in block order by the
+ * last block to finish) and are bit-reproducible from call to call, in deterministic mode or not.  ws: DEVICE,
+ * b200_bg_scale_ws_bytes() bytes, 16-byte aligned; its first word is a ticket each call leaves at zero, so a caller that
+ * zeroed the workspace once passes ws_is_zeroed = 1 (0 = cleared here first).  One workspace serves calls queued one after
+ * another on one stream.
+ *   b200_background_forward: background[c] = 1 / (1 + exp(-logit[c])) for c < 3 (splatfacto.py:706-707), the colour the
+ *       blend kernels then read as `background`.
+ *   b200_background_vjp: g_logit[c] = (v_b[c] * (1 - background[c])) * background[c] with v_b[c] = sum_px v_rgb[px][c] *
+ *       (sum_s final_Ts[px][s]) * (1 / n_samples), the reference's v_background (gsplat/rasterize.py:266-270) through the
+ *       sigmoid; v_rgb (num_pixels, 3), final_Ts (num_pixels, n_samples).  g_logit (3 floats) is OVERWRITTEN.
+ *   b200_scale_regularizer: when word [4] of adam_state (the b200_adam_prepare state: steps prepared so far, the index of
+ *       the step whose loss this is) is a multiple of `every`, value[0] += weight * mean_i(max(r_i, max_ratio) - max_ratio)
+ *       with r_i = amax_j(exp(log_scales[i][j])) / amin_j(exp(log_scales[i][j])) (splatfacto.py:968-977), and its
+ *       gradient, torch's (ties split evenly, half the gradient at r_i == max_ratio), ADDED into g_log_scales
+ *       (num_points, 3); otherwise nothing is touched.  One thread per Gaussian row, no atomics. */
+B200_API size_t b200_bg_scale_ws_bytes(void);
+B200_API int b200_background_forward(const float *logit, float *background, void *stream);
+B200_API int b200_background_vjp(long long num_pixels, int n_samples, const float *v_rgb, const float *final_Ts,
+                                 const float *background, float *g_logit, void *ws, int ws_is_zeroed, void *stream);
+B200_API int b200_scale_regularizer(int num_points, const float *log_scales, float max_ratio, float weight, int every,
+                                    const void *adam_state, float *g_log_scales, float *value, void *ws, int ws_is_zeroed,
+                                    void *stream);
+
 #ifdef __cplusplus
 }
 #endif
