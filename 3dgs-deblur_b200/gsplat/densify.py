@@ -143,8 +143,7 @@ class Densifier:
             if n_splits:
                 z = (normal_samples or (lambda k: torch.randn((k, 3), device=dev)))(samps * n_splits).to(dev).float().contiguous()
             old = {k: v.detach() for k, v in p.items()}
-            old_cam = {k: getattr(m, k).detach().clone() for k in ("cam_vel", "cam_pose", "learnable_bg")
-                       if getattr(m, k, None) is not None}
+            old_rows = {k: getattr(m, k).detach().clone() for k in m.row_fields}
             old_slices = dict(m.slices)
             old_flat = m.flat
             old_avg = old_sq = None
@@ -153,8 +152,7 @@ class Densifier:
             m._reallocate(new_n)  # new flat / flat_grad buffers + parameter views (same field order and layout rules)
             if self.adam is not None:
                 self.adam.rebind(m.flat, m.flat_grad)
-            fields = [k for k in old if k in m.params]
-            for name in fields:
+            for name in old:
                 width = old[name][0].numel()
                 field = {"means": 1 if z is not None else 0, "log_scales": 2}.get(name, 0)  # (no split, no re-sampled child)
                 check(lib.b200_densify_gather(n, samps, field, width, ptr(old[name]), ptr(m.params[name]), ptr(ws), ptr(counts),
@@ -165,7 +163,7 @@ class Densifier:
                     for src_buf, dst_buf in ((old_avg, self.adam.exp_avg), (old_sq, self.adam.exp_avg_sq)):
                         check(lib.b200_densify_gather(n, samps, 3, width, src_buf.data_ptr() + 4 * a0, dst_buf.data_ptr() + 4 * a1,
                                                       ptr(ws), ptr(counts), None, None, None, stream()))
-            for name, rows in old_cam.items():  # camera rows and the background logit: carried over with their moments
+            for name, rows in old_rows.items():  # the fixed-count rows: carried over with their moments
                 getattr(m, name).data.copy_(rows)
                 if self.adam is not None:
                     a0, b0 = old_slices[name]

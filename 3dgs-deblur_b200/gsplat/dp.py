@@ -26,13 +26,31 @@ from typing import Dict, List, Optional
 import torch
 import torch.distributed as dist
 
-# flat layout: the geometry/opacity rows (11 floats per Gaussian) and the per-camera rows first, the SH coefficients
-# (48 of the 59 floats at K = 16) last, so "everything but SH" and "SH" are each ONE contiguous slice to exchange
-FIELDS = ("means", "log_scales", "quats", "opacity_logit", "sh_dc", "sh_rest")
+# The flat layout: every field a model can have, in buffer order, as (name, shape, learning-rate group(s)).  Shapes count
+# N Gaussians, C training cameras and K SH coefficients per colour channel.  A field whose rows are the N Gaussians is a
+# parameter in FlatGaussians.params; every other one is a fixed-count row, the attribute of that name (None for a model
+# without it).  The group (gsplat.optim) is one name for every element, or (group_a, split, group_b): the first `split`
+# floats of each row in group_a, the rest in group_b.  A model has sh_dc and sh_rest (split SH layout) or sh (block), and
+# the velocity, pose and background rows it was built with.  The geometry/opacity rows (11 floats per Gaussian) and the
+# fixed-count rows come first, the SH coefficients (48 of the 59 floats at K = 16) last, so "everything but SH" and "SH"
+# are each ONE contiguous slice to exchange.
+FIELDS = (
+    ("means", ("N", 3), "means"),
+    ("log_scales", ("N", 3), "log_scales"),
+    ("quats", ("N", 4), "quats"),
+    ("opacity_logit", ("N", 1), "opacity_logit"),
+    ("cam_vel", ("C", 6), ("cam_vel_linear", 3, "cam_vel_angular")),
+    ("cam_pose", ("C", 6), ("cam_pose_trans", 3, "cam_pose_rot")),
+    ("learnable_bg", (3,), "background_color"),
+    ("sh_dc", ("N", 1, 3), "sh_dc"),
+    ("sh_rest", ("N", "K-1", 3), "sh_rest"),
+    ("sh", ("N", "K", 3), ("sh_dc", 3, "sh_rest")),
+)
 
 
 class FlatGaussians:
-    """Gaussian parameters as views into one flat buffer (+ a flat gradient buffer of the same layout)."""
+    """Gaussian parameters as views into one flat buffer (+ a flat gradient buffer of the same layout).  `fields`: the
+    model's FIELDS entries in flat order, with its shapes; `row_fields`: the names of its fixed-count rows."""
 
     def __init__(self, scene: Dict, device, n_cameras: int = 0, optimize_velocities: bool = False, sh_layout: str = "split",
                  optimize_poses: bool = False, learnable_background: bool = False):
@@ -48,54 +66,52 @@ class FlatGaussians:
             raise ValueError("sh_layout must be 'split' or 'block'")
         if optimize_poses and n_cameras < 1:
             raise ValueError("optimize_poses needs n_cameras >= 1")
-        N = scene["means"].shape[0]
-        K = scene["sh_rest"].shape[1] + 1
-        self.N, self.K, self.sh_layout = N, K, sh_layout
-        self._n_vel = n_cameras if optimize_velocities else 0
-        self._n_pose = n_cameras if optimize_poses else 0
-        self._n_bg = 3 if learnable_background else 0
-        widths = dict(means=3, log_scales=3, quats=4, opacity_logit=1, sh_dc=3, sh_rest=3 * (K - 1))
-        shapes = dict(means=(N, 3), log_scales=(N, 3), quats=(N, 4), opacity_logit=(N, 1), sh_dc=(N, 1, 3),
-                      sh_rest=(N, K - 1, 3))
-        extra = 6 * (self._n_vel + self._n_pose) + self._n_bg
-        # pad the camera rows so the SH coefficients start on a 16-byte boundary (the slice-wise device-state Adam and
-        # the SH kernels' vector accesses want that)
-        pad = (-(N * 11 + extra)) % 4
-        total = N * sum(widths.values()) + extra + pad
-        self.flat = torch.zeros(total, dtype=torch.float32, device=device)
-        self.flat_grad = torch.zeros_like(self.flat)
-        self.params: Dict[str, torch.Tensor] = {}
-        self.slices: Dict[str, tuple] = {}
-        self.cam_vel: Optional[torch.Tensor] = None
-        self.cam_pose: Optional[torch.Tensor] = None
-        self.learnable_bg: Optional[torch.Tensor] = None
+        self.K, self.sh_layout, self._n_cameras = scene["sh_rest"].shape[1] + 1, sh_layout, n_cameras
+        has = dict(cam_vel=optimize_velocities and n_cameras > 0, cam_pose=optimize_poses, learnable_bg=learnable_background,
+                   sh_dc=sh_layout == "split", sh_rest=sh_layout == "split", sh=sh_layout == "block")
+        self._table = [f for f in FIELDS if has.get(f[0], True)]
+        self.row_fields = [name for name, shape, _ in self._table if shape[0] != "N"]  # in flat order
+        for name, shape, _ in FIELDS:  # the fixed-count rows the model lacks stay None
+            if shape[0] != "N":
+                setattr(self, name, None)
+        self._bind(scene["means"].shape[0], device)
+        for name, p in self.params.items():  # the scene's values, written through flat
+            dst = self.flat[slice(*self.slices[name])].view(p.shape)
+            parts = [("sh_dc", dst[:, :1]), ("sh_rest", dst[:, 1:])] if name == "sh" else [(name, dst)]
+            for key, part in parts:
+                part.copy_(scene[key].to(device).reshape(part.shape))
 
-        def take(name, off, numel, shape):
-            view = self.flat[off:off + numel].view(shape)
-            p = view.requires_grad_(True)
-            p.grad = self.flat_grad[off:off + numel].view(shape)
-            self.slices[name] = (off, off + numel)
-            return p
-
+    def _bind(self, n: int, device):
+        """Zeroed flat / flat_grad buffers for `n` Gaussians, and every field of the model a leaf over its slice of `flat`
+        with the same slice of `flat_grad` as .grad; sets N, fields (the model's FIELDS entries with its shapes), slices,
+        params, the fixed-count rows, sh_start and floats_per_gaussian."""
+        dims = {"N": n, "C": self._n_cameras, "K": self.K, "K-1": self.K - 1}
+        self.fields = [(name, tuple(dims.get(d, d) for d in shape), groups) for name, shape, groups in self._table]
+        self.N, self.slices, self.params = n, {}, {}
         off = 0
-        for name in FIELDS:
-            if name == "sh_dc":  # camera rows (+ alignment padding) sit between the geometry block and the SH block
-                off = self._take_camera_rows(take, off)
-                off += pad
-                if sh_layout == "block":
-                    blk = self.flat[off:off + N * 3 * K].view(N, K, 3)
-                    blk[:, :1].copy_(scene["sh_dc"].to(device).reshape(N, 1, 3))
-                    blk[:, 1:].copy_(scene["sh_rest"].to(device).reshape(N, K - 1, 3))
-                    self.params["sh"] = take("sh", off, N * 3 * K, (N, K, 3))
-                    self.slices["sh_dc"] = self.slices["sh_rest"] = self.slices["sh"]
-                    off += N * 3 * K
-                    break
-            self.flat[off:off + N * widths[name]].view(shapes[name]).copy_(scene[name].to(device).reshape(shapes[name]))
-            self.params[name] = take(name, off, N * widths[name], shapes[name])
-            off += N * widths[name]
-        assert off == total
-        self.sh_start = self.slices["sh_dc"][0]  # flat[sh_start:] = all SH coefficients
-        self.floats_per_gaussian = sum(widths.values())
+        for name, shape, _ in self.fields:
+            # flat[sh_start:] = all SH coefficients, from a 16-byte boundary (the slice-wise device-state Adam and the SH
+            # kernels' vector accesses want that)
+            if name in ("sh_dc", "sh"):
+                off = self.sh_start = off + -off % 4
+            self.slices[name] = (off, off + math.prod(shape))
+            off += math.prod(shape)
+        if self.sh_layout == "block":
+            self.slices["sh_dc"] = self.slices["sh_rest"] = self.slices["sh"]
+        self.flat = torch.zeros(off, dtype=torch.float32, device=device)
+        self.flat_grad = torch.zeros_like(self.flat)
+        for name, shape, _ in self.fields:
+            a, b = self.slices[name]
+            self._set_leaf(name, self.flat[a:b].view(shape), self.flat_grad[a:b].view(shape))
+        self.floats_per_gaussian = sum(math.prod(shape[1:]) for name, shape, _ in self.fields if name in self.params)
+
+    def _set_leaf(self, name, leaf, grad):
+        leaf.requires_grad_(True)
+        leaf.grad = grad
+        if name in self.row_fields:
+            setattr(self, name, leaf)
+        else:
+            self.params[name] = leaf
 
     @property
     def views(self) -> Dict[str, torch.Tensor]:
@@ -103,79 +119,19 @@ class FlatGaussians:
         sh = self.params["sh"].detach()
         return {"sh_dc": sh[:, :1], "sh_rest": sh[:, 1:]}
 
-    def _take_camera_rows(self, take, off):
-        """The velocity rows, the pose rows, then the background logit, from flat offset `off`; returns the offset after
-        them."""
-        if self._n_vel:
-            self.cam_vel = take("cam_vel", off, 6 * self._n_vel, (self._n_vel, 6))
-            off += 6 * self._n_vel
-        if self._n_pose:
-            self.cam_pose = take("cam_pose", off, 6 * self._n_pose, (self._n_pose, 6))
-            off += 6 * self._n_pose
-        if self._n_bg:
-            self.learnable_bg = take("learnable_bg", off, 3, (3,))
-            off += 3
-        return off
-
     def rebind_leaves(self):
         """Replace every parameter by a fresh leaf tensor over the same storage (same .grad views).  Autograd ties a
         leaf's gradient accumulator to the stream that is current when the accumulator is first created; a trainer that
         captures its backward pass into a CUDA graph on its own stream calls this (on that stream) so that no accumulator
         made earlier on the legacy default stream forces the capture to synchronise with it."""
-        for name in list(self.params):
-            old = self.params[name]
-            new = old.detach().requires_grad_(True)
-            new.grad = old.grad
-            self.params[name] = new
-        if self.cam_vel is not None:
-            new = self.cam_vel.detach().requires_grad_(True)
-            new.grad = self.cam_vel.grad
-            self.cam_vel = new
-        if self.cam_pose is not None:
-            new = self.cam_pose.detach().requires_grad_(True)
-            new.grad = self.cam_pose.grad
-            self.cam_pose = new
-        if self.learnable_bg is not None:
-            new = self.learnable_bg.detach().requires_grad_(True)
-            new.grad = self.learnable_bg.grad
-            self.learnable_bg = new
+        for name, old in zip(list(self.params) + self.row_fields, self.parameters()):
+            self._set_leaf(name, old.detach(), old.grad)
 
     def _reallocate(self, new_n: int):
-        """New flat / gradient buffers for `new_n` Gaussians with the same field order, camera rows and layout rules; the
-        parameter views are rebuilt (contents uninitialised: gsplat.densify.Densifier fills them).  Anything that cached
-        pointers into the old buffers (optimizer, captured graphs) must be rebound by the caller."""
-        K, dev = self.K, self.flat.device
-        extra = 6 * (self._n_vel + self._n_pose) + self._n_bg
-        pad = (-(new_n * 11 + extra)) % 4
-        widths = dict(means=3, log_scales=3, quats=4, opacity_logit=1, sh_dc=3, sh_rest=3 * (K - 1))
-        shapes = dict(means=(new_n, 3), log_scales=(new_n, 3), quats=(new_n, 4), opacity_logit=(new_n, 1), sh_dc=(new_n, 1, 3),
-                      sh_rest=(new_n, K - 1, 3))
-        total = new_n * sum(widths.values()) + extra + pad
-        self.flat = torch.zeros(total, dtype=torch.float32, device=dev)
-        self.flat_grad = torch.zeros_like(self.flat)
-        self.params, self.slices, self.cam_vel, self.cam_pose, self.learnable_bg = {}, {}, None, None, None
-        self.N = new_n
-
-        def take(name, off, numel, shape):
-            pr = self.flat[off:off + numel].view(shape).requires_grad_(True)
-            pr.grad = self.flat_grad[off:off + numel].view(shape)
-            self.slices[name] = (off, off + numel)
-            return pr
-
-        off = 0
-        for name in FIELDS:
-            if name == "sh_dc":
-                off = self._take_camera_rows(take, off)
-                off += pad
-                if self.sh_layout == "block":
-                    self.params["sh"] = take("sh", off, new_n * 3 * K, (new_n, K, 3))
-                    self.slices["sh_dc"] = self.slices["sh_rest"] = self.slices["sh"]
-                    off += new_n * 3 * K
-                    break
-            self.params[name] = take(name, off, new_n * widths[name], shapes[name])
-            off += new_n * widths[name]
-        assert off == total
-        self.sh_start = self.slices["sh_dc"][0]
+        """New flat / gradient buffers for `new_n` Gaussians with the same fields; the parameter views are rebuilt
+        (contents uninitialised: gsplat.densify.Densifier fills them).  Anything that cached pointers into the old buffers
+        (optimizer, captured graphs) must be rebound by the caller."""
+        self._bind(new_n, self.flat.device)
 
     def sh_coeffs(self) -> torch.Tensor:
         """(N, K, 3) coefficients as spherical_harmonics wants them."""
@@ -184,14 +140,8 @@ class FlatGaussians:
         return torch.cat((self.params["sh_dc"], self.params["sh_rest"]), dim=1)  # splatfacto.py:840-842
 
     def parameters(self) -> List[torch.Tensor]:
-        ps = list(self.params.values())
-        if self.cam_vel is not None:
-            ps.append(self.cam_vel)
-        if self.cam_pose is not None:
-            ps.append(self.cam_pose)
-        if self.learnable_bg is not None:
-            ps.append(self.learnable_bg)
-        return ps
+        """The per-Gaussian parameters, then the fixed-count rows."""
+        return list(self.params.values()) + [getattr(self, name) for name in self.row_fields]
 
     def zero_grad(self):
         self.flat_grad.zero_()
@@ -764,20 +714,13 @@ class PipelinedTrainer:
         self.sh_update_ctas = int(os.environ.get("B200_SH_UPDATE_CTAS", "0"))
         self.sh_update_pieces = int(os.environ.get("B200_SH_UPDATE_PIECES", "8"))
         # the SH block is exchanged in `sh_chunks` pieces so that the update of piece i runs while piece i+1 is on the wire
-        lo, total = model.sh_start, model.flat.numel()
-        n_sh = max(1, int(sh_chunks)) if self.distributed else 1
-        cuts = [lo + ((total - lo) * k // n_sh) // 4 * 4 for k in range(n_sh)] + [total]
-        self._sh_bounds = [(cuts[k], cuts[k + 1]) for k in range(n_sh) if cuts[k + 1] > cuts[k]]
+        self._cut_sh(max(1, int(sh_chunks)) if self.distributed else 1)
         # per-group rates: None = one rate for the whole buffer (the float path, unchanged)
         if isinstance(lr, str):
             if lr != "splatfacto":
                 raise ValueError(f"lr must be a float, a dict of per-group rates or 'splatfacto', got {lr!r}")
             from gsplat.optim import splatfacto_background_lr, splatfacto_lr, splatfacto_pose_lr
-            lr = splatfacto_lr()
-            if getattr(model, "cam_pose", None) is not None:
-                lr.update(splatfacto_pose_lr())
-            if self.learnable_bg:
-                lr.update(splatfacto_background_lr())
+            lr = {**splatfacto_lr(), **splatfacto_pose_lr(), **splatfacto_background_lr()}  # rows the model lacks: ignored
         self.lr_groups = dict(lr) if isinstance(lr, dict) else None
         if self.lr_groups is not None and optimizer != "b200":
             raise ValueError("per-group learning rates need optimizer='b200' (the grouped device-state Adam)")
@@ -1139,6 +1082,12 @@ class PipelinedTrainer:
             self._torch_opts[which].step()
         g.zero_()
 
+    def _cut_sh(self, pieces: int):
+        """`_sh_bounds`: the SH block as `pieces` exchange slices cut on 16-byte boundaries, empty pieces dropped."""
+        lo, total = self.model.sh_start, self.model.flat.numel()
+        cuts = [lo + ((total - lo) * k // pieces) // 4 * 4 for k in range(pieces)] + [total]
+        self._sh_bounds = [(cuts[k], cuts[k + 1]) for k in range(pieces) if cuts[k + 1] > cuts[k]]
+
     def on_resize(self):
         """The model's buffers were reallocated (gsplat.densify.Densifier.refine): drop the captured graphs (they address
         the old buffers), recompute the exchange slices and the per-group segment table, put the new leaves on this
@@ -1149,10 +1098,7 @@ class PipelinedTrainer:
         self._geo = None
         self._prepared = False
         m = self.model
-        lo, total = m.sh_start, m.flat.numel()
-        n_sh = len(self._sh_bounds)
-        cuts = [lo + ((total - lo) * k // n_sh) // 4 * 4 for k in range(n_sh)] + [total]
-        self._sh_bounds = [(cuts[k], cuts[k + 1]) for k in range(n_sh) if cuts[k + 1] > cuts[k]]
+        self._cut_sh(len(self._sh_bounds))
         if self.lr_groups is not None and self.adam is not None:  # every group boundary moved with N
             from gsplat.optim import group_segments
             self.adam.set_groups(group_segments(m, self.lr_groups)[2])

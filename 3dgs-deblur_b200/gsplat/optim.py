@@ -124,55 +124,34 @@ def group_segments(model, lr):
     POSE_GROUPS and BACKGROUND_GROUP names: float = constant rate, or an ExponentialDecay) -> (names, schedules, segments).
     `names` / `schedules` are the groups the model has, in GROUPS, POSE_GROUPS, BACKGROUND_GROUP order (group index =
     position); `segments` are
-    (begin, end, period, split, group_a, group_b) rows over global flat indices, sorted.  Split SH layout: one segment per
-    field; block layout: one periodic segment over the (N, K, 3) block, the first 3 floats of each row sh_dc.  The velocity
-    rows and the pose rows are one periodic segment each (period 6, split 3), the background logit one plain segment.  The
-    alignment pad belongs to no group.  ValueError for an unknown name and for a group the model has without a rate;
-    velocity, pose or background rates for a model without those rows are ignored, as nerfstudio ignores configured groups
-    that have no parameters."""
+    (begin, end, period, split, group_a, group_b) rows over global flat indices, sorted: one per non-empty field of the
+    model (gsplat.dp.FIELDS), plain for a field of one group, periodic (period = the row's width) for a field whose rows
+    split into two groups -- the velocity and pose rows, and the block layout's (N, K, 3) SH block, the first 3 floats of
+    each row sh_dc.  The alignment pad belongs to no group.  ValueError for an unknown name and for a group the model has
+    without a rate; velocity, pose or background rates for a model without those rows are ignored, as nerfstudio ignores
+    configured groups that have no parameters."""
     known = GROUPS + POSE_GROUPS + (BACKGROUND_GROUP,)
     unknown = sorted(set(lr) - set(known))
     if unknown:
         raise ValueError(f"group_segments: unknown parameter group(s) {unknown}; known: {list(known)}")
-    sl = model.slices
-    present = [n for n in GROUPS[:4] if sl[n][1] > sl[n][0]]
-    if model.sh_layout == "block":
-        present += ["sh_dc"] + (["sh_rest"] if model.K > 1 else [])
-    else:
-        present += [n for n in ("sh_dc", "sh_rest") if sl[n][1] > sl[n][0]]
-    if model.cam_vel is not None:
-        present += ["cam_vel_linear", "cam_vel_angular"]
-    cam_pose = getattr(model, "cam_pose", None)
-    if cam_pose is not None:
-        present += list(POSE_GROUPS)
-    learnable_bg = getattr(model, "learnable_bg", None)
-    if learnable_bg is not None:
-        present.append(BACKGROUND_GROUP)
+    rows = []  # (begin, end, period, split, group_a, group_b) of every non-empty field, groups by name
+    for name, shape, groups in model.fields:
+        a, b = model.slices[name]
+        if b == a:  # sh_rest at K = 1
+            continue
+        if isinstance(groups, str):
+            rows.append((a, b, 0, 0, groups, groups))
+        else:  # a row no wider than the split (the block's at K = 1) is all group_a
+            g_a, split, g_b = groups
+            period = math.prod(shape[1:])
+            rows.append((a, b, period, split, g_a, g_b if period > split else g_a))
+    owned = {g for row in rows for g in row[4:]}
+    present = [n for n in known if n in owned]
     missing = [n for n in present if n not in lr]
     if missing:
         raise ValueError(f"group_segments: no learning rate for the model's group(s) {missing}")
     idx = {n: i for i, n in enumerate(present)}
-    segs = []
-    for n in present[:4]:
-        segs.append((sl[n][0], sl[n][1], 0, 0, idx[n], idx[n]))
-    if model.cam_vel is not None:
-        a, b = sl["cam_vel"]
-        segs.append((a, b, 6, 3, idx["cam_vel_linear"], idx["cam_vel_angular"]))
-    if cam_pose is not None:
-        a, b = sl["cam_pose"]
-        segs.append((a, b, 6, 3, idx["cam_pose_trans"], idx["cam_pose_rot"]))
-    if learnable_bg is not None:
-        a, b = sl["learnable_bg"]
-        segs.append((a, b, 0, 0, idx[BACKGROUND_GROUP], idx[BACKGROUND_GROUP]))
-    if model.sh_layout == "block":
-        a, b = sl["sh"]
-        g_dc = idx["sh_dc"]
-        segs.append((a, b, 3 * model.K, 3, g_dc, idx.get("sh_rest", g_dc)))
-    else:
-        for n in ("sh_dc", "sh_rest"):
-            if n in idx:
-                segs.append((sl[n][0], sl[n][1], 0, 0, idx[n], idx[n]))
-    segs.sort()
+    segs = sorted((a, b, period, split, idx[g_a], idx[g_b]) for a, b, period, split, g_a, g_b in rows)
     return present, [lr[n] for n in present], segs
 
 

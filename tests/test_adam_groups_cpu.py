@@ -3,9 +3,10 @@
 - gsplat.optim's restated schedules (and tests/adam_groups_f64.py's) equal the reference's LambdaLR values, and
   float64 grouped Adam follows the reference's per-group torch Adam, both from tests/golden/lr_schedule.npz
   (tests/golden/make_golden_lr.py: nerfstudio's own Optimizers, ExponentialDecayScheduler and train_iteration order).
-- group_segments maps every flat index to its group, for both SH layouts, with and without camera rows, odd N, and
-  after a reallocation; its argument errors.
+- group_segments maps every flat index to its group, for both SH layouts, K = 4 and K = 1, with and without velocity,
+  pose and background rows, odd N, and after a reallocation; its argument errors.
 - PipelinedTrainer's SH degree for each image, on stand-in phases."""
+import itertools
 import os
 
 import numpy as np
@@ -84,14 +85,15 @@ def test_grouped_f64_adam_follows_the_reference(gold):
 
 # ---- group_segments -------------------------------------------------------------------------------------------------
 
-def _model(n, n_cameras, layout, K=4):
+def _model(n, n_cameras, layout, K=4, poses=False, bg=False):
     from gsplat import dp
 
     g = torch.Generator().manual_seed(n)
     scene = dict(means=torch.randn(n, 3, generator=g), log_scales=torch.randn(n, 3, generator=g),
                  quats=torch.randn(n, 4, generator=g), opacity_logit=torch.randn(n, 1, generator=g),
                  sh_dc=torch.randn(n, 1, 3, generator=g), sh_rest=torch.randn(n, K - 1, 3, generator=g))
-    return dp.FlatGaussians(scene, "cpu", n_cameras=n_cameras, optimize_velocities=n_cameras > 0, sh_layout=layout)
+    return dp.FlatGaussians(scene, "cpu", n_cameras=n_cameras, optimize_velocities=n_cameras > 0, sh_layout=layout,
+                            optimize_poses=poses, learnable_background=bg)
 
 
 def _expected_groups(model):
@@ -100,10 +102,14 @@ def _expected_groups(model):
     sl, N, K = model.slices, model.N, model.K
     for name in ("means", "log_scales", "quats", "opacity_logit"):
         out[sl[name][0]:sl[name][1]] = name
-    if model.cam_vel is not None:
-        a, b = sl["cam_vel"]
-        cols = np.arange(b - a) % 6
-        out[a:b] = np.where(cols < 3, "cam_vel_linear", "cam_vel_angular")
+    for row, first, rest in (("cam_vel", "cam_vel_linear", "cam_vel_angular"), ("cam_pose", "cam_pose_trans", "cam_pose_rot")):
+        if getattr(model, row) is not None:  # (n_cameras, 6): columns 0-2 one group, 3-5 the other
+            a, b = sl[row]
+            cols = np.arange(b - a) % 6
+            out[a:b] = np.where(cols < 3, first, rest)
+    if model.learnable_bg is not None:
+        a, b = sl["learnable_bg"]
+        out[a:b] = "background_color"
     if model.sh_layout == "block":
         a, b = sl["sh"]
         row = np.arange(b - a) % (3 * K)
@@ -118,23 +124,29 @@ def _expected_groups(model):
 @pytest.mark.parametrize("n_cameras", [0, 3])
 @pytest.mark.parametrize("n", [1, 7, 33])
 def test_group_segments_maps_every_index(layout, n_cameras, n):
-    from gsplat.optim import group_segments, splatfacto_lr
+    """Every SH size (K = 4 and K = 1) with the pose rows (where there are cameras) and the background row on and off."""
+    from gsplat.optim import (BACKGROUND_GROUP, GROUPS, POSE_GROUPS, group_segments, splatfacto_background_lr,
+                              splatfacto_lr, splatfacto_pose_lr)
 
-    model = _model(n, n_cameras, layout)
-    for m in (model, None):
-        if m is None:  # densification reallocates: every boundary moves
-            model._reallocate(2 * n + 3)
-            m = model
-        names, scheds, segs = group_segments(m, splatfacto_lr())
-        got = AG.group_of(segs, m.flat.numel())
-        want = _expected_groups(m)
-        named = np.array([None if g < 0 else names[g] for g in got], object)
-        assert (named == want).all()
-        pad = want == None  # noqa: E711
-        assert pad.sum() == (-(m.N * 11 + 6 * n_cameras)) % 4  # only the alignment pad is in no group
-        assert [s[0] for s in segs] == sorted(s[0] for s in segs) and len(segs) <= 16
-        if n_cameras == 0:
-            assert "cam_vel_linear" not in names  # configured velocity rates without rows are ignored
+    for K, poses, bg in itertools.product((4, 1), (False, True) if n_cameras else (False,), (False, True)):
+        lr = dict(splatfacto_lr(), **(splatfacto_pose_lr() if poses else {}), **(splatfacto_background_lr() if bg else {}))
+        model = _model(n, n_cameras, layout, K, poses, bg)
+        for m in (model, None):
+            if m is None:  # densification reallocates: every boundary moves
+                model._reallocate(2 * n + 3)
+                m = model
+            names, scheds, segs = group_segments(m, lr)
+            got = AG.group_of(segs, m.flat.numel())
+            want = _expected_groups(m)
+            named = np.array([None if g < 0 else names[g] for g in got], object)
+            assert (named == want).all(), (K, poses, bg)
+            assert names == [g for g in GROUPS + POSE_GROUPS + (BACKGROUND_GROUP,) if g in set(want)]
+            pad = want == None  # noqa: E711
+            # only the alignment pad is in no group
+            assert pad.sum() == (-(m.N * 11 + 6 * n_cameras * (1 + poses) + 3 * bg)) % 4, (K, poses, bg)
+            assert [s[0] for s in segs] == sorted(s[0] for s in segs) and len(segs) <= 16
+            if n_cameras == 0:
+                assert "cam_vel_linear" not in names  # configured velocity rates without rows are ignored
 
 
 def test_group_segments_argument_errors():
