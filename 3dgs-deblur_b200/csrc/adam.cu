@@ -176,6 +176,62 @@ __global__ void adam_prepare_groups_kernel(AdamState *st, int32_t *veto_flag, do
     }
 }
 
+// ---- per-group step counts and step masks -------------------------------------------------------------------------
+// nerfstudio steps an optimizer only when one of its parameters has a gradient (engine/optimizers.py:158-171), and
+// torch's Adam keeps a step count per parameter: on a step that gives some groups no gradient (Splatfacto's detached eval
+// cameras) those groups keep their parameters, moments and step counts.  The masked prepare keeps a step count per group
+// in the group table (B200_ADAM_GROUP_TABLE_FLOATS floats: lr_g / bc1(t_g), 1 / sqrt(bc2(t_g)), t_g, the step's mask) and
+// marks the state with skip = 2 so that the grouped update reads each group's own constants and the mask.
+constexpr int kTabBc2 = B200_ADAM_MAX_GROUPS, kTabSteps = 2 * B200_ADAM_MAX_GROUPS, kTabMask = 3 * B200_ADAM_MAX_GROUPS;
+constexpr int kSkipVeto = 1, kSkipPerGroup = 2;
+
+// Which groups step: all of them, or with a non-zero *detached only `keep` plus `cond_group` when the step index is a
+// multiple of cond_every (the scale regulariser's clock).  A vetoed step is handled as by adam_prepare_groups_kernel.
+__global__ void adam_prepare_groups_masked_kernel(AdamState *st, int32_t *veto_flag, const int32_t *detached,
+                                                  unsigned keep, int cond_group, int cond_every, double beta1,
+                                                  double beta2, LrTable tab, float *table) {
+    const int t = threadIdx.x;
+    const bool veto = veto_flag && *veto_flag != 0;
+    const bool det = detached && *detached != 0;
+    const int idx = st->seen, step = st->step + 1;
+    __syncthreads();  // every thread has read the state before thread 0 advances it
+    if (veto) {
+        if (t == 0) {
+            *veto_flag = 0;
+            st->seen = idx + 1;
+            st->skip = kSkipVeto;
+            st->ring[st->vetoed % 10] = idx;
+            st->vetoed += 1;
+        }
+        return;
+    }
+    const unsigned all = tab.n >= 32 ? ~0u : (1u << tab.n) - 1u;
+    unsigned mask = all;
+    if (det) {
+        mask = keep;
+        if (cond_group >= 0 && idx % cond_every == 0) mask |= 1u << cond_group;
+        mask &= all;
+    }
+    int32_t *steps = reinterpret_cast<int32_t *>(table + kTabSteps);
+    if (t < tab.n && ((mask >> t) & 1u)) {  // a masked group keeps its count and its constants
+        const int tg = steps[t] + 1;
+        steps[t] = tg;
+        const double bc1 = 1.0 - pow(beta1, (double)tg), bc2 = 1.0 - pow(beta2, (double)tg);
+        table[t] = (float)(scheduled_lr(tab.g[t], idx) / bc1);
+        table[kTabBc2 + t] = (float)(1.0 / sqrt(bc2));
+    }
+    if (t == 0) {
+        if (veto_flag) *veto_flag = 0;
+        reinterpret_cast<uint32_t *>(table)[kTabMask] = mask;
+        st->seen = idx + 1;
+        st->skip = kSkipPerGroup;
+        st->step = step;
+        const double bc1 = 1.0 - pow(beta1, (double)step), bc2 = 1.0 - pow(beta2, (double)step);
+        st->lr_over_bc1 = (float)(scheduled_lr(tab.g[0], idx) / bc1);
+        st->inv_sqrt_bc2 = (float)(1.0 / sqrt(bc2));
+    }
+}
+
 __device__ __forceinline__ int segment_of(const SegTable &T, long long e) {
     int j = -1;
     for (int k = 0; k < T.n; ++k)
@@ -196,14 +252,16 @@ __device__ __forceinline__ int group_at(const SegTable &T, long long e) {
     return (int)period_offset(S, e) < S.split ? S.ga : S.gb;
 }
 
-// one element of group gi (-1: in no segment -- parameter and moments stay, the gradient is still cleared)
+// one element of group gi (-1: in no segment, or a group outside `mask` -- parameter and moments stay, the gradient is
+// still cleared); per_group: the group's own 1 / sqrt(bc2) from the masked prepare's table
 __device__ __forceinline__ void adam_group_one(float &p, float &g, float &m, float &v, int gi, AdamArgs a,
-                                               const float *__restrict__ group_lr) {
-    if (gi < 0) {
+                                               const float *__restrict__ group_lr, unsigned mask, bool per_group) {
+    if (gi < 0 || !((mask >> gi) & 1u)) {
         if (a.zero_grad) g = 0.f;
         return;
     }
     a.lr_over_bc1 = __ldg(group_lr + gi);
+    if (per_group) a.inv_sqrt_bc2 = __ldg(group_lr + kTabBc2 + gi);
     adam_one(p, g, m, v, a);
 }
 
@@ -214,7 +272,9 @@ __global__ void __launch_bounds__(ADAM_THREADS) adam_groups_kernel(long long n, 
                                                                    const AdamState *__restrict__ st,
                                                                    const float *__restrict__ group_lr, SegTable segs) {
     a.inv_sqrt_bc2 = st->inv_sqrt_bc2;
-    const bool skip = st->skip != 0;
+    const int mode = st->skip;  // 0 one bias correction, kSkipVeto vetoed, kSkipPerGroup per-group counts and a mask
+    const bool skip = mode == kSkipVeto, per_group = mode == kSkipPerGroup;
+    const unsigned mask = per_group ? __ldg(reinterpret_cast<const unsigned *>(group_lr) + kTabMask) : ~0u;
     const long long n4 = n >> 2;
     const long long stride = (long long)gridDim.x * blockDim.x;
     float4 *p4 = reinterpret_cast<float4 *>(p), *g4 = reinterpret_cast<float4 *>(g);
@@ -225,13 +285,18 @@ __global__ void __launch_bounds__(ADAM_THREADS) adam_groups_kernel(long long n, 
             continue;
         }
         const long long e0 = goff + (i << 2);
-        float4 P = p4[i], G = g4[i], M = m4[i], V = v4[i];
         const int j = segment_of(segs, e0);
+        if (j >= 0 && e0 + 4 <= segs.s[j].end && segs.s[j].period == 0 && !((mask >> segs.s[j].ga) & 1u)) {
+            if (a.zero_grad) g4[i] = make_float4(0.f, 0.f, 0.f, 0.f);  // a masked group: only the gradient is cleared
+            continue;
+        }
+        float4 P = p4[i], G = g4[i], M = m4[i], V = v4[i];
         int gi[4];
         if (j >= 0 && e0 + 4 <= segs.s[j].end) {  // the whole vector lies in one segment
             const Segment &S = segs.s[j];
             if (S.period == 0) {  // fast path: one group, one constant
                 a.lr_over_bc1 = __ldg(group_lr + S.ga);
+                if (per_group) a.inv_sqrt_bc2 = __ldg(group_lr + kTabBc2 + S.ga);
                 adam_one(P.x, G.x, M.x, V.x, a); adam_one(P.y, G.y, M.y, V.y, a);
                 adam_one(P.z, G.z, M.z, V.z, a); adam_one(P.w, G.w, M.w, V.w, a);
                 p4[i] = P; m4[i] = M; v4[i] = V;
@@ -248,15 +313,17 @@ __global__ void __launch_bounds__(ADAM_THREADS) adam_groups_kernel(long long n, 
 #pragma unroll
             for (int c = 0; c < 4; ++c) gi[c] = group_at(segs, e0 + c);
         }
-        adam_group_one(P.x, G.x, M.x, V.x, gi[0], a, group_lr); adam_group_one(P.y, G.y, M.y, V.y, gi[1], a, group_lr);
-        adam_group_one(P.z, G.z, M.z, V.z, gi[2], a, group_lr); adam_group_one(P.w, G.w, M.w, V.w, gi[3], a, group_lr);
+        adam_group_one(P.x, G.x, M.x, V.x, gi[0], a, group_lr, mask, per_group);
+        adam_group_one(P.y, G.y, M.y, V.y, gi[1], a, group_lr, mask, per_group);
+        adam_group_one(P.z, G.z, M.z, V.z, gi[2], a, group_lr, mask, per_group);
+        adam_group_one(P.w, G.w, M.w, V.w, gi[3], a, group_lr, mask, per_group);
         p4[i] = P; m4[i] = M; v4[i] = V;
         if (a.zero_grad) g4[i] = G;
     }
     if (blockIdx.x == 0 && threadIdx.x < (int)(n & 3)) {
         const long long i = (n4 << 2) + threadIdx.x;
         if (skip) { if (a.zero_grad) g[i] = 0.f; }
-        else adam_group_one(p[i], g[i], m[i], v[i], group_at(segs, goff + i), a, group_lr);
+        else adam_group_one(p[i], g[i], m[i], v[i], group_at(segs, goff + i), a, group_lr, mask, per_group);
     }
 }
 
@@ -362,13 +429,10 @@ extern "C" int b200_adam_step_state_background(long long numel, float *param, fl
 }
 
 // ---- per-group learning rates: host side ---------------------------------------------------------------------------
-extern "C" int b200_adam_prepare_groups(void *state, int32_t *veto_flag, int n_groups, const double *groups, double beta1,
-                                        double beta2, float *group_lr, void *stream) {
-    B200_REQUIRE(state && group_lr, "null state or group_lr");
+static int lr_table(int n_groups, const double *groups, LrTable &tab) {
     B200_REQUIRE(n_groups >= 1 && n_groups <= B200_ADAM_MAX_GROUPS, "n_groups must be in [1, B200_ADAM_MAX_GROUPS]");
     B200_REQUIRE(groups, "null group table");
-    B200_REQUIRE(beta1 >= 0.0 && beta1 < 1.0 && beta2 >= 0.0 && beta2 < 1.0, "betas must lie in [0, 1)");
-    LrTable tab{};
+    tab = LrTable{};
     tab.n = n_groups;
     for (int k = 0; k < n_groups; ++k) {
         const double *w = groups + (size_t)k * B200_LR_GROUP_DOUBLES;
@@ -383,8 +447,38 @@ extern "C" int b200_adam_prepare_groups(void *state, int32_t *veto_flag, int n_g
             B200_REQUIRE(w[6] == 0.0 || w[6] == 1.0, "ramp must be 0 (cosine) or 1 (linear)");
         }
     }
+    return B200_OK;
+}
+
+extern "C" int b200_adam_prepare_groups(void *state, int32_t *veto_flag, int n_groups, const double *groups, double beta1,
+                                        double beta2, float *group_lr, void *stream) {
+    B200_REQUIRE(state && group_lr, "null state or group_lr");
+    B200_REQUIRE(beta1 >= 0.0 && beta1 < 1.0 && beta2 >= 0.0 && beta2 < 1.0, "betas must lie in [0, 1)");
+    LrTable tab;
+    const int rc = lr_table(n_groups, groups, tab);
+    if (rc != B200_OK) return rc;
     adam_prepare_groups_kernel<<<1, 32, 0, as_stream(stream)>>>(static_cast<AdamState *>(state), veto_flag, beta1, beta2,
                                                                 tab, group_lr);
+    B200_LAUNCH_CHECK();
+    return B200_OK;
+}
+
+extern "C" int b200_adam_prepare_groups_masked(void *state, int32_t *veto_flag, const int32_t *detached,
+                                               unsigned detached_groups, int cond_group, int cond_every, int n_groups,
+                                               const double *groups, double beta1, double beta2, float *group_table,
+                                               void *stream) {
+    B200_REQUIRE(state && group_table, "null state or group_table");
+    B200_REQUIRE(beta1 >= 0.0 && beta1 < 1.0 && beta2 >= 0.0 && beta2 < 1.0, "betas must lie in [0, 1)");
+    B200_REQUIRE(cond_group < n_groups, "cond_group must be < n_groups (or negative: none)");
+    B200_REQUIRE(cond_group < 0 || cond_every >= 1, "cond_every must be >= 1");
+    B200_REQUIRE(aligned16(group_table), "group_table must be 16-byte aligned");
+    LrTable tab;
+    const int rc = lr_table(n_groups, groups, tab);
+    if (rc != B200_OK) return rc;
+    adam_prepare_groups_masked_kernel<<<1, 32, 0, as_stream(stream)>>>(static_cast<AdamState *>(state), veto_flag, detached,
+                                                                       detached_groups, cond_group < 0 ? -1 : cond_group,
+                                                                       cond_every < 1 ? 1 : cond_every, beta1, beta2, tab,
+                                                                       group_table);
     B200_LAUNCH_CHECK();
     return B200_OK;
 }

@@ -130,6 +130,20 @@ __global__ void __launch_bounds__(kThreads) scale_regularizer_kernel(int n, cons
     if (reduce_ticketed<1>(sum, partial, ticket, total)) value[0] += (total[0] / (float)n) * weight;
 }
 
+// Splatfacto's detached eval cameras (splatfacto.py:706-709, :767-773): the step's loss reaches only the camera rows.
+// The fused backward has written every row; with a non-zero *detached the Gaussian and background rows are cleared here,
+// before the scale regulariser adds its gradient, so that they hold exactly what the reference's graph gives them.
+struct GradRanges { int n; long long begin[B200_DETACHED_MAX_RANGES], end[B200_DETACHED_MAX_RANGES]; };
+
+__global__ void __launch_bounds__(kThreads) detached_grad_rows_kernel(const int32_t *__restrict__ detached, GradRanges r,
+                                                                      float *__restrict__ grad) {
+    if (*detached == 0) return;
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (int k = 0; k < r.n; ++k)
+        for (long long i = r.begin[k] + (long long)blockIdx.x * blockDim.x + threadIdx.x; i < r.end[k]; i += stride)
+            grad[i] = 0.f;
+}
+
 int blocks_for(long long n) {
     const long long want = (n + kThreads - 1) / kThreads;
     return (int)(want < 1 ? 1 : (want > kMaxBlocks ? kMaxBlocks : want));
@@ -182,6 +196,26 @@ extern "C" B200_API int b200_scale_regularizer(int num_points, const float *log_
     scale_regularizer_kernel<<<blocks_for(num_points), kThreads, 0, st>>>(
         num_points, log_scales, max_ratio, weight, every, static_cast<const int32_t *>(adam_state), g_log_scales, value,
         partial, ticket);
+    B200_LAUNCH_CHECK();
+    return B200_OK;
+}
+
+extern "C" B200_API int b200_detached_grad_rows(const int32_t *detached, int n_ranges, const long long *ranges, float *grad,
+                                               void *stream) {
+    B200_REQUIRE(detached && grad, "detached_grad_rows: null pointer");
+    B200_REQUIRE(n_ranges >= 0 && n_ranges <= B200_DETACHED_MAX_RANGES,
+                 "detached_grad_rows: n_ranges must be in [0, B200_DETACHED_MAX_RANGES]");
+    B200_REQUIRE(n_ranges == 0 || ranges, "detached_grad_rows: null range table");
+    GradRanges r{};
+    long long longest = 0;
+    for (int k = 0; k < n_ranges; ++k) {
+        B200_REQUIRE(ranges[2 * k] >= 0 && ranges[2 * k] <= ranges[2 * k + 1], "detached_grad_rows: need 0 <= begin <= end");
+        r.begin[k] = ranges[2 * k];
+        r.end[k] = ranges[2 * k + 1];
+        if (r.end[k] - r.begin[k] > longest) longest = r.end[k] - r.begin[k];
+    }
+    r.n = n_ranges;
+    detached_grad_rows_kernel<<<blocks_for(longest), kThreads, 0, as_stream(stream)>>>(detached, r, grad);
     B200_LAUNCH_CHECK();
     return B200_OK;
 }

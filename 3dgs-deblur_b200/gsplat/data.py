@@ -72,13 +72,33 @@ def orient_and_center(poses: np.ndarray, method: str = "up", center_method: str 
 
 
 def split_indices(n: int, split: str, eval_mode: str = "fraction", train_split_fraction: float = 0.9,
-                  eval_interval: int = 8) -> np.ndarray:
-    """dataparsers_utils.py:23-43 ("fraction"), :69-86 ("interval"), "all"."""
+                  eval_interval: int = 8, optimize_eval_cameras: bool = False, filenames: Optional[List[str]] = None):
+    """dataparsers_utils.py:23-43 ("fraction"), :46-68 ("filename": basenames containing "train" or "eval", needs
+    `filenames`), :69-86 ("interval"), "all".
+
+    optimize_eval_cameras (3dgs-deblur's --optimize-eval-cameras, nerfstudio_dataparser.py:241-252): the train split
+    becomes the eval images followed by the training images, and the call returns (indices, detached) with detached[i]
+    True for the eval images at the front -- their loss may move only their own camera's pose and velocity rows.  The
+    val / test splits keep their order and are all detached, as the reference marks them.  "all" keeps every image
+    trained and none detached."""
     i_all = np.arange(n)
     if eval_mode == "fraction":
         n_train = math.ceil(n * train_split_fraction)
         i_train = np.linspace(0, n - 1, n_train, dtype=int)
         i_eval = np.setdiff1d(i_all, i_train)
+    elif eval_mode == "filename":
+        if filenames is None or len(filenames) != n:
+            raise ValueError("eval_mode 'filename' needs the n image filenames")
+        i_train, i_eval = [], []
+        for i, name in enumerate(filenames):
+            base = os.path.basename(name)
+            if "train" in base:
+                i_train.append(i)
+            elif "eval" in base:
+                i_eval.append(i)
+            else:
+                raise ValueError("frame should contain train/eval in its name to use this eval-frame-index eval mode")
+        i_train, i_eval = np.array(i_train, dtype=np.int64), np.array(i_eval, dtype=np.int64)
     elif eval_mode == "interval":
         i_train = i_all[i_all % eval_interval != 0]
         i_eval = i_all[i_all % eval_interval == 0]
@@ -86,11 +106,21 @@ def split_indices(n: int, split: str, eval_mode: str = "fraction", train_split_f
         i_train = i_eval = i_all
     else:
         raise ValueError(f"unsupported eval_mode: {eval_mode}")
+    detach = optimize_eval_cameras and eval_mode != "all"
+    if detach:
+        i_train = np.hstack([i_eval, i_train]).ravel().astype(np.int64)
     if split == "train":
-        return i_train
-    if split in ("val", "test"):
-        return i_eval
-    raise ValueError(f"Unknown dataparser split {split}")
+        idx = i_train
+    elif split in ("val", "test"):
+        idx = i_eval
+    else:
+        raise ValueError(f"Unknown dataparser split {split}")
+    if not optimize_eval_cameras:
+        return idx
+    detached = np.zeros(len(idx), bool)
+    if detach:  # the reference's rule, position < len(i_eval), in either split (val / test: all of them)
+        detached[:len(i_eval)] = True
+    return idx, detached
 
 
 def _auto_downscale(data_dir: str, rel_path: str) -> int:
@@ -109,12 +139,16 @@ def _auto_downscale(data_dir: str, rel_path: str) -> int:
 
 def load_transforms(path: str, split: str = "train", *, scale_factor: float = 1.0, downscale_factor: Optional[int] = None,
                     orientation_method: str = "up", center_method: str = "poses", auto_scale_poses: bool = True,
-                    eval_mode: str = "fraction", train_split_fraction: float = 0.9, eval_interval: int = 8) -> Dict:
+                    eval_mode: str = "fraction", train_split_fraction: float = 0.9, eval_interval: int = 8,
+                    optimize_eval_cameras: bool = False) -> Dict:
     """Parse a nerfstudio dataset directory (or its transforms.json) the way the reference's dataparser does.
 
     Returns a dict: image_filenames (list), camera_to_worlds (n,3,4) f32, fx, fy, cx, cy (n,) f32, height, width (n,) i64,
     velocities (n,6) f32 or None (linear part already in scene units), exposure_time, rolling_shutter_time (floats or
-    None), dataparser_scale (float), dataparser_transform (3,4) f32, indices (n,) into the name-sorted frame list."""
+    None), dataparser_scale (float), dataparser_transform (3,4) f32, indices (n,) into the name-sorted frame list, and
+    detached: None, or with optimize_eval_cameras a bool (n,) marking the eval images split_indices put at the front of
+    the train split (pass their positions as PipelinedTrainer(detached_cameras=...)).  A dataset that lists its split
+    files ("<split>_filenames") cannot optimise its eval cameras (AssertionError, as the reference asserts)."""
     if path.endswith(".json"):
         meta_path, data_dir = path, os.path.dirname(path)
     else:
@@ -173,7 +207,10 @@ def load_transforms(path: str, split: str = "train", *, scale_factor: float = 1.
     poses[:, :3, 3] *= scale
 
     split_key = f"{split}_filenames"
+    detached = None
     if split_key in meta:
+        if optimize_eval_cameras:
+            raise AssertionError("optimize_eval_cameras needs a split rule, not listed <split>_filenames")
         wanted = {fname(x, downscale_factor) for x in meta[split_key]}
         unmatched = wanted.difference(names)
         if unmatched:
@@ -182,7 +219,10 @@ def load_transforms(path: str, split: str = "train", *, scale_factor: float = 1.
     elif any(f"{s}_filenames" in meta for s in ("train", "val", "test")):
         raise RuntimeError(f"The dataset's list of filenames for split {split} is missing.")
     else:
-        idx = split_indices(len(names), split, eval_mode, train_split_fraction, eval_interval).astype(np.int64)
+        idx = split_indices(len(names), split, eval_mode, train_split_fraction, eval_interval, optimize_eval_cameras, names)
+        if optimize_eval_cameras:
+            idx, detached = idx
+        idx = idx.astype(np.int64)
 
     if velocities is not None:
         velocities = velocities[idx].copy()
@@ -204,7 +244,7 @@ def load_transforms(path: str, split: str = "train", *, scale_factor: float = 1.
         image_filenames=[names[i] for i in idx], camera_to_worlds=poses[idx][:, :3, :4].copy(),
         fx=f32(fx), fy=f32(fy), cx=f32(cx), cy=f32(cy), height=size(height), width=size(width),
         velocities=velocities, exposure_time=meta.get("exposure_time"), rolling_shutter_time=meta.get("rolling_shutter_time"),
-        dataparser_scale=scale_out, dataparser_transform=transform_out, indices=idx)
+        dataparser_scale=scale_out, dataparser_transform=transform_out, indices=idx, detached=detached)
 
 
 _PLY_TYPES = {"char": "i1", "uchar": "u1", "int8": "i1", "uint8": "u1", "short": "i2", "ushort": "u2", "int16": "i2",

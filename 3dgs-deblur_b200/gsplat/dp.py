@@ -226,8 +226,10 @@ class ImageShardedTrainer:
     """One process per GPU; rank r renders image (step * world + r) % n_images; one gradient exchange per step."""
 
     def __init__(self, model: FlatGaussians, scene: Dict, lr: float = 1e-3, group=None, overlap_sh: bool = True,
-                 fused: bool = False, loss_fn=None, sh_chunks: int = 1, optimizer: str = "b200"):
+                 fused: bool = False, loss_fn=None, sh_chunks: int = 1, optimizer: str = "b200", detached_cameras=None):
         self.model, self.scene = model, scene
+        if detached_cameras is not None:
+            raise ValueError("ImageShardedTrainer does not detach eval cameras: use PipelinedTrainer(operators='fused')")
         if model.cam_pose is not None:
             raise ValueError("ImageShardedTrainer does not optimise camera poses: use PipelinedTrainer(operators='fused')")
         if model.learnable_bg is not None:
@@ -609,7 +611,8 @@ class PipelinedTrainer:
                  optimizer: str = "b200", sh_chunks: int = 1, operators: Optional[str] = None,
                  rasterize_mode: str = "antialiased", color_mode: str = "sh", num_downscales: int = 0,
                  resolution_schedule: int = 3000, sh_degree_interval: int = 0, camera_l2=None,
-                 scale_regularization: bool = False, max_gauss_ratio: float = 10.0):
+                 scale_regularization: bool = False, max_gauss_ratio: float = 10.0, detached_cameras=None,
+                 optimize_eval_velocities: bool = True):
         """operators: "dropin" = the two phases on the reference-compatible operators under autograd (`geometry_phase` /
         `shading_phase`); "fused" = on the fused raw-parameter kernels (`fused_geometry_phase` / `fused_shading_phase`:
         same numbers, ~45 fewer launches per step); None = fused where it applies (CUDA, sh_layout "split"), else drop-in.
@@ -631,7 +634,15 @@ class PipelinedTrainer:
         scale_regularization / max_gauss_ratio: Splatfacto's use_scale_regularization: at steps k with k % 10 == 0 (k =
         `steps`, vetoed steps included, read on the device) 0.1 * mean(max(amax(e^s) / amin(e^s), max_gauss_ratio) -
         max_gauss_ratio) over all Gaussians is added to the returned loss and its gradient to log_scales'.  Needs CUDA and
-        optimizer="b200"."""
+        optimizer="b200".
+        detached_cameras: None, a set of camera indices, or a bool per camera row (gsplat.data.load_transforms'
+        `detached` with optimize_eval_cameras): 3dgs-deblur's --optimize-eval-cameras (splatfacto.py:706-709, :767-773).
+        A step on an image whose `cam_index` is detached renders and back-propagates as usual, but its loss reaches only
+        the camera rows: the Gaussian and background rows' gradients are cleared on the device (b200_detached_grad_rows)
+        before the scale regulariser adds its own, and the device Adam steps only the pose and velocity groups (and
+        log_scales when the regulariser fires), each group keeping its own step count (gsplat.optim.FlatAdam.
+        use_group_masks).  The same captured graphs serve both kinds of step.  A float `lr` becomes that rate for every
+        group.  Fused operators, optimizer="b200" and CUDA only; optimize_eval_velocities=False is not supported."""
         self.model, self.scene = model, dict(scene)
         if int(num_downscales) != num_downscales or not 0 <= num_downscales <= 4:
             raise ValueError("num_downscales must be an integer from 0 to 4 (factors up to 16)")
@@ -679,6 +690,20 @@ class PipelinedTrainer:
         if self.scale_regularization and (model.flat.device.type != "cuda" or optimizer != "b200"):
             raise ValueError("scale_regularization needs a CUDA model and optimizer='b200' (it reads the device step "
                              "count of the Adam state)")
+        self._detached = None
+        if detached_cameras is not None:
+            if not optimize_eval_velocities:
+                raise ValueError("optimize_eval_velocities=False is not supported: it needs per-row masks inside the "
+                                 "velocity groups")
+            if operators != "fused" or optimizer != "b200" or model.flat.device.type != "cuda":
+                raise ValueError("detached_cameras need operators='fused', optimizer='b200' and a CUDA model (the step "
+                                 "mask is decided on the device)")
+            dc = list(detached_cameras)
+            if dc and all(isinstance(x, (bool,)) or type(x).__name__ == "bool_" for x in dc):
+                dc = [i for i, x in enumerate(dc) if x]
+            self._detached = {int(i) for i in dc}
+            if any(i < 0 for i in self._detached):
+                raise ValueError("detached_cameras: camera indices must be >= 0")
         self.operators = operators
         phases = (fused_geometry_phase, fused_shading_phase) if operators == "fused" else (geometry_phase, shading_phase)
         modes = dict(rasterize_mode=rasterize_mode, color_mode=color_mode)
@@ -697,6 +722,9 @@ class PipelinedTrainer:
         # static per-step inputs / outputs
         self.st = dict(cam=torch.zeros(21, dtype=torch.float32, device=dev), cam_index=torch.zeros(1, dtype=torch.int64, device=dev))
         self.status = torch.zeros(4, dtype=torch.int32, device=dev)       # [overflow, entries, max entries, reference isects]
+        # detached cameras: [0] this image's word (read by phase B), [1] the step's (all ranks detached; read by Adam)
+        self.detached_words = torch.zeros(2, dtype=torch.int32, device=dev) if self._detached is not None else None
+        self._det_work = None
         self.flag = self.status[0:1]                                      # this step's veto (reduced with MAX across ranks)
         self.loss = torch.zeros((), dtype=torch.float32, device=dev)
         self.capacity = capacity
@@ -721,6 +749,9 @@ class PipelinedTrainer:
                 raise ValueError(f"lr must be a float, a dict of per-group rates or 'splatfacto', got {lr!r}")
             from gsplat.optim import splatfacto_background_lr, splatfacto_lr, splatfacto_pose_lr
             lr = {**splatfacto_lr(), **splatfacto_pose_lr(), **splatfacto_background_lr()}  # rows the model lacks: ignored
+        if self._detached is not None and not isinstance(lr, dict):  # a mask needs the group table
+            from gsplat.optim import BACKGROUND_GROUP, GROUPS, POSE_GROUPS
+            lr = {name: float(lr) for name in GROUPS + POSE_GROUPS + (BACKGROUND_GROUP,)}
         self.lr_groups = dict(lr) if isinstance(lr, dict) else None
         if self.lr_groups is not None and optimizer != "b200":
             raise ValueError("per-group learning rates need optimizer='b200' (the grouped device-state Adam)")
@@ -732,6 +763,12 @@ class PipelinedTrainer:
                 self.lr_group_names, scheds, segs = group_segments(model, self.lr_groups)
                 self.adam = FlatAdam(model.flat, model.flat_grad, lr=0.0, eps=1e-15).use_device_state(groups=scheds)
                 self.adam.set_groups(segs)
+                if self._detached is not None:
+                    names = self.lr_group_names
+                    cams = [names.index(n) for n in ("cam_vel_linear", "cam_vel_angular", "cam_pose_trans", "cam_pose_rot")
+                            if n in names]
+                    reg = names.index("log_scales") if self.scale_regularization else None
+                    self.adam.use_group_masks(cams, reg, 10)
         elif optimizer == "torch":  # CPU / gloo tests of this host logic: same slices, torch's Adam, host-side veto
             self.adam = None
             lo, total = model.sh_start, model.flat.numel()
@@ -771,6 +808,8 @@ class PipelinedTrainer:
                     (self._full if self._full is not None else self.scene)[k] = float(cam[k])
         self.st["cam"].copy_(row, non_blocking=True)
         self.st["cam_index"].fill_(int(cam_index))
+        if self.detached_words is not None:
+            self.detached_words.fill_(int(int(cam_index) in self._detached))
 
     def downscale_factor(self, image: int) -> int:
         """Splatfacto's _get_downscale_factor (splatfacto.py:660-667) for the image trained at step `image`."""
@@ -886,6 +925,7 @@ class PipelinedTrainer:
             with torch.cuda.graph(g, stream=self.main):
                 tgt = self._as_target(e["target"])
                 self.loss.copy_(self.shading_fn(self.model, e["geo"], self.scene, tgt, self.loss_fn, self.sh_degree))
+                self._detached_rows()
                 self._camera_regularisers()
                 self._scale_regulariser()
             e["gB"], e["nB"] = g, self._lib_launches() - n0
@@ -893,9 +933,31 @@ class PipelinedTrainer:
             return
         tgt = self._as_target(target)
         self.loss.copy_(self.shading_fn(self.model, self._geo, self.scene, tgt, self.loss_fn, self.sh_degree))
+        self._detached_rows()
         self._camera_regularisers()
         self._scale_regulariser()
         e["warm"] += 1
+
+    def _detached_rows(self):
+        """detached_cameras: on a detached image the Gaussian and background rows of the gradient are cleared on the
+        device (nothing happens on other images), so they hold what the reference's detached graph gives them."""
+        if self.detached_words is None:
+            return
+        from gsplat import _lib
+        m = self.model
+        ranges = []
+        for name, _, _ in m.fields:
+            if name in ("cam_vel", "cam_pose"):
+                continue
+            a, b_ = m.slices[name]
+            if ranges and ranges[-1][1] >= a - 3:  # neighbours (across the SH alignment pad, which has no group)
+                ranges[-1][1] = b_
+            else:
+                ranges.append([a, b_])
+        tab = torch.tensor(ranges, dtype=torch.int64).reshape(-1)
+        with _lib.on_device(self.device):
+            _lib.check(_lib.load().b200_detached_grad_rows(self.detached_words.data_ptr(), len(ranges), tab.data_ptr(),
+                                                           m.flat_grad.data_ptr(), _lib.stream()))
 
     def _camera_regularisers(self):
         """camera_l2: the regulariser values added to the step's loss, their gradients to the camera rows' gradients."""
@@ -987,6 +1049,9 @@ class PipelinedTrainer:
             self._A_done = True
             if self.distributed:  # this image's overflow flag, agreed on by all ranks before anyone's Adam reads it
                 self._flag_work = dist.all_reduce(self.flag, op=dist.ReduceOp.MAX, group=self.group, async_op=True)
+                if self.detached_words is not None:  # a group steps if any rank's image gave it a gradient
+                    self._det_work = dist.all_reduce(self.detached_words[1:2], op=dist.ReduceOp.MIN, group=self.group,
+                                                     async_op=True)
 
     def train_step(self, target: torch.Tensor, next_cam=None, next_index: int = 0):
         """Trains on the prepared image (B, exchange, update) and, given `next_cam`, runs A for the next image while the
@@ -1021,10 +1086,13 @@ class PipelinedTrainer:
             works = [dist.all_reduce(m.flat_grad[:lo], op=self._op, group=self.group, async_op=True)]
             works += [dist.all_reduce(m.flat_grad[a:b_], op=self._op, group=self.group, async_op=True) for a, b_ in self._sh_bounds]
             self._flag_work.wait()
+            if self._det_work is not None:
+                self._det_work.wait()
+                self._det_work = None
         scale = 1.0 if (self._avg or not self.distributed) else 1.0 / self.world
         veto_host = False
         if self.adam is not None:
-            self.adam.prepare(self.flag)
+            self.adam.prepare(self.flag, None if self.detached_words is None else self.detached_words[1:2])
             if self.cuda:
                 self.ev_prepared.record()
         else:  # torch optimizer (CPU tests): the veto is read on the host

@@ -155,6 +155,10 @@ def group_segments(model, lr):
     return present, [lr[n] for n in present], segs
 
 
+MAX_GROUPS = 16          # B200_ADAM_MAX_GROUPS
+GROUP_TABLE_FLOATS = 64  # B200_ADAM_GROUP_TABLE_FLOATS: lr / bc1 [16] | 1 / sqrt(bc2) [16] | step counts [16] | mask
+
+
 class FlatAdam:
     def __init__(self, flat: torch.Tensor, flat_grad: torch.Tensor, lr: float = 1e-3, betas=(0.9, 0.999), eps: float = 1e-15):
         _lib.require_cuda(flat, flat_grad)
@@ -178,10 +182,10 @@ class FlatAdam:
         if getattr(self, "state", None) is None:
             nbytes = self._lib.b200_adam_state_bytes()
             self.state = torch.zeros(nbytes // 4, dtype=torch.int32, device=self.flat.device)
-        self.groups = None
+        self.groups = self._mask = None
         if groups is not None:
             groups = list(groups)
-            if not 1 <= len(groups) <= 16:
+            if not 1 <= len(groups) <= MAX_GROUPS:
                 raise ValueError("FlatAdam: between 1 and 16 learning-rate groups (B200_ADAM_MAX_GROUPS)")
             self._group_table = torch.tensor([_group_row(g) for g in groups], dtype=torch.float64)
             self.groups = groups
@@ -208,12 +212,52 @@ class FlatAdam:
             return None
         return [lr_at(g, int(step)) for g in self.groups]
 
-    def prepare(self, veto_flag=None):
+    def use_group_masks(self, detached_groups, cond_group=None, cond_every: int = 10):
+        """Per-group step counts and per-step masks (b200_adam_prepare_groups_masked), for steps whose loss gives some
+        groups no gradient (Splatfacto's detached eval cameras: nerfstudio then skips those groups' optimizers, and torch's
+        Adam keeps their step counts).  After this, `prepare(veto_flag, detached)` with a non-zero device word `detached`
+        steps only the group indices in `detached_groups`, plus `cond_group` at steps whose index is a multiple of
+        `cond_every` (the scale regulariser's clock); every other group keeps its parameters, moments and step count.
+        With `detached` zero or None every group steps.  `group_lr` becomes the 64-float group table; `group_steps()`
+        reads the counts.  Needs use_device_state(groups=...)."""
+        if getattr(self, "groups", None) is None:
+            raise ValueError("FlatAdam.use_group_masks: call use_device_state(groups=...) first")
+        bits = 0
+        for g in detached_groups:
+            if not 0 <= int(g) < len(self.groups):
+                raise ValueError(f"FlatAdam.use_group_masks: group index {g} outside the group table")
+            bits |= 1 << int(g)
+        if cond_group is not None and not 0 <= int(cond_group) < len(self.groups):
+            raise ValueError(f"FlatAdam.use_group_masks: group index {cond_group} outside the group table")
+        if int(cond_every) < 1:
+            raise ValueError("FlatAdam.use_group_masks: cond_every must be >= 1")
+        table = torch.zeros(GROUP_TABLE_FLOATS, dtype=torch.float32, device=self.flat.device)
+        table[:len(self.groups)] = self.group_lr
+        self.group_lr = table
+        self._mask = (bits, -1 if cond_group is None else int(cond_group), int(cond_every))
+        return self
+
+    def group_steps(self):
+        """Steps each group has taken (host list; synchronises).  None without use_group_masks."""
+        if getattr(self, "_mask", None) is None:
+            return None
+        return self.group_lr[2 * MAX_GROUPS:2 * MAX_GROUPS + len(self.groups)].view(torch.int32).tolist()
+
+    def prepare(self, veto_flag=None, detached=None):
         """Once per step, before the first `update_state`.  veto_flag: device int32[1] (or None); non-zero skips this step's
-        update on the device (gradients are still cleared) and is reset to zero."""
+        update on the device (gradients are still cleared) and is reset to zero.  detached: device int32[1] (or None),
+        read after use_group_masks only (see there)."""
         veto = None if veto_flag is None else veto_flag.data_ptr()
         with _lib.on_device(self.flat.device):
-            if getattr(self, "groups", None) is not None:
+            if getattr(self, "_mask", None) is not None:
+                bits, cond, every = self._mask
+                check(self._lib.b200_adam_prepare_groups_masked(
+                    self.state.data_ptr(), veto, None if detached is None else detached.data_ptr(), bits, cond, every,
+                    len(self.groups), self._group_table.data_ptr(), self.betas[0], self.betas[1],
+                    self.group_lr.data_ptr(), stream()))
+            elif detached is not None:
+                raise ValueError("FlatAdam.prepare: a detached word needs use_group_masks")
+            elif getattr(self, "groups", None) is not None:
                 check(self._lib.b200_adam_prepare_groups(self.state.data_ptr(), veto, len(self.groups),
                                                          self._group_table.data_ptr(), self.betas[0], self.betas[1],
                                                          self.group_lr.data_ptr(), stream()))

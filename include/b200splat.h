@@ -745,6 +745,32 @@ B200_API int b200_adam_step_state_groups_background(long long numel, long long o
                                                     double beta1, double beta2, double eps, double grad_scale, int zero_grad,
                                                     int ctas_per_sm, void *stream);
 
+/* Per-group step counts and per-step group masks (Splatfacto's detached eval cameras: nerfstudio steps an optimizer only
+ * when one of its parameters has a gradient, engine/optimizers.py:158-171, and torch's Adam keeps a step count per
+ * parameter, so a group without a gradient keeps its parameters, moments and step count).
+ *   group_table: DEVICE float[B200_ADAM_GROUP_TABLE_FLOATS], 16-byte aligned, zeroed by the caller before the first step:
+ *       [g] lr_g(s) / (1 - beta1^t_g), [16 + g] 1 / sqrt(1 - beta2^t_g), [32 + g] t_g (int32: steps group g has taken),
+ *       [48] the mask of the last prepared step (uint32, bit g = group g steps).
+ *   b200_adam_prepare_groups_masked: b200_adam_prepare_groups with each group's bias corrections counted by its own t_g.
+ *       detached: DEVICE int32 or null.  Null or zero: every group steps.  Non-zero: only the groups of the bit mask
+ *       detached_groups step, and group cond_group as well when the step index s (word [4] before the increment) is a
+ *       multiple of cond_every (cond_group < 0: none).  A group that steps advances t_g and gets new constants; the others
+ *       keep both.  The schedules stay on s.  A vetoed step vetoes every group, as before, and leaves the table alone.
+ *       The state is marked (word [3] = 2) so that b200_adam_step_state_groups / _background, called with group_lr =
+ *       group_table, give every element its own group's constants and leave the parameters and moments of a group outside
+ *       the mask bit-unchanged while still clearing its gradient.  Use only the grouped update after this prepare.
+ * b200_detached_grad_rows: when *detached (DEVICE int32) is non-zero, grad[i] = 0 for i in each [begin, end) of ranges
+ * (HOST long long[n_ranges][2], by value); otherwise nothing is touched.  The fused trainer clears the Gaussian and
+ * background rows of a detached image's gradient with it, after the backward and before the scale regulariser. */
+#define B200_ADAM_GROUP_TABLE_FLOATS 64
+#define B200_DETACHED_MAX_RANGES 4
+B200_API int b200_adam_prepare_groups_masked(void *state, int32_t *veto_flag, const int32_t *detached,
+                                             unsigned detached_groups, int cond_group, int cond_every, int n_groups,
+                                             const double *groups, double beta1, double beta2, float *group_table,
+                                             void *stream);
+B200_API int b200_detached_grad_rows(const int32_t *detached, int n_ranges, const long long *ranges, float *grad,
+                                     void *stream);
+
 /* ---- rasterization without a host sync ---------------------------------------------------------------------------
  * The reference reads the intersection count back to size its lists (gsplat/utils.py:123-124 `.item()`); the two-phase
  * culled binning above reads the culled count.  In CAPACITY mode the caller sizes the lists from a running high-water
