@@ -31,31 +31,12 @@ constexpr int ADAM_THREADS = 256;
 struct AdamState {
     float lr_over_bc1, inv_sqrt_bc2;
     int step;          // optimizer steps applied so far
-    int skip;          // 1 = the current step is vetoed
+    int skip;          // 1 = the current step is vetoed, 2 = per-group counts and a mask in the group table
     int seen;          // steps prepared so far (applied + vetoed)
     int vetoed;        // steps vetoed so far
     int ring[10];      // `seen` index (0-based) of the last 10 vetoed steps, slot = vetoed % 10
 };
 static_assert(sizeof(AdamState) == 64, "AdamState is 64 bytes (B200_ADAM_STATE_BYTES)");
-
-__global__ void adam_prepare_kernel(AdamState *st, int32_t *veto_flag, double lr, double beta1, double beta2) {
-    if (threadIdx.x != 0 || blockIdx.x != 0) return;
-    const bool veto = veto_flag && *veto_flag != 0;
-    if (veto_flag) *veto_flag = 0;  // consumed: the next step starts clean
-    const int idx = st->seen;
-    st->seen = idx + 1;
-    st->skip = veto ? 1 : 0;
-    if (veto) {
-        st->ring[st->vetoed % 10] = idx;
-        st->vetoed += 1;
-        return;
-    }
-    const int step = st->step + 1;
-    st->step = step;
-    const double bc1 = 1.0 - pow(beta1, (double)step), bc2 = 1.0 - pow(beta2, (double)step);
-    st->lr_over_bc1 = (float)(lr / bc1);
-    st->inv_sqrt_bc2 = (float)(1.0 / sqrt(bc2));
-}
 
 __global__ void __launch_bounds__(ADAM_THREADS) adam_state_kernel(long long n, float *__restrict__ p, float *__restrict__ g,
                                                                   float *__restrict__ m, float *__restrict__ v, AdamArgs a,
@@ -110,11 +91,19 @@ __global__ void adam_head_kernel(int n, float *p, float *g, float *m, float *v, 
     if ((int)threadIdx.x < n) adam_one(p[threadIdx.x], g[threadIdx.x], m[threadIdx.x], v[threadIdx.x], a);
 }
 
-// ---- per-group learning rates ----------------------------------------------------------------------------------------
+// ---- per-group learning rates, step counts and masks --------------------------------------------------------------
 // Splatfacto steps one Adam per parameter group, each with its own rate and scheduler (nerfstudio/configs/
 // method_configs.py: the splatfacto optimizers table).  Here one pass still updates any slice of the flat buffers: a
 // segment table maps each GLOBAL flat index to its group, and the prepare kernel leaves lr_g(s) / bc1 of every group in
-// a small device buffer.  Both tables travel by value in the kernel parameters (no copy, capturable).
+// the group table.  Both tables travel by value in the kernel parameters (no copy, capturable).  A single rate is one
+// constant group and no segment table: the update then runs adam_state_kernel on the state's constants.
+//
+// nerfstudio steps an optimizer only when one of its parameters has a gradient (engine/optimizers.py:158-171), and
+// torch's Adam keeps a step count per parameter: on a step that gives some groups no gradient (Splatfacto's detached eval
+// cameras) those groups keep their parameters, moments and step counts.  Given a `detached` word, the prepare keeps a
+// step count per group in the group table (B200_ADAM_GROUP_TABLE_FLOATS floats: lr_g / bc1(t_g), 1 / sqrt(bc2(t_g)), t_g,
+// the step's mask) and marks the state with skip = 2 so that the grouped update reads each group's own constants and the
+// mask.
 
 struct LrGroup {  // nerfstudio's ExponentialDecayScheduler (engine/schedulers.py), or a constant rate
     double lr_init, lr_final, lr_pre_warmup, warmup_steps, max_steps;
@@ -144,55 +133,20 @@ __device__ double scheduled_lr(const LrGroup &G, long long s) {
     return init * (lr / init);  // LambdaLR: base_lr * (func_lr(step) / lr_init)
 }
 
-// adam_prepare_kernel's state update (AdamState.lr_over_bc1 takes group 0's constant), then one thread per group writes
-// (float)(lr_g(s) / bc1) with s = the index of the step being prepared (vetoed steps included).  A vetoed step leaves
-// the group constants as they were, as adam_prepare_kernel leaves lr_over_bc1.
-__global__ void adam_prepare_groups_kernel(AdamState *st, int32_t *veto_flag, double beta1, double beta2, LrTable tab,
-                                           float *group_lr) {
-    const int t = threadIdx.x;
-    const bool veto = veto_flag && *veto_flag != 0;
-    const int idx = st->seen, step = st->step + 1;
-    __syncthreads();  // every thread has read the state before thread 0 advances it
-    if (veto) {
-        if (t == 0) {
-            *veto_flag = 0;
-            st->seen = idx + 1;
-            st->skip = 1;
-            st->ring[st->vetoed % 10] = idx;
-            st->vetoed += 1;
-        }
-        return;
-    }
-    const double bc1 = 1.0 - pow(beta1, (double)step);
-    if (t < tab.n) group_lr[t] = (float)(scheduled_lr(tab.g[t], idx) / bc1);
-    if (t == 0) {
-        if (veto_flag) *veto_flag = 0;
-        st->seen = idx + 1;
-        st->skip = 0;
-        st->step = step;
-        const double bc2 = 1.0 - pow(beta2, (double)step);
-        st->lr_over_bc1 = (float)(scheduled_lr(tab.g[0], idx) / bc1);
-        st->inv_sqrt_bc2 = (float)(1.0 / sqrt(bc2));
-    }
-}
-
-// ---- per-group step counts and step masks -------------------------------------------------------------------------
-// nerfstudio steps an optimizer only when one of its parameters has a gradient (engine/optimizers.py:158-171), and
-// torch's Adam keeps a step count per parameter: on a step that gives some groups no gradient (Splatfacto's detached eval
-// cameras) those groups keep their parameters, moments and step counts.  The masked prepare keeps a step count per group
-// in the group table (B200_ADAM_GROUP_TABLE_FLOATS floats: lr_g / bc1(t_g), 1 / sqrt(bc2(t_g)), t_g, the step's mask) and
-// marks the state with skip = 2 so that the grouped update reads each group's own constants and the mask.
 constexpr int kTabBc2 = B200_ADAM_MAX_GROUPS, kTabSteps = 2 * B200_ADAM_MAX_GROUPS, kTabMask = 3 * B200_ADAM_MAX_GROUPS;
 constexpr int kSkipVeto = 1, kSkipPerGroup = 2;
 
-// Which groups step: all of them, or with a non-zero *detached only `keep` plus `cond_group` when the step index is a
-// multiple of cond_every (the scale regulariser's clock).  A vetoed step is handled as by adam_prepare_groups_kernel.
-__global__ void adam_prepare_groups_masked_kernel(AdamState *st, int32_t *veto_flag, const int32_t *detached,
-                                                  unsigned keep, int cond_group, int cond_every, double beta1,
-                                                  double beta2, LrTable tab, float *table) {
+// The state's update (bias corrections count applied steps; AdamState.lr_over_bc1 takes group 0's constant), then thread
+// g writes group g's constants with s = the index of the step being prepared (vetoed steps included).  Without a
+// `detached` word every group steps at the global count.  With one, the groups that step are all of them, or with a
+// non-zero *detached only `keep` plus `cond_group` when s is a multiple of cond_every (the scale regulariser's clock); a
+// group outside the mask keeps its count and its constants.  A vetoed step leaves the group table as it was.
+__global__ void adam_prepare_step_kernel(AdamState *st, int32_t *veto_flag, const int32_t *detached, unsigned keep,
+                                         int cond_group, int cond_every, double beta1, double beta2, LrTable tab,
+                                         float *table) {
     const int t = threadIdx.x;
     const bool veto = veto_flag && *veto_flag != 0;
-    const bool det = detached && *detached != 0;
+    const bool per_group = detached != nullptr, det = per_group && *detached != 0;
     const int idx = st->seen, step = st->step + 1;
     __syncthreads();  // every thread has read the state before thread 0 advances it
     if (veto) {
@@ -213,18 +167,18 @@ __global__ void adam_prepare_groups_masked_kernel(AdamState *st, int32_t *veto_f
         mask &= all;
     }
     int32_t *steps = reinterpret_cast<int32_t *>(table + kTabSteps);
-    if (t < tab.n && ((mask >> t) & 1u)) {  // a masked group keeps its count and its constants
-        const int tg = steps[t] + 1;
-        steps[t] = tg;
-        const double bc1 = 1.0 - pow(beta1, (double)tg), bc2 = 1.0 - pow(beta2, (double)tg);
+    if (t < tab.n && ((mask >> t) & 1u)) {
+        int tg = step;
+        if (per_group) steps[t] = tg = steps[t] + 1;
+        const double bc1 = 1.0 - pow(beta1, (double)tg);
         table[t] = (float)(scheduled_lr(tab.g[t], idx) / bc1);
-        table[kTabBc2 + t] = (float)(1.0 / sqrt(bc2));
+        if (per_group) table[kTabBc2 + t] = (float)(1.0 / sqrt(1.0 - pow(beta2, (double)tg)));
     }
     if (t == 0) {
         if (veto_flag) *veto_flag = 0;
-        reinterpret_cast<uint32_t *>(table)[kTabMask] = mask;
+        if (per_group) reinterpret_cast<uint32_t *>(table)[kTabMask] = mask;
         st->seen = idx + 1;
-        st->skip = kSkipPerGroup;
+        st->skip = per_group ? kSkipPerGroup : 0;
         st->step = step;
         const double bc1 = 1.0 - pow(beta1, (double)step), bc2 = 1.0 - pow(beta2, (double)step);
         st->lr_over_bc1 = (float)(scheduled_lr(tab.g[0], idx) / bc1);
@@ -370,65 +324,7 @@ extern "C" int b200_adam_step(long long numel, float *param, float *grad, float 
 
 extern "C" size_t b200_adam_state_bytes(void) { return sizeof(AdamState); }
 
-// Once per optimisation step, before the first b200_adam_step_state of that step.  `state` = DEVICE, b200_adam_state_bytes()
-// bytes, zero-initialised by the caller before the first step.  veto_flag (DEVICE int32, may be null): non-zero = this
-// step's render was incomplete (b200_bin_cull_emit_capacity status[0], reduced with MAX across ranks by a data-parallel
-// caller): the step is skipped and the flag cleared.  state int32 words [2] step, [4] steps seen, [5] steps vetoed,
-// [6..15] ring of vetoed step indices let the host find out later which images to repeat.
-extern "C" int b200_adam_prepare(void *state, int32_t *veto_flag, double lr, double beta1, double beta2, void *stream) {
-    B200_REQUIRE(state, "null state");
-    B200_REQUIRE(beta1 >= 0.0 && beta1 < 1.0 && beta2 >= 0.0 && beta2 < 1.0, "betas must lie in [0, 1)");
-    adam_prepare_kernel<<<1, 32, 0, as_stream(stream)>>>(static_cast<AdamState *>(state), veto_flag, lr, beta1, beta2);
-    B200_LAUNCH_CHECK();
-    return B200_OK;
-}
-
-// b200_adam_step with the step count / bias corrections / veto read from the device state prepared above.
-static int adam_state_launch(long long numel, float *param, float *grad, float *exp_avg, float *exp_avg_sq, const void *state,
-                             double beta1, double beta2, double eps, double grad_scale, int zero_grad, long long max_blocks,
-                             void *stream) {
-    B200_REQUIRE(numel >= 0, "numel must be >= 0");
-    if (numel == 0) return B200_OK;
-    B200_REQUIRE(param && grad && exp_avg && exp_avg_sq && state, "null pointer");
-    const uintptr_t mis = reinterpret_cast<uintptr_t>(param) & 15u;
-    B200_REQUIRE(mis == 0 && (reinterpret_cast<uintptr_t>(grad) & 15u) == 0 && (reinterpret_cast<uintptr_t>(exp_avg) & 15u) == 0 &&
-                     (reinterpret_cast<uintptr_t>(exp_avg_sq) & 15u) == 0,
-                 "the slice must start on a 16-byte boundary of the four buffers");
-    AdamArgs a;
-    a.lr_over_bc1 = 0.f; a.inv_sqrt_bc2 = 0.f;
-    a.one_minus_beta1 = (float)(1.0 - beta1); a.beta2 = (float)beta2; a.one_minus_beta2 = (float)(1.0 - beta2);
-    a.eps = (float)eps; a.grad_scale = (float)grad_scale; a.zero_grad = zero_grad ? 1 : 0;
-    const long long n4 = numel >> 2;
-    long long want = (n4 + ADAM_THREADS - 1) / ADAM_THREADS;
-    const int blocks = (int)(want < 1 ? 1 : (want > max_blocks ? max_blocks : want));
-    adam_state_kernel<<<blocks, ADAM_THREADS, 0, as_stream(stream)>>>(numel, param, grad, exp_avg, exp_avg_sq, a,
-                                                                     static_cast<const AdamState *>(state));
-    B200_LAUNCH_CHECK();
-    return B200_OK;
-}
-
-extern "C" int b200_adam_step_state(long long numel, float *param, float *grad, float *exp_avg, float *exp_avg_sq,
-                                    const void *state, double beta1, double beta2, double eps, double grad_scale,
-                                    int zero_grad, void *stream) {
-    return adam_state_launch(numel, param, grad, exp_avg, exp_avg_sq, state, beta1, beta2, eps, grad_scale, zero_grad, 1ll << 30,
-                             stream);
-}
-
-// The same update as a BACKGROUND kernel: at most ctas_per_sm resident CTAs per SM looping over the slice, so that
-// kernels launched beside it on other streams (whatever their priority; memset nodes of a captured graph carry none)
-// always find free thread slots instead of queueing behind a grid of thousands of short CTAs.
-extern "C" int b200_adam_step_state_background(long long numel, float *param, float *grad, float *exp_avg, float *exp_avg_sq,
-                                               const void *state, double beta1, double beta2, double eps, double grad_scale,
-                                               int zero_grad, int ctas_per_sm, void *stream) {
-    B200_REQUIRE(ctas_per_sm >= 1 && ctas_per_sm <= 32, "ctas_per_sm must be in [1, 32]");
-    int dev = 0, sms = 0;
-    B200_CUDA(cudaGetDevice(&dev));
-    B200_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    return adam_state_launch(numel, param, grad, exp_avg, exp_avg_sq, state, beta1, beta2, eps, grad_scale, zero_grad,
-                             (long long)sms * ctas_per_sm, stream);
-}
-
-// ---- per-group learning rates: host side ---------------------------------------------------------------------------
+// ---- device-resident step state: host side ---------------------------------------------------------------------
 static int lr_table(int n_groups, const double *groups, LrTable &tab) {
     B200_REQUIRE(n_groups >= 1 && n_groups <= B200_ADAM_MAX_GROUPS, "n_groups must be in [1, B200_ADAM_MAX_GROUPS]");
     B200_REQUIRE(groups, "null group table");
@@ -450,23 +346,9 @@ static int lr_table(int n_groups, const double *groups, LrTable &tab) {
     return B200_OK;
 }
 
-extern "C" int b200_adam_prepare_groups(void *state, int32_t *veto_flag, int n_groups, const double *groups, double beta1,
-                                        double beta2, float *group_lr, void *stream) {
-    B200_REQUIRE(state && group_lr, "null state or group_lr");
-    B200_REQUIRE(beta1 >= 0.0 && beta1 < 1.0 && beta2 >= 0.0 && beta2 < 1.0, "betas must lie in [0, 1)");
-    LrTable tab;
-    const int rc = lr_table(n_groups, groups, tab);
-    if (rc != B200_OK) return rc;
-    adam_prepare_groups_kernel<<<1, 32, 0, as_stream(stream)>>>(static_cast<AdamState *>(state), veto_flag, beta1, beta2,
-                                                                tab, group_lr);
-    B200_LAUNCH_CHECK();
-    return B200_OK;
-}
-
-extern "C" int b200_adam_prepare_groups_masked(void *state, int32_t *veto_flag, const int32_t *detached,
-                                               unsigned detached_groups, int cond_group, int cond_every, int n_groups,
-                                               const double *groups, double beta1, double beta2, float *group_table,
-                                               void *stream) {
+extern "C" int b200_adam_prepare_step(void *state, int32_t *veto_flag, const int32_t *detached, unsigned detached_groups,
+                                      int cond_group, int cond_every, int n_groups, const double *groups, double beta1,
+                                      double beta2, float *group_table, void *stream) {
     B200_REQUIRE(state && group_table, "null state or group_table");
     B200_REQUIRE(beta1 >= 0.0 && beta1 < 1.0 && beta2 >= 0.0 && beta2 < 1.0, "betas must lie in [0, 1)");
     B200_REQUIRE(cond_group < n_groups, "cond_group must be < n_groups (or negative: none)");
@@ -475,18 +357,22 @@ extern "C" int b200_adam_prepare_groups_masked(void *state, int32_t *veto_flag, 
     LrTable tab;
     const int rc = lr_table(n_groups, groups, tab);
     if (rc != B200_OK) return rc;
-    adam_prepare_groups_masked_kernel<<<1, 32, 0, as_stream(stream)>>>(static_cast<AdamState *>(state), veto_flag, detached,
-                                                                       detached_groups, cond_group < 0 ? -1 : cond_group,
-                                                                       cond_every < 1 ? 1 : cond_every, beta1, beta2, tab,
-                                                                       group_table);
+    adam_prepare_step_kernel<<<1, 32, 0, as_stream(stream)>>>(static_cast<AdamState *>(state), veto_flag, detached,
+                                                              detached_groups, cond_group < 0 ? -1 : cond_group,
+                                                              cond_every < 1 ? 1 : cond_every, beta1, beta2, tab,
+                                                              group_table);
     B200_LAUNCH_CHECK();
     return B200_OK;
 }
 
-static int adam_groups_launch(long long numel, long long offset, float *param, float *grad, float *exp_avg, float *exp_avg_sq,
-                              int n_segments, const long long *segments, const void *state, const float *group_lr,
-                              double beta1, double beta2, double eps, double grad_scale, int zero_grad, long long max_blocks,
-                              void *stream) {
+// ctas_per_sm > 0 runs the update as a BACKGROUND kernel: at most ctas_per_sm resident CTAs per SM loop over the slice, so
+// that kernels launched beside it on other streams (whatever their priority; memset nodes of a captured graph carry none)
+// always find free thread slots instead of queueing behind a grid of thousands of short CTAs.
+extern "C" int b200_adam_update(long long numel, long long offset, float *param, float *grad, float *exp_avg,
+                                float *exp_avg_sq, int n_segments, const long long *segments, const void *state,
+                                const float *group_table, double beta1, double beta2, double eps, double grad_scale,
+                                int zero_grad, int ctas_per_sm, void *stream) {
+    B200_REQUIRE(ctas_per_sm >= 0 && ctas_per_sm <= 32, "ctas_per_sm must be in [0, 32]");
     B200_REQUIRE(numel >= 0 && offset >= 0, "numel and offset must be >= 0");
     B200_REQUIRE(n_segments >= 0 && n_segments <= B200_ADAM_MAX_SEGMENTS, "n_segments must be in [0, B200_ADAM_MAX_SEGMENTS]");
     B200_REQUIRE(n_segments == 0 || segments, "null segment table");
@@ -504,7 +390,7 @@ static int adam_groups_launch(long long numel, long long offset, float *param, f
         S.begin = w[0]; S.end = w[1]; S.period = (int)w[2]; S.split = (int)w[3]; S.ga = (int)w[4]; S.gb = (int)w[5];
     }
     if (numel == 0) return B200_OK;
-    B200_REQUIRE(param && grad && exp_avg && exp_avg_sq && state && group_lr, "null pointer");
+    B200_REQUIRE(param && grad && exp_avg && exp_avg_sq && state && (n_segments == 0 || group_table), "null pointer");
     B200_REQUIRE(((reinterpret_cast<uintptr_t>(param) | reinterpret_cast<uintptr_t>(grad) | reinterpret_cast<uintptr_t>(exp_avg) |
                    reinterpret_cast<uintptr_t>(exp_avg_sq)) & 15u) == 0,
                  "the slice must start on a 16-byte boundary of the four buffers");
@@ -512,32 +398,22 @@ static int adam_groups_launch(long long numel, long long offset, float *param, f
     a.lr_over_bc1 = 0.f; a.inv_sqrt_bc2 = 0.f;
     a.one_minus_beta1 = (float)(1.0 - beta1); a.beta2 = (float)beta2; a.one_minus_beta2 = (float)(1.0 - beta2);
     a.eps = (float)eps; a.grad_scale = (float)grad_scale; a.zero_grad = zero_grad ? 1 : 0;
+    long long max_blocks = 1ll << 30;
+    if (ctas_per_sm > 0) {
+        int dev = 0, sms = 0;
+        B200_CUDA(cudaGetDevice(&dev));
+        B200_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+        max_blocks = (long long)sms * ctas_per_sm;
+    }
     const long long n4 = numel >> 2;
     long long want = (n4 + ADAM_THREADS - 1) / ADAM_THREADS;
     const int blocks = (int)(want < 1 ? 1 : (want > max_blocks ? max_blocks : want));
-    adam_groups_kernel<<<blocks, ADAM_THREADS, 0, as_stream(stream)>>>(numel, offset, param, grad, exp_avg, exp_avg_sq, a,
-                                                                      static_cast<const AdamState *>(state), group_lr, segs);
+    const AdamState *st = static_cast<const AdamState *>(state);
+    if (n_segments == 0)
+        adam_state_kernel<<<blocks, ADAM_THREADS, 0, as_stream(stream)>>>(numel, param, grad, exp_avg, exp_avg_sq, a, st);
+    else
+        adam_groups_kernel<<<blocks, ADAM_THREADS, 0, as_stream(stream)>>>(numel, offset, param, grad, exp_avg, exp_avg_sq,
+                                                                          a, st, group_table, segs);
     B200_LAUNCH_CHECK();
     return B200_OK;
-}
-
-extern "C" int b200_adam_step_state_groups(long long numel, long long offset, float *param, float *grad, float *exp_avg,
-                                           float *exp_avg_sq, int n_segments, const long long *segments, const void *state,
-                                           const float *group_lr, double beta1, double beta2, double eps, double grad_scale,
-                                           int zero_grad, void *stream) {
-    return adam_groups_launch(numel, offset, param, grad, exp_avg, exp_avg_sq, n_segments, segments, state, group_lr, beta1,
-                              beta2, eps, grad_scale, zero_grad, 1ll << 30, stream);
-}
-
-extern "C" int b200_adam_step_state_groups_background(long long numel, long long offset, float *param, float *grad,
-                                                      float *exp_avg, float *exp_avg_sq, int n_segments,
-                                                      const long long *segments, const void *state, const float *group_lr,
-                                                      double beta1, double beta2, double eps, double grad_scale, int zero_grad,
-                                                      int ctas_per_sm, void *stream) {
-    B200_REQUIRE(ctas_per_sm >= 1 && ctas_per_sm <= 32, "ctas_per_sm must be in [1, 32]");
-    int dev = 0, sms = 0;
-    B200_CUDA(cudaGetDevice(&dev));
-    B200_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    return adam_groups_launch(numel, offset, param, grad, exp_avg, exp_avg_sq, n_segments, segments, state, group_lr, beta1,
-                              beta2, eps, grad_scale, zero_grad, (long long)sms * ctas_per_sm, stream);
 }

@@ -58,15 +58,8 @@ SIGNATURES = {
                                      _p, _p, _p, _p, _p, _p, _p, _p]),
     "b200_adam_step": (_i, [C.c_longlong, _p, _p, _p, _p, _i, _d, _d, _d, _d, _d, _i, _p]),
     "b200_adam_state_bytes": (_sz, []),
-    "b200_adam_prepare": (_i, [_p, _p, _d, _d, _d, _p]),
-    "b200_adam_step_state": (_i, [C.c_longlong, _p, _p, _p, _p, _p, _d, _d, _d, _d, _i, _p]),
-    "b200_adam_step_state_background": (_i, [C.c_longlong, _p, _p, _p, _p, _p, _d, _d, _d, _d, _i, _i, _p]),
-    "b200_adam_prepare_groups": (_i, [_p, _p, _i, _p, _d, _d, _p, _p]),
-    "b200_adam_step_state_groups": (_i, [C.c_longlong, C.c_longlong, _p, _p, _p, _p, _i, _p, _p, _p, _d, _d, _d, _d, _i,
-                                         _p]),
-    "b200_adam_step_state_groups_background": (_i, [C.c_longlong, C.c_longlong, _p, _p, _p, _p, _i, _p, _p, _p, _d, _d,
-                                                    _d, _d, _i, _i, _p]),
-    "b200_adam_prepare_groups_masked": (_i, [_p, _p, _p, _u, _i, _i, _i, _p, _d, _d, _p, _p]),
+    "b200_adam_prepare_step": (_i, [_p, _p, _p, _u, _i, _i, _i, _p, _d, _d, _p, _p]),
+    "b200_adam_update": (_i, [C.c_longlong, C.c_longlong, _p, _p, _p, _p, _i, _p, _p, _p, _d, _d, _d, _d, _i, _i, _p]),
     "b200_detached_grad_rows": (_i, [_p, _i, _p, _p, _p]),
     "b200_bin_cull_emit_capacity": (_i, [_i, _i, _p, _p, _p, _u, _u, _u, _u, _f, _f, _p, _p, _sz, _p, _p, _p, _p]),
     "b200_blend_forward_packed_status": (_i, [_u, _u, _u, _u, _p, _p, _p, _f, _f, _p, _p, _p, _p, _p, _p, _p]),

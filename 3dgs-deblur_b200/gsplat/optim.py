@@ -9,8 +9,8 @@ instead of a Python optimizer round trip per slice.  CUDA only.
 
 Per-group learning rates: Splatfacto gives every parameter group its own rate, and the means and camera-velocity groups a
 schedule (`splatfacto_lr`).  `group_segments` maps the flat layout to those groups, and `FlatAdam.use_device_state(groups=
-...)` + `set_groups(segments)` switch to the grouped device-state kernels (b200_adam_prepare_groups,
-b200_adam_step_state_groups), which give every element its own group's rate in the same single pass."""
+...)` + `set_groups(segments)` switch the device-state update (b200_adam_prepare_step, b200_adam_update) to the grouped
+kernel, which gives every element its own group's rate in the same single pass."""
 import math
 
 import numpy as np
@@ -169,34 +169,36 @@ class FlatAdam:
         self.exp_avg_sq = torch.zeros_like(flat)
         self.lr, self.betas, self.eps = float(lr), (float(betas[0]), float(betas[1])), float(eps)
         self.step_count = 0
+        self.state = self.groups = self._mask = None
         self._ptrs = (flat.data_ptr(), flat_grad.data_ptr(), self.exp_avg.data_ptr(), self.exp_avg_sq.data_ptr())
         self._lib = _lib.load()
 
     # ---- device-resident step state (no host sync, CUDA-graph friendly) ------------------------------------------
     def use_device_state(self, groups=None):
-        """Switch to the device-resident step count / bias corrections / veto (b200_adam_prepare,
-        b200_adam_step_state): `prepare(veto_flag)` once per step, then `update_state(begin, end)` per slice.
+        """Switch to the device-resident step count / bias corrections / veto (b200_adam_prepare_step, b200_adam_update):
+        `prepare(veto_flag)` once per step, then `update_state(begin, end)` per slice.  Without groups, `lr` is one
+        constant group that every element uses.
         groups: a list of per-group rates (float = constant, or ExponentialDecay; group index = position) for the grouped
-        kernels; `set_groups(segments)` then says which flat elements belong to which group.  `group_lr` (device
+        kernel; `set_groups(segments)` then says which flat elements belong to which group.  `group_lr` (device
         float32[groups]) holds each group's lr / (1 - beta1^step) of the last prepared step."""
-        if getattr(self, "state", None) is None:
+        if self.state is None:
             nbytes = self._lib.b200_adam_state_bytes()
             self.state = torch.zeros(nbytes // 4, dtype=torch.int32, device=self.flat.device)
-        self.groups = self._mask = None
-        if groups is not None:
-            groups = list(groups)
-            if not 1 <= len(groups) <= MAX_GROUPS:
-                raise ValueError("FlatAdam: between 1 and 16 learning-rate groups (B200_ADAM_MAX_GROUPS)")
-            self._group_table = torch.tensor([_group_row(g) for g in groups], dtype=torch.float64)
-            self.groups = groups
-            self.group_lr = torch.zeros(len(groups), dtype=torch.float32, device=self.flat.device)
-            self._segments = torch.zeros((0, 6), dtype=torch.int64)
+        self.groups = None if groups is None else list(groups)
+        rates = [self.lr] if groups is None else self.groups
+        if not 1 <= len(rates) <= MAX_GROUPS:
+            raise ValueError("FlatAdam: between 1 and 16 learning-rate groups (B200_ADAM_MAX_GROUPS)")
+        self._rates = torch.tensor([_group_row(g) for g in rates], dtype=torch.float64)
+        self._table = torch.zeros(GROUP_TABLE_FLOATS, dtype=torch.float32, device=self.flat.device)
+        self.group_lr = self._table[:len(rates)]
+        self._segments = torch.zeros((0, 6), dtype=torch.int64)
+        self._mask = None
         return self
 
     def set_groups(self, segments):
         """The segment table of the grouped update: (begin, end, period, split, group_a, group_b) rows over GLOBAL flat
         indices, sorted and disjoint (group_segments builds it from a model).  Elements in no segment are not updated."""
-        if getattr(self, "groups", None) is None:
+        if self.groups is None:
             raise ValueError("FlatAdam.set_groups: call use_device_state(groups=...) first")
         segs = torch.tensor([list(map(int, s)) for s in segments], dtype=torch.int64).reshape(-1, 6)
         if segs.shape[0] > 16:
@@ -208,19 +210,19 @@ class FlatAdam:
     def learning_rates(self, step: int):
         """Each group's rate (float64) at schedule position `step` -- the index of a prepared step, vetoed ones included
         (PipelinedTrainer.steps) -- computed on the host, no device sync.  None without groups."""
-        if getattr(self, "groups", None) is None:
+        if self.groups is None:
             return None
         return [lr_at(g, int(step)) for g in self.groups]
 
     def use_group_masks(self, detached_groups, cond_group=None, cond_every: int = 10):
-        """Per-group step counts and per-step masks (b200_adam_prepare_groups_masked), for steps whose loss gives some
-        groups no gradient (Splatfacto's detached eval cameras: nerfstudio then skips those groups' optimizers, and torch's
-        Adam keeps their step counts).  After this, `prepare(veto_flag, detached)` with a non-zero device word `detached`
-        steps only the group indices in `detached_groups`, plus `cond_group` at steps whose index is a multiple of
-        `cond_every` (the scale regulariser's clock); every other group keeps its parameters, moments and step count.
-        With `detached` zero or None every group steps.  `group_lr` becomes the 64-float group table; `group_steps()`
-        reads the counts.  Needs use_device_state(groups=...)."""
-        if getattr(self, "groups", None) is None:
+        """Per-group step counts and per-step masks, for steps whose loss gives some groups no gradient (Splatfacto's
+        detached eval cameras: nerfstudio then skips those groups' optimizers, and torch's Adam keeps their step counts).
+        After this, `prepare(veto_flag, detached)` with a non-zero device word `detached` steps only the group indices in
+        `detached_groups`, plus `cond_group` at steps whose index is a multiple of `cond_every` (the scale regulariser's
+        clock); every other group keeps its parameters, moments and step count.  With `detached` zero or None every group
+        steps.  `group_lr` becomes the 64-float group table; `group_steps()` reads the counts.  Needs
+        use_device_state(groups=...)."""
+        if self.groups is None:
             raise ValueError("FlatAdam.use_group_masks: call use_device_state(groups=...) first")
         bits = 0
         for g in detached_groups:
@@ -231,69 +233,52 @@ class FlatAdam:
             raise ValueError(f"FlatAdam.use_group_masks: group index {cond_group} outside the group table")
         if int(cond_every) < 1:
             raise ValueError("FlatAdam.use_group_masks: cond_every must be >= 1")
-        table = torch.zeros(GROUP_TABLE_FLOATS, dtype=torch.float32, device=self.flat.device)
-        table[:len(self.groups)] = self.group_lr
-        self.group_lr = table
-        self._mask = (bits, -1 if cond_group is None else int(cond_group), int(cond_every))
+        self.group_lr = self._table
+        # the prepare keeps per-group counts only when it is given a word: prepare(veto, None) passes this zero one
+        self._mask = (bits, -1 if cond_group is None else int(cond_group), int(cond_every),
+                      torch.zeros(1, dtype=torch.int32, device=self.flat.device))
         return self
 
     def group_steps(self):
         """Steps each group has taken (host list; synchronises).  None without use_group_masks."""
-        if getattr(self, "_mask", None) is None:
+        if self._mask is None:
             return None
-        return self.group_lr[2 * MAX_GROUPS:2 * MAX_GROUPS + len(self.groups)].view(torch.int32).tolist()
+        return self._table[2 * MAX_GROUPS:2 * MAX_GROUPS + len(self.groups)].view(torch.int32).tolist()
 
     def prepare(self, veto_flag=None, detached=None):
         """Once per step, before the first `update_state`.  veto_flag: device int32[1] (or None); non-zero skips this step's
         update on the device (gradients are still cleared) and is reset to zero.  detached: device int32[1] (or None),
         read after use_group_masks only (see there)."""
-        veto = None if veto_flag is None else veto_flag.data_ptr()
+        if self._mask is not None:
+            bits, cond, every, no_detach = self._mask
+            detached = no_detach if detached is None else detached
+        elif detached is not None:
+            raise ValueError("FlatAdam.prepare: a detached word needs use_group_masks")
+        else:
+            bits, cond, every = 0, -1, 1
         with _lib.on_device(self.flat.device):
-            if getattr(self, "_mask", None) is not None:
-                bits, cond, every = self._mask
-                check(self._lib.b200_adam_prepare_groups_masked(
-                    self.state.data_ptr(), veto, None if detached is None else detached.data_ptr(), bits, cond, every,
-                    len(self.groups), self._group_table.data_ptr(), self.betas[0], self.betas[1],
-                    self.group_lr.data_ptr(), stream()))
-            elif detached is not None:
-                raise ValueError("FlatAdam.prepare: a detached word needs use_group_masks")
-            elif getattr(self, "groups", None) is not None:
-                check(self._lib.b200_adam_prepare_groups(self.state.data_ptr(), veto, len(self.groups),
-                                                         self._group_table.data_ptr(), self.betas[0], self.betas[1],
-                                                         self.group_lr.data_ptr(), stream()))
-            else:
-                check(self._lib.b200_adam_prepare(self.state.data_ptr(), veto, self.lr, self.betas[0], self.betas[1],
-                                                  stream()))
+            check(self._lib.b200_adam_prepare_step(
+                self.state.data_ptr(), _lib.ptr(veto_flag), _lib.ptr(detached), bits, cond, every, self._rates.shape[0],
+                self._rates.data_ptr(), self.betas[0], self.betas[1], self._table.data_ptr(), stream()))
 
     def update_state(self, begin: int = 0, end: int = None, grad_scale: float = 1.0, zero_grad: bool = True,
                      background_ctas: int = 0):
-        """background_ctas > 0: run as a background kernel with that many resident CTAs per SM
-        (b200_adam_step_state_background) -- for an update queued on a second stream beside latency-bound kernels."""
+        """Every element at its own group's rate, or at `lr` without groups.  background_ctas > 0: run as a background
+        kernel with that many resident CTAs per SM -- for an update queued on a second stream beside latency-bound
+        kernels."""
         end = self.flat.numel() if end is None else end
         if not (0 <= begin <= end <= self.flat.numel()) or begin % 4:
             raise ValueError(f"FlatAdam.update_state: bad slice [{begin}, {end}) (must start on a 16-byte boundary)")
+        segs = self._segments
+        if self.groups is not None and not segs.shape[0]:
+            raise ValueError("FlatAdam.update_state: a grouped update needs set_groups(segments) with at least one segment")
         off = 4 * begin
         p, g, m, v = self._ptrs
-        if getattr(self, "groups", None) is not None:  # every element at its own group's rate
-            segs = self._segments
-            with _lib.on_device(self.flat.device):
-                args = (end - begin, begin, p + off, g + off, m + off, v + off, segs.shape[0], segs.data_ptr(),
-                        self.state.data_ptr(), self.group_lr.data_ptr(), self.betas[0], self.betas[1], self.eps,
-                        float(grad_scale), 1 if zero_grad else 0)
-                if background_ctas > 0:
-                    check(self._lib.b200_adam_step_state_groups_background(*args, int(background_ctas), stream()))
-                else:
-                    check(self._lib.b200_adam_step_state_groups(*args, stream()))
-            return
         with _lib.on_device(self.flat.device):
-            if background_ctas > 0:
-                check(self._lib.b200_adam_step_state_background(
-                    end - begin, p + off, g + off, m + off, v + off, self.state.data_ptr(), self.betas[0], self.betas[1],
-                    self.eps, float(grad_scale), 1 if zero_grad else 0, int(background_ctas), stream()))
-            else:
-                check(self._lib.b200_adam_step_state(end - begin, p + off, g + off, m + off, v + off, self.state.data_ptr(),
-                                                     self.betas[0], self.betas[1], self.eps, float(grad_scale),
-                                                     1 if zero_grad else 0, stream()))
+            check(self._lib.b200_adam_update(end - begin, begin, p + off, g + off, m + off, v + off, segs.shape[0],
+                                             segs.data_ptr(), self.state.data_ptr(), self._table.data_ptr(), self.betas[0],
+                                             self.betas[1], self.eps, float(grad_scale), 1 if zero_grad else 0,
+                                             max(int(background_ctas), 0), stream()))
 
     def rebind(self, flat: torch.Tensor, flat_grad: torch.Tensor):
         """The parameter buffers were reallocated (densification): fresh zero moments of the new size; the caller fills them

@@ -691,83 +691,63 @@ B200_API int b200_adam_step(long long numel, float *param, float *grad, float *e
                             double lr, double beta1, double beta2, double eps, double grad_scale, int zero_grad,
                             void *stream);
 
-/* Device-resident optimizer state: the step count, the bias corrections and a per-step VETO live on the device, so a
- * trainer that never synchronises with the host (CUDA-graph replays, capacity-mode binning below) can still skip the
- * update of a step whose render turned out incomplete.  state: DEVICE, b200_adam_state_bytes() bytes, zeroed by the caller
- * before the first step; as int32 words: [2] optimizer steps applied, [3] current step vetoed (0/1), [4] steps prepared,
- * [5] steps vetoed, [6..15] indices (0-based, in `steps prepared` numbering) of the last 10 vetoed steps, slot = count % 10.
- *   b200_adam_prepare: once per step before the first update.  veto_flag: DEVICE int32 or null; non-zero = veto this step
- *       (a data-parallel caller reduces it with MAX across ranks first); it is cleared here.
- *   b200_adam_step_state: b200_adam_step with step / bias corrections / veto read from `state`; a vetoed step leaves
- *       param and moments untouched and still clears the gradient slice.  The slice must start 16-byte aligned. */
-B200_API size_t b200_adam_state_bytes(void);
-B200_API int b200_adam_prepare(void *state, int32_t *veto_flag, double lr, double beta1, double beta2, void *stream);
-B200_API int b200_adam_step_state(long long numel, float *param, float *grad, float *exp_avg, float *exp_avg_sq,
-                                  const void *state, double beta1, double beta2, double eps, double grad_scale,
-                                  int zero_grad, void *stream);
-/* The same update as a background kernel for a caller that runs it on a second stream beside latency-bound work: at most
- * ctas_per_sm (1..32) resident CTAs of 256 threads per SM loop over the slice, so kernels launched beside it always find
- * free thread slots instead of queueing behind a grid of thousands of short CTAs.  Same arithmetic, same result. */
-B200_API int b200_adam_step_state_background(long long numel, float *param, float *grad, float *exp_avg, float *exp_avg_sq,
-                                             const void *state, double beta1, double beta2, double eps, double grad_scale,
-                                             int zero_grad, int ctas_per_sm, void *stream);
-
-/* Per-group learning rates (Splatfacto steps one Adam per parameter group, each with its own rate and scheduler:
- * nerfstudio/configs/method_configs.py, the splatfacto optimizers).  Same state, same arithmetic; only lr differs.
- *   groups: HOST double[n_groups][B200_LR_GROUP_DOUBLES], read during the call and passed to the kernel by value (so it
- *       can be captured): {kind (0 constant, 1 exponential decay), lr_init, lr_final, lr_pre_warmup, warmup_steps,
- *       max_steps, ramp (0 cosine, 1 linear)}.  Kind 1 is nerfstudio's ExponentialDecayScheduler (engine/schedulers.py)
- *       under LambdaLR: lr_g(s) = lr_init * (func_lr(s) / lr_init), in double.  Kind 0 uses lr_init exactly.
- *   b200_adam_prepare_groups: b200_adam_prepare's state update (AdamState's lr_over_bc1 takes group 0's value), then
- *       group_lr[g] = (float)(lr_g(s) / (1 - beta1^step)) for every group: group_lr is DEVICE float[n_groups].  The
- *       schedule position s is the index of the step being prepared, vetoed steps included: `steps prepared` (word [4])
- *       before the increment.  Bias corrections count applied steps, as before.  A vetoed step leaves group_lr as it was.
- *   b200_adam_step_state_groups: b200_adam_step_state over numel floats whose first one is GLOBAL flat index `offset`;
- *       every element uses its own group's group_lr.  segments: HOST long long[n_segments][B200_ADAM_SEGMENT_WORDS],
- *       sorted and disjoint, by value like `groups`: {begin, end, period, split, group_a, group_b}.  Global index i in
- *       [begin, end) belongs to group_a when period == 0 or (i - begin) % period < split, else to group_b.  An element in
- *       no segment keeps its parameter and moments bit-unchanged; its gradient is still cleared.  A vetoed step moves
- *       nothing and clears the gradient slice.  The slice must start 16-byte aligned; it need not start or end on a
- *       segment boundary. */
+/* Device-resident Adam: the step count, the bias corrections, per-group learning rates and a per-step VETO live on the
+ * device, so a trainer that never synchronises with the host (CUDA-graph replays, capacity-mode binning below) can follow
+ * Splatfacto's schedules and still skip the update of a step whose render turned out incomplete.  Splatfacto steps one
+ * Adam per parameter group, each with its own rate and scheduler (nerfstudio/configs/method_configs.py, the splatfacto
+ * optimizers); a single rate is one constant group.  Same arithmetic as b200_adam_step.
+ *   state: DEVICE, b200_adam_state_bytes() bytes, zeroed by the caller before the first step; as int32 words: [2] optimizer
+ *       steps applied, [3] the current step: 0 one count for every group, 1 vetoed, 2 per-group counts; [4] steps
+ *       prepared, [5] steps vetoed, [6..15] indices (0-based, in `steps prepared` numbering) of the last 10 vetoed steps,
+ *       slot = count % 10.
+ *   group_table: DEVICE float[B200_ADAM_GROUP_TABLE_FLOATS], 16-byte aligned, zeroed by the caller before the first step:
+ *       [g] lr_g(s) / (1 - beta1^t_g), [16 + g] 1 / sqrt(1 - beta2^t_g), [32 + g] t_g (int32: steps group g has taken),
+ *       [48] the mask of the last prepared step (uint32, bit g = group g steps).  Without per-group counts only [g] is
+ *       written, with t_g = the steps applied.
+ *   b200_adam_prepare_step: once per step before the first update.  veto_flag: DEVICE int32 or null; non-zero = veto this
+ *       step (a data-parallel caller reduces it with MAX across ranks first); it is cleared here, and a vetoed step leaves
+ *       the group table as it was.  groups: HOST double[n_groups][B200_LR_GROUP_DOUBLES], read during the call and passed
+ *       to the kernel by value (so it can be captured): {kind (0 constant, 1 exponential decay), lr_init, lr_final,
+ *       lr_pre_warmup, warmup_steps, max_steps, ramp (0 cosine, 1 linear)}.  Kind 1 is nerfstudio's
+ *       ExponentialDecayScheduler (engine/schedulers.py) under LambdaLR: lr_g(s) = lr_init * (func_lr(s) / lr_init), in
+ *       double.  Kind 0 uses lr_init exactly.  The schedule position s is the index of the step being prepared, vetoed
+ *       steps included: word [4] before the increment.  The state's own bias corrections count applied steps, and its
+ *       lr / bc1 is group 0's.
+ *       detached: DEVICE int32 or null.  Null: every group steps at the count of applied steps (word [3] = 0).  Otherwise
+ *       each group keeps its own count t_g (word [3] = 2), for Splatfacto's detached eval cameras: nerfstudio steps an
+ *       optimizer only when one of its parameters has a gradient (engine/optimizers.py:158-171), and torch's Adam keeps a
+ *       step count per parameter.  *detached zero: every group steps.  Non-zero: only the groups of the bit mask
+ *       detached_groups step, and group cond_group as well when s is a multiple of cond_every (cond_group < 0: none).  A
+ *       group that steps advances t_g and gets new constants; the others keep both.
+ *   b200_adam_update: the update of numel floats whose first one is GLOBAL flat index `offset`; the slice must start
+ *       16-byte aligned.  A vetoed step moves nothing and clears the gradient slice.  n_segments == 0: every element uses
+ *       the state's constants.  n_segments > 0: every element uses its own group's constants from group_table.
+ *       segments: HOST long long[n_segments][B200_ADAM_SEGMENT_WORDS], sorted and disjoint, by value like `groups`:
+ *       {begin, end, period, split, group_a, group_b}.  Global index i in [begin, end) belongs to group_a when
+ *       period == 0 or (i - begin) % period < split, else to group_b.  An element in no segment, or in a group outside the
+ *       step's mask, keeps its parameter and moments bit-unchanged; its gradient is still cleared.  The slice need not
+ *       start or end on a segment boundary.  After a prepare with a `detached` word, pass the segment table: without one
+ *       the update reads word [3] = 2 as a veto.  ctas_per_sm: 0 = many short CTAs; 1..32 = a background kernel for a
+ *       caller that runs it on a second stream beside latency-bound work: at most ctas_per_sm resident CTAs of 256 threads
+ *       per SM loop over the slice, so kernels launched beside it always find free thread slots instead of queueing
+ *       behind a grid of thousands of short CTAs.  Same arithmetic, same result.
+ * b200_detached_grad_rows: when *detached (DEVICE int32) is non-zero, grad[i] = 0 for i in each [begin, end) of ranges
+ * (HOST long long[n_ranges][2], by value); otherwise nothing is touched.  The fused trainer clears the Gaussian and
+ * background rows of a detached image's gradient with it, after the backward and before the scale regulariser. */
 #define B200_ADAM_MAX_GROUPS 16
 #define B200_ADAM_MAX_SEGMENTS 16
 #define B200_LR_GROUP_DOUBLES 7
 #define B200_ADAM_SEGMENT_WORDS 6
-B200_API int b200_adam_prepare_groups(void *state, int32_t *veto_flag, int n_groups, const double *groups, double beta1,
-                                      double beta2, float *group_lr, void *stream);
-B200_API int b200_adam_step_state_groups(long long numel, long long offset, float *param, float *grad, float *exp_avg,
-                                         float *exp_avg_sq, int n_segments, const long long *segments, const void *state,
-                                         const float *group_lr, double beta1, double beta2, double eps, double grad_scale,
-                                         int zero_grad, void *stream);
-B200_API int b200_adam_step_state_groups_background(long long numel, long long offset, float *param, float *grad,
-                                                    float *exp_avg, float *exp_avg_sq, int n_segments,
-                                                    const long long *segments, const void *state, const float *group_lr,
-                                                    double beta1, double beta2, double eps, double grad_scale, int zero_grad,
-                                                    int ctas_per_sm, void *stream);
-
-/* Per-group step counts and per-step group masks (Splatfacto's detached eval cameras: nerfstudio steps an optimizer only
- * when one of its parameters has a gradient, engine/optimizers.py:158-171, and torch's Adam keeps a step count per
- * parameter, so a group without a gradient keeps its parameters, moments and step count).
- *   group_table: DEVICE float[B200_ADAM_GROUP_TABLE_FLOATS], 16-byte aligned, zeroed by the caller before the first step:
- *       [g] lr_g(s) / (1 - beta1^t_g), [16 + g] 1 / sqrt(1 - beta2^t_g), [32 + g] t_g (int32: steps group g has taken),
- *       [48] the mask of the last prepared step (uint32, bit g = group g steps).
- *   b200_adam_prepare_groups_masked: b200_adam_prepare_groups with each group's bias corrections counted by its own t_g.
- *       detached: DEVICE int32 or null.  Null or zero: every group steps.  Non-zero: only the groups of the bit mask
- *       detached_groups step, and group cond_group as well when the step index s (word [4] before the increment) is a
- *       multiple of cond_every (cond_group < 0: none).  A group that steps advances t_g and gets new constants; the others
- *       keep both.  The schedules stay on s.  A vetoed step vetoes every group, as before, and leaves the table alone.
- *       The state is marked (word [3] = 2) so that b200_adam_step_state_groups / _background, called with group_lr =
- *       group_table, give every element its own group's constants and leave the parameters and moments of a group outside
- *       the mask bit-unchanged while still clearing its gradient.  Use only the grouped update after this prepare.
- * b200_detached_grad_rows: when *detached (DEVICE int32) is non-zero, grad[i] = 0 for i in each [begin, end) of ranges
- * (HOST long long[n_ranges][2], by value); otherwise nothing is touched.  The fused trainer clears the Gaussian and
- * background rows of a detached image's gradient with it, after the backward and before the scale regulariser. */
 #define B200_ADAM_GROUP_TABLE_FLOATS 64
 #define B200_DETACHED_MAX_RANGES 4
-B200_API int b200_adam_prepare_groups_masked(void *state, int32_t *veto_flag, const int32_t *detached,
-                                             unsigned detached_groups, int cond_group, int cond_every, int n_groups,
-                                             const double *groups, double beta1, double beta2, float *group_table,
-                                             void *stream);
+B200_API size_t b200_adam_state_bytes(void);
+B200_API int b200_adam_prepare_step(void *state, int32_t *veto_flag, const int32_t *detached, unsigned detached_groups,
+                                    int cond_group, int cond_every, int n_groups, const double *groups, double beta1,
+                                    double beta2, float *group_table, void *stream);
+B200_API int b200_adam_update(long long numel, long long offset, float *param, float *grad, float *exp_avg,
+                              float *exp_avg_sq, int n_segments, const long long *segments, const void *state,
+                              const float *group_table, double beta1, double beta2, double eps, double grad_scale,
+                              int zero_grad, int ctas_per_sm, void *stream);
 B200_API int b200_detached_grad_rows(const int32_t *detached, int n_ranges, const long long *ranges, float *grad,
                                      void *stream);
 
@@ -777,7 +757,7 @@ B200_API int b200_detached_grad_rows(const int32_t *detached, int n_ranges, cons
  * mark instead: b200_bin_cull_count with totals_host_pinned = NULL, then b200_bin_cull_emit_capacity.  The id list has
  * `capacity` slots: the real entries in the reference's order, then padding that belongs to no tile.
  * status: DEVICE int32[4]: [0] |= 1 if this image's entries did not fit (lists incomplete: discard the render -- veto the
- * optimizer step with b200_adam_prepare, grow the capacity, repeat the image), [1] entries of this image, [2] running
+ * optimizer step with b200_adam_prepare_step, grow the capacity, repeat the image), [1] entries of this image, [2] running
  * maximum, [3] the reference's num_intersects of this image.  b200_blend_forward_packed_status = b200_blend_forward_packed
  * plus the reference's empty-render branch (rasterize.py:136-144: background image, final_Ts = 0, alpha = 1) taken on
  * the device when status[3] < 1.  b200_set_record_colors patches the colours of packed records (everything the binning
@@ -856,7 +836,7 @@ B200_API int b200_camera_l2(int num_rows, const float *rows, float w_a, float w_
  *   b200_background_vjp: g_logit[c] = (v_b[c] * (1 - background[c])) * background[c] with v_b[c] = sum_px v_rgb[px][c] *
  *       (sum_s final_Ts[px][s]) * (1 / n_samples), the reference's v_background (gsplat/rasterize.py:266-270) through the
  *       sigmoid; v_rgb (num_pixels, 3), final_Ts (num_pixels, n_samples).  g_logit (3 floats) is OVERWRITTEN.
- *   b200_scale_regularizer: when word [4] of adam_state (the b200_adam_prepare state: steps prepared so far, the index of
+ *   b200_scale_regularizer: when word [4] of adam_state (the b200_adam_prepare_step state: steps prepared so far, the index of
  *       the step whose loss this is) is a multiple of `every`, value[0] += weight * mean_i(max(r_i, max_ratio) - max_ratio)
  *       with r_i = amax_j(exp(log_scales[i][j])) / amin_j(exp(log_scales[i][j])) (splatfacto.py:968-977), and its
  *       gradient, torch's (ties split evenly, half the gradient at r_i == max_ratio), ADDED into g_log_scales

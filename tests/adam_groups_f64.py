@@ -1,7 +1,8 @@
-"""Float64 reference of the grouped device-state Adam (b200_adam_prepare_groups / b200_adam_step_state_groups).
-TEST INFRASTRUCTURE ONLY: the schedules are restated from nerfstudio's ExponentialDecayScheduler (engine/schedulers.py:
-92-141) under LambdaLR, the element -> group map from the segment semantics of include/b200splat.h, and the update is
-step_f64.adam (adam_one in float64 with its fp32 bound) applied group by group with each group's fp32 constant."""
+"""Float64 reference of the grouped device-state Adam (b200_adam_prepare_step, b200_adam_update with a segment
+table).  TEST INFRASTRUCTURE ONLY: the schedules are restated from nerfstudio's ExponentialDecayScheduler
+(engine/schedulers.py:92-141) under LambdaLR, the element -> group map from the segment semantics of
+include/b200splat.h, and the update is step_f64.adam (adam_one in float64 with its fp32 bound) applied group by group
+with each group's fp32 constant."""
 import numpy as np
 
 import step_f64 as SF

@@ -1,5 +1,5 @@
-"""Float64 reference of the masked grouped device-state Adam (b200_adam_prepare_groups_masked + the grouped update), the
-optimizer side of Splatfacto's detached eval cameras.  TEST INFRASTRUCTURE ONLY.
+"""Float64 reference of the masked grouped device-state Adam (b200_adam_prepare_step with a detached word + the grouped
+update), the optimizer side of Splatfacto's detached eval cameras.  TEST INFRASTRUCTURE ONLY.
 
 nerfstudio steps a group's torch Adam only when one of its parameters has a gradient (engine/optimizers.py:158-171); a
 group without one keeps its parameters, moments and step count.  So every group g carries its own count t_g, and a step

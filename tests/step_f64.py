@@ -305,7 +305,7 @@ def flat_grad(layout, vf, live, cam_index, modes, deg):
 # ---- Adam ---------------------------------------------------------------------------------------------------------------
 
 def adam_constants(step, lr, betas=BETAS, eps=EPS):
-    """The fp32 constants of one update: adam_prepare_kernel's bias corrections (formed in double) and AdamArgs."""
+    """The fp32 constants of one update: the prepare kernel's bias corrections (formed in double) and AdamArgs."""
     b1, b2 = betas
     bc1, bc2 = 1.0 - b1 ** step, 1.0 - b2 ** step
     f = P.f32

@@ -2,6 +2,7 @@
 allowance.
 
 1. One constant group over everything is bit-for-bit the single-rate update (vetoes, 16-byte pieces, background form).
+   A grouped update without a segment table, and a negative or non-finite single rate, raise.
 2. Splatfacto's per-group constants read back from the device are within 1 ulp of float64 across the schedules' turns.
 3. Every element's update is within step_f64.adam's bound at its group's device constant, both SH layouts.
 4. PipelinedTrainer(lr="splatfacto") against the float64 step reference (tests/test_gpu_trainer_f64.py's harness),
@@ -63,6 +64,21 @@ def test_one_constant_group_is_bitwise_the_single_rate_update():
             assert torch.equal(_bits(x), _bits(y)), f"step {step}"
         assert float(B.flat_grad.abs().max()) == 0.0
     assert int(A.state[2]) == 17 and int(A.state[4]) == 20 and int(A.state[5]) == 3
+
+
+def test_groups_without_segments_and_bad_single_rates_raise():
+    from gsplat.optim import FlatAdam
+
+    adam = FlatAdam(torch.zeros(16, device="cuda"), torch.zeros(16, device="cuda")).use_device_state(groups=[1e-3, 2e-3])
+    adam.prepare()
+    with pytest.raises(ValueError, match="set_groups"):  # an empty segment table would be the single-rate update
+        adam.update_state()
+    adam.set_groups([])
+    with pytest.raises(ValueError, match="set_groups"):
+        adam.update_state()
+    for lr in (-1e-3, float("nan"), float("inf")):
+        with pytest.raises(ValueError, match="learning rates"):
+            FlatAdam(torch.zeros(16, device="cuda"), torch.zeros(16, device="cuda"), lr=lr).use_device_state()
 
 
 # ---- 2 ---------------------------------------------------------------------------------------------------------------

@@ -1,10 +1,10 @@
 """GPU: detached eval cameras (3dgs-deblur's --optimize-eval-cameras) in the fused trainer, with no outlier allowance.
 
-1. The masked grouped Adam (b200_adam_prepare_groups_masked + b200_adam_step_state_groups) against tests/detached_f64.py
-   at sizes 1, 3, 4, 5, 255 and 257 with segment boundaries inside 16-byte vectors, masks that change every step, and
-   a veto on a masked step: stepping groups within step_f64.adam's bound at their own step counts, masked groups and
-   vetoed steps bit-unchanged, gradients cleared, per-group counts and constants as the restatement gives them.  With
-   no group ever masked the results are bitwise those of the unmasked entry points.
+1. The masked grouped Adam (b200_adam_prepare_step with a detached word, then b200_adam_update) against
+   tests/detached_f64.py at sizes 1, 3, 4, 5, 255 and 257 with segment boundaries inside 16-byte vectors, masks that
+   change every step, and a veto on a masked step: stepping groups within step_f64.adam's bound at their own step
+   counts, masked groups and vetoed steps bit-unchanged, gradients cleared, per-group counts and constants as the
+   restatement gives them.  With no group ever masked the results are bitwise those of the unmasked prepare.
 2. b200_detached_grad_rows clears its ranges exactly when the device word is set.
 3. PipelinedTrainer(detached_cameras={1}) with pose rows, velocity rows, the learned background and the scale regulariser
    at max_gauss_ratio 2 over 12 steps, eager, with graphs and deterministic: every after_backward gradient and loss held

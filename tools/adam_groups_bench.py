@@ -1,5 +1,6 @@
-"""Time the grouped device-state Adam (per-group rates, b200_adam_step_state_groups) against the single-rate update
-(b200_adam_step_state) over the trainer's flat buffer, and PipelinedTrainer with lr="splatfacto" against lr=1e-4.
+"""Time the grouped device-state Adam (per-group rates: b200_adam_update with a segment table) against the single-rate
+update (b200_adam_update without one) over the trainer's flat buffer, and PipelinedTrainer with lr="splatfacto" against
+lr=1e-4.
 
     python tools/adam_groups_bench.py [--rounds 3] [--out results.json]
 
