@@ -25,9 +25,16 @@ __device__ __forceinline__ void adam_one(float &p, float &g, float &m, float &v,
 
 constexpr int ADAM_THREADS = 256;
 
+// b200_adam_update's zero_grad for a step whose veto is `skip`: 1 clear, 0 keep.  B200_ADAM_CLEAR_ON_VETO keeps the
+// gradient of an applied step (a caller whose backward overwrites the slice every step skips the 4-byte store) and clears
+// that of a vetoed one, which leaves the buffer as a clearing update would have left it.
+__device__ __forceinline__ int clears(int zero_grad, bool skip) {
+    return zero_grad == B200_ADAM_CLEAR_ON_VETO ? (skip ? 1 : 0) : zero_grad;
+}
+
 // Device-resident optimizer state for a step the host never synchronises with (CUDA-graph replays, optimistic list
 // capacities): the step count and the bias corrections live on the device, and a step whose render was incomplete is
-// vetoed there -- parameters and moments stay, the gradient slice is still cleared.
+// vetoed there -- parameters and moments stay, the gradient slice is still cleared (unless zero_grad is 0).
 struct AdamState {
     float lr_over_bc1, inv_sqrt_bc2;
     int step;          // optimizer steps applied so far
@@ -43,6 +50,7 @@ __global__ void __launch_bounds__(ADAM_THREADS) adam_state_kernel(long long n, f
                                                                   const AdamState *__restrict__ st) {
     a.lr_over_bc1 = st->lr_over_bc1; a.inv_sqrt_bc2 = st->inv_sqrt_bc2;
     const bool skip = st->skip != 0;
+    a.zero_grad = clears(a.zero_grad, skip);
     const long long n4 = n >> 2;
     const long long stride = (long long)gridDim.x * blockDim.x;
     float4 *p4 = reinterpret_cast<float4 *>(p), *g4 = reinterpret_cast<float4 *>(g);
@@ -228,6 +236,7 @@ __global__ void __launch_bounds__(ADAM_THREADS) adam_groups_kernel(long long n, 
     a.inv_sqrt_bc2 = st->inv_sqrt_bc2;
     const int mode = st->skip;  // 0 one bias correction, kSkipVeto vetoed, kSkipPerGroup per-group counts and a mask
     const bool skip = mode == kSkipVeto, per_group = mode == kSkipPerGroup;
+    a.zero_grad = clears(a.zero_grad, skip);
     const unsigned mask = per_group ? __ldg(reinterpret_cast<const unsigned *>(group_lr) + kTabMask) : ~0u;
     const long long n4 = n >> 2;
     const long long stride = (long long)gridDim.x * blockDim.x;
@@ -373,6 +382,7 @@ extern "C" int b200_adam_update(long long numel, long long offset, float *param,
                                 const float *group_table, double beta1, double beta2, double eps, double grad_scale,
                                 int zero_grad, int ctas_per_sm, void *stream) {
     B200_REQUIRE(ctas_per_sm >= 0 && ctas_per_sm <= 32, "ctas_per_sm must be in [0, 32]");
+    B200_REQUIRE(zero_grad >= 0 && zero_grad <= B200_ADAM_CLEAR_ON_VETO, "zero_grad must be 0, 1 or B200_ADAM_CLEAR_ON_VETO");
     B200_REQUIRE(numel >= 0 && offset >= 0, "numel and offset must be >= 0");
     B200_REQUIRE(n_segments >= 0 && n_segments <= B200_ADAM_MAX_SEGMENTS, "n_segments must be in [0, B200_ADAM_MAX_SEGMENTS]");
     B200_REQUIRE(n_segments == 0 || segments, "null segment table");
@@ -397,7 +407,7 @@ extern "C" int b200_adam_update(long long numel, long long offset, float *param,
     AdamArgs a;
     a.lr_over_bc1 = 0.f; a.inv_sqrt_bc2 = 0.f;
     a.one_minus_beta1 = (float)(1.0 - beta1); a.beta2 = (float)beta2; a.one_minus_beta2 = (float)(1.0 - beta2);
-    a.eps = (float)eps; a.grad_scale = (float)grad_scale; a.zero_grad = zero_grad ? 1 : 0;
+    a.eps = (float)eps; a.grad_scale = (float)grad_scale; a.zero_grad = zero_grad;
     long long max_blocks = 1ll << 30;
     if (ctas_per_sm > 0) {
         int dev = 0, sms = 0;

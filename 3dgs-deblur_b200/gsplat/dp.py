@@ -429,8 +429,16 @@ def fused_geometry_phase(model: FlatGaussians, st: Dict, scene: Dict, capacity: 
     normalisation, projection, sigmoid * compensation, blend record -- what `geometry_phase` spends 11 launches on, 8 of
     them PyTorch glue) + the capacity-mode binning.  Same interface and the same numbers as `geometry_phase` up to
     float rounding of the activations.  No autograd graph: `fused_shading_phase` differentiates with
-    b200_fused_preprocess_backward.  rasterize_mode as in `geometry_phase` (b200_fused_geometry_forward_mode)."""
-    import gsplat.cuda as _C
+    b200_fused_preprocess_backward.  rasterize_mode as in `geometry_phase` (b200_fused_geometry_forward_mode).
+    The two halves are `fused_projection_phase` and `fused_binning_phase`."""
+    geo = fused_projection_phase(model, st, scene, rasterize_mode, color_mode)
+    return fused_binning_phase(geo, scene, capacity, status)
+
+
+def fused_projection_phase(model: FlatGaussians, st: Dict, scene: Dict, rasterize_mode: str = "antialiased",
+                           color_mode: str = "sh"):
+    """The first half of `fused_geometry_phase`: the camera of the step and the geometry kernel's records (colours left
+    for `fused_colors`), depths, radii and tile counts."""
     from gsplat import _lib
     from gsplat._lib import check, ptr, stream
 
@@ -463,24 +471,59 @@ def fused_geometry_phase(model: FlatGaussians, st: Dict, scene: Dict, capacity: 
                 check(lib.b200_fused_geometry_forward_mode(mode, *args))
             else:
                 check(lib.b200_fused_geometry_forward(*args))
-            ids, bins = _C.bin_cull_capacity(packed, depths, radii, nth, H, W, bw, blur, rs, ex, capacity, status)
-    return dict(packed=packed, depths=depths, radii=radii, num_tiles_hit=nth, ids=ids, bins=bins, vel=vel, cam=cam,
-                cam_in=cam_in, cam_index=st["cam_index"], status=status, blur=blur, absgrad=None)
+    return dict(packed=packed, depths=depths, radii=radii, num_tiles_hit=nth, vel=vel, cam=cam, cam_in=cam_in,
+                cam_index=st["cam_index"], blur=blur, absgrad=None)
+
+
+def fused_binning_phase(geo: Dict, scene: Dict, capacity: int, status: torch.Tensor):
+    """The second half of `fused_geometry_phase`: the capacity-mode tile lists of `fused_projection_phase`'s records
+    (the binning reads every record field but the colours), added to `geo`."""
+    import gsplat.cuda as _C
+    from gsplat import _lib
+
+    H, W, bw = scene["H"], scene["W"], scene["block_width"]
+    rs, ex = float(scene["rolling_shutter_time"]), float(scene["exposure_time"])
+    with torch.no_grad(), _lib.on_device(geo["packed"].device):
+        geo["ids"], geo["bins"] = _C.bin_cull_capacity(geo["packed"], geo["depths"], geo["radii"], geo["num_tiles_hit"], H,
+                                                       W, bw, geo["blur"], rs, ex, capacity, status)
+    geo["status"] = status
+    return geo
+
+
+def fused_colors(model: FlatGaussians, geo: Dict, sh_degree_to_use: int = 3, rasterize_mode: str = "antialiased",
+                 color_mode: str = "sh"):
+    """The colours of the records of `fused_projection_phase` (b200_fused_colors_forward): clamp(SH + 0.5, 0) of every
+    Gaussian with radius > 0 at the step's camera position, or sigmoid(sh_dc) with color_mode "sigmoid"."""
+    from gsplat import _lib
+    from gsplat._lib import check, ptr, stream
+
+    p = model.params
+    mode = _lib.render_mode(rasterize_mode, color_mode, "fused_colors")
+    if mode & _lib.COLOR_SIGMOID:
+        sh_degree_to_use = 0  # sigmoid(sh_dc) reads no SH basis
+    lib = _lib.load()
+    with torch.no_grad(), _lib.on_device(model.flat.device):
+        args = (model.N, ptr(p["means"]), ptr(p["sh_dc"]), ptr(p["sh_rest"]), model.K, sh_degree_to_use,
+                ptr(geo["cam"][18:21]), ptr(geo["radii"]), ptr(geo["packed"]), stream())
+        if mode:
+            check(lib.b200_fused_colors_forward_mode(mode, *args))
+        else:
+            check(lib.b200_fused_colors_forward(*args))
 
 
 def fused_shading_phase(model: FlatGaussians, geo: Dict, scene: Dict, target: torch.Tensor, loss_fn, sh_degree_to_use: int = 3,
-                        rasterize_mode: str = "antialiased", color_mode: str = "sh"):
-    """Phase B on the C ABI: SH colours into the records (b200_fused_colors_forward), blend, `loss_fn` (autograd sees
-    only loss_fn(rgb, target)), blend backward, and ONE kernel for everything behind it (b200_fused_preprocess_backward:
-    SH, clamp, sigmoid * compensation, projection VJP, exp, normalisation) that writes the model's flat gradient buffer
-    row by row -- no accumulate passes, no memsets.  The gradient rows are OVERWRITTEN (the buffer is zero between steps:
-    FlatAdam clears what it consumes); the camera-velocity row is accumulated.  The two render modes as in
-    `geometry_phase` / `shading_phase`, through the _mode entry points.  A model with `learnable_bg` blends over
+                        rasterize_mode: str = "antialiased", color_mode: str = "sh", colors: bool = True):
+    """Phase B on the C ABI: SH colours into the records (`fused_colors`; colors=False: the caller has written them),
+    blend, `loss_fn` (autograd sees only loss_fn(rgb, target)), blend backward, and ONE kernel for everything behind it
+    (b200_fused_preprocess_backward: SH, clamp, sigmoid * compensation, projection VJP, exp, normalisation) that writes
+    the model's flat gradient buffer row by row -- no accumulate passes, no memsets.  Every Gaussian row is OVERWRITTEN,
+    zeros included; the camera-velocity row is accumulated (the caller clears it between steps).  The two render modes
+    as in `geometry_phase` / `shading_phase`, through the _mode entry points.  A model with `learnable_bg` blends over
     sigmoid(learnable_bg) (geo["background"], written on the device) and writes the logit's gradient
     (gsplat.background)."""
     import gsplat.cuda as _C
     from gsplat import _lib
-    from gsplat._lib import check, ptr, stream
+    from gsplat._lib import ptr
 
     if model.sh_layout != "split":
         raise ValueError("fused_shading_phase reads sh_dc / sh_rest apart: build the model with sh_layout='split'")
@@ -492,23 +535,18 @@ def fused_shading_phase(model: FlatGaussians, geo: Dict, scene: Dict, target: to
     cam, vel, packed, radii = geo["cam"], geo["vel"], geo["packed"], geo["radii"]
     cam_pos = cam[18:21]
     bg = scene["background"]
-    lib = _lib.load()
     if model.learnable_bg is not None:  # the blend's background is sigmoid(learnable_bg), computed on the device
         from gsplat.background import background_forward_, background_vjp_
         with _lib.on_device(dev):
             bg = torch.empty(3, dtype=torch.float32, device=dev)
             background_forward_(model.learnable_bg.detach(), bg)
         geo["background"] = bg
+    if colors:
+        fused_colors(model, geo, sh_degree_to_use, rasterize_mode, color_mode)
     mode = _lib.render_mode(rasterize_mode, color_mode, "fused_shading_phase")
     if mode & _lib.COLOR_SIGMOID:
         sh_degree_to_use = 0  # sigmoid(sh_dc) reads no SH basis
     with torch.no_grad(), _lib.on_device(dev):
-        args = (n, ptr(p["means"]), ptr(p["sh_dc"]), ptr(p["sh_rest"]), K, sh_degree_to_use, ptr(cam_pos), ptr(radii),
-                ptr(packed), stream())
-        if mode:
-            check(lib.b200_fused_colors_forward_mode(mode, *args))
-        else:
-            check(lib.b200_fused_colors_forward(*args))
         rgb, Ts, fi, visits = _C.blend_forward_packed(H, W, bw, S, geo["ids"], geo["bins"], packed, rs, ex, bg,
                                                       status=geo["status"], record=True)
     from gsplat.losses import l1_loss, l1_loss_and_grad
@@ -709,6 +747,15 @@ class PipelinedTrainer:
         modes = dict(rasterize_mode=rasterize_mode, color_mode=color_mode)
         self.geometry_fn = geometry_fn or functools.partial(phases[0], **modes)  # (tests inject CPU stand-ins with the
         self.shading_fn = shading_fn or functools.partial(phases[1], **modes)     # same interface)
+        # The trainer's own fused phases: A runs as projection + binning and the records' colours are written between
+        # them, behind the SH update on `side`, so that B starts with the blend; and as the fused backward overwrites every
+        # Gaussian gradient row, the update clears only the rows added into (camera, background) -- and everything on a
+        # vetoed step.
+        self._own_fused = (operators == "fused" and geometry_fn is None and shading_fn is None and optimizer == "b200"
+                           and model.flat.device.type == "cuda")
+        if self._own_fused:
+            self.shading_fn = functools.partial(fused_shading_phase, colors=False, **modes)
+        self._grads_left = False  # the last update left Gaussian gradient rows for the next backward to overwrite
         self.distributed = dist.is_available() and dist.is_initialized() and dist.get_world_size(group) > 1
         self.group = group
         self.rank = dist.get_rank(group) if self.distributed else 0
@@ -738,8 +785,10 @@ class PipelinedTrainer:
         self._flag_work = None
         self._pending_sh = None
         self.optimizer = optimizer
-        # SH update launch shape: 0 = one short CTA per 256 vectors (default), > 0 = that many resident CTAs per SM
-        self.sh_update_ctas = int(os.environ.get("B200_SH_UPDATE_CTAS", "0"))
+        # SH update launch shape: 0 = one short CTA per 256 vectors, > 0 = that many resident CTAs per SM.  The update has
+        # slack beside the next image's binning (it ends ~100 us before it on one H100), so it runs as one resident CTA
+        # per SM by default: it then takes less of the bandwidth and the SMs the binning kernels need (DESIGN 5.7)
+        self.sh_update_ctas = int(os.environ.get("B200_SH_UPDATE_CTAS", "1"))
         self.sh_update_pieces = int(os.environ.get("B200_SH_UPDATE_PIECES", "8"))
         # the SH block is exchanged in `sh_chunks` pieces so that the update of piece i runs while piece i+1 is on the wire
         self._cut_sh(max(1, int(sh_chunks)) if self.distributed else 1)
@@ -790,6 +839,7 @@ class PipelinedTrainer:
             self.side = torch.cuda.Stream(device=dev, priority=0)
             model.rebind_leaves()  # gradient accumulators are (re)created on `main` by the first step
             self.ev_prepared, self.ev_sh_done, self.ev_poll = torch.cuda.Event(), torch.cuda.Event(), torch.cuda.Event()
+            self.ev_projected = torch.cuda.Event()
             self._host_words = torch.zeros(2, 24, dtype=torch.int32).pin_memory()   # status (4) | adam state (16) | quat flag
             self._host_ev = [torch.cuda.Event(), torch.cuda.Event()]
             self._host_seen = [False, False]
@@ -888,34 +938,75 @@ class PipelinedTrainer:
         from gsplat import _lib
         return _lib.load().b200_launch_count() if self.cuda else 0
 
-    def _run_A(self, e):
+    def _A_parts(self):
+        """Phase A as the pieces it is run and captured in: the geometry function, or with the trainer's own fused phases
+        the projection and the binning, so that the records' colours (`_colors`) can be written between them."""
+        if not self._own_fused:
+            return (lambda geo: self.geometry_fn(self.model, self.st, self.scene, self.capacity, self.status),)
+        modes = dict(rasterize_mode=self.rasterize_mode, color_mode=self.color_mode)
+        return (lambda geo: fused_projection_phase(self.model, self.st, self.scene, **modes),
+                lambda geo: fused_binning_phase(geo, self.scene, self.capacity, self.status))
+
+    def _run_A(self, e, colors_on=None):
         if self.use_graphs and e["gA"] is not None:
-            e["gA"].replay()
+            for k, g in enumerate(e["gA"]):
+                g.replay()
+                if k == 0:
+                    self._colors(e["geo"], colors_on)
             self.graph_kernel_launches += e["nA"]
             self._geo = e["geo"]
             return
-        if self.use_graphs and e["warm"] >= 2:  # two eager warm-up rounds (allocator, lazy inits), then capture
-            g = torch.cuda.CUDAGraph()
-            # torch does not collect garbage before a capture: an unreachable trainer's pinned host buffers, released by
-            # a collection in the middle of the capture, would invalidate it
-            gc.collect()
-            n0 = self._lib_launches()
-            with torch.cuda.graph(g, stream=self.main):
-                e["geo"] = self.geometry_fn(self.model, self.st, self.scene, self.capacity, self.status)
-            e["gA"], e["nA"] = g, self._lib_launches() - n0   # libb200splat kernels recorded in the graph
-            g.replay()  # (capture does not execute)
-            self._geo = e["geo"]
+        capture = self.use_graphs and e["warm"] >= 2  # two eager warm-up rounds (allocator, lazy inits), then capture
+        geo, graphs, launches = None, [], 0
+        for k, part in enumerate(self._A_parts()):
+            if capture:
+                g = torch.cuda.CUDAGraph()
+                # torch does not collect garbage before a capture: an unreachable trainer's pinned host buffers, released
+                # by a collection in the middle of the capture, would invalidate it
+                gc.collect()
+                n0 = self._lib_launches()
+                with torch.cuda.graph(g, stream=self.main):
+                    geo = part(geo)
+                launches += self._lib_launches() - n0  # libb200splat kernels recorded in the graph
+                g.replay()  # (capture does not execute)
+                graphs.append(g)
+            else:
+                geo = part(geo)
+            if k == 0:
+                self._colors(geo, colors_on)
+        if capture:
+            e["gA"], e["nA"], e["geo"] = graphs, launches, geo
+        self._geo = geo
+
+    def _colors(self, geo, on):
+        """With the trainer's own fused phases: the colours of A's records from the SH rows as the last update left them.
+        on = `side`: queued there behind the SH update, once the projection is done (B, which waits for `side`, then
+        starts with the blend); None: on `main`, after any SH update still pending."""
+        if not self._own_fused:
             return
-        self._geo = self.geometry_fn(self.model, self.st, self.scene, self.capacity, self.status)
-        e["geo_eager"] = True
+        args = (self.model, geo, self.sh_degree, self.rasterize_mode, self.color_mode)
+        if on is None:
+            if self._pending_sh is not None:
+                torch.cuda.current_stream().wait_event(self.ev_sh_done)
+                self._pending_sh = None
+            fused_colors(*args)
+            return
+        self.ev_projected.record()
+        with torch.cuda.stream(on):
+            on.wait_event(self.ev_projected)
+            fused_colors(*args)
 
     def _run_B(self, e, target):
-        if self.use_graphs and e["gB"] is not None:
+        # B's graph reads the tensors of its entry's A graph, so it is replayed (or captured) only when that graph produced
+        # this image's records: a host poll between A and B (sync_status) can move the list capacity, and with it the
+        # entry.  (The trainer's own fused phases write this image's colours into those records only.)
+        bound = self._geo is e["geo"]
+        if self.use_graphs and e["gB"] is not None and bound:
             e["target"].copy_(target, non_blocking=True)
             e["gB"].replay()
             self.graph_kernel_launches += e["nB"]
             return
-        if self.use_graphs and e["gA"] is not None and e["warm"] >= 2:
+        if self.use_graphs and e["gA"] is not None and e["warm"] >= 2 and bound:
             # B is captured against the tensors A's graph writes (static addresses), with a static target buffer
             e["target"] = torch.empty_like(target)
             e["target"].copy_(target)
@@ -1043,9 +1134,9 @@ class PipelinedTrainer:
         self._prepared = True
         self._A_done = False
 
-    def _ensure_A(self, e):
+    def _ensure_A(self, e, colors_on=None):
         if not self._A_done:
-            self._run_A(e)
+            self._run_A(e, colors_on)
             self._A_done = True
             if self.distributed:  # this image's overflow flag, agreed on by all ranks before anyone's Adam reads it
                 self._flag_work = dist.all_reduce(self.flag, op=dist.ReduceOp.MAX, group=self.group, async_op=True)
@@ -1116,10 +1207,11 @@ class PipelinedTrainer:
                     if works is not None:
                         works[1 + j].wait()
                     self._update(a, b_, scale, veto_host, 1)
-                self.ev_sh_done.record(self.side)
             self._pending_sh = True
-            if next_cam is not None:
-                self._ensure_A(self._entry((tuple(target.shape), target.dtype)))
+            if next_cam is not None:  # (the next image's colours go behind the SH update)
+                self._ensure_A(self._entry((tuple(target.shape), target.dtype)), self.side)
+            self.ev_sh_done.record(self.side)
+            self._grads_left = self._own_fused
         else:
             for j in range(len(self._sh_bounds)):
                 if works is not None:
@@ -1130,6 +1222,15 @@ class PipelinedTrainer:
 
     def _update(self, a, b_, scale, veto_host, which):
         if self.adam is not None:
+            clear = "veto" if self._own_fused else True  # (the backward overwrites the Gaussian rows: see __init__)
+            m = self.model
+            if which == 0 and self._own_fused and m.row_fields:
+                # the Gaussian rows, then the camera / background rows behind them, which the step adds into: cleared.  The
+                # cut is on a 16-byte boundary, so up to 3 floats of the last Gaussian rows are cleared as well
+                cut = m.slices["opacity_logit"][1] // 4 * 4
+                self.adam.update_state(a, cut, scale, clear)
+                self.adam.update_state(cut, b_, scale, True)
+                return
             if which == 1 and self.sh_update_pieces > 1:
                 # the SH slice is updated on the side stream beside the next image's projection / binning.  One launch would
                 # queue its whole grid (tens of thousands of short CTAs) ahead of whatever arrives later at the same
@@ -1139,9 +1240,9 @@ class PipelinedTrainer:
                 cuts = [a + ((b_ - a) * k // n) // 4 * 4 for k in range(n)] + [b_]
                 for lo_, hi_ in zip(cuts[:-1], cuts[1:]):
                     if hi_ > lo_:
-                        self.adam.update_state(lo_, hi_, scale, True, background_ctas=self.sh_update_ctas)
+                        self.adam.update_state(lo_, hi_, scale, clear, background_ctas=self.sh_update_ctas)
                 return
-            self.adam.update_state(a, b_, scale, True, background_ctas=self.sh_update_ctas if which == 1 else 0)
+            self.adam.update_state(a, b_, scale, clear, background_ctas=self.sh_update_ctas if which == 1 else 0)
             return
         g = self.model.flat_grad[a:b_]
         if not veto_host:
@@ -1193,11 +1294,16 @@ class PipelinedTrainer:
 
     def finish(self):
         """Order the caller's stream after everything queued so far, the SH update on the side stream included (call
-        before reading parameters)."""
+        before reading parameters).  The gradient buffer is then zero, as a clearing optimizer leaves it: the updates of
+        the trainer's own fused steps leave the Gaussian rows to the next backward, which overwrites them, so they are
+        cleared here."""
         with self._OnMain(self):
             if self.cuda and self._pending_sh is not None:
                 torch.cuda.current_stream().wait_event(self.ev_sh_done)
                 self._pending_sh = None
+            if self._grads_left:
+                self.model.flat_grad.zero_()
+                self._grads_left = False
 
     # ---- lagged host view of the device status (overflow / vetoes / input check) ---------------------------------
     def _poll_host(self):

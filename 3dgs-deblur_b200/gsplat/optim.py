@@ -156,6 +156,7 @@ def group_segments(model, lr):
 
 
 MAX_GROUPS = 16          # B200_ADAM_MAX_GROUPS
+CLEAR_ON_VETO = 2        # B200_ADAM_CLEAR_ON_VETO
 GROUP_TABLE_FLOATS = 64  # B200_ADAM_GROUP_TABLE_FLOATS: lr / bc1 [16] | 1 / sqrt(bc2) [16] | step counts [16] | mask
 
 
@@ -261,14 +262,19 @@ class FlatAdam:
                 self.state.data_ptr(), _lib.ptr(veto_flag), _lib.ptr(detached), bits, cond, every, self._rates.shape[0],
                 self._rates.data_ptr(), self.betas[0], self.betas[1], self._table.data_ptr(), stream()))
 
-    def update_state(self, begin: int = 0, end: int = None, grad_scale: float = 1.0, zero_grad: bool = True,
+    def update_state(self, begin: int = 0, end: int = None, grad_scale: float = 1.0, zero_grad=True,
                      background_ctas: int = 0):
-        """Every element at its own group's rate, or at `lr` without groups.  background_ctas > 0: run as a background
-        kernel with that many resident CTAs per SM -- for an update queued on a second stream beside latency-bound
-        kernels."""
+        """Every element at its own group's rate, or at `lr` without groups.  zero_grad: True clears the gradient slice
+        behind the update, False leaves it, "veto" clears it on a vetoed step only (for a slice the next backward
+        overwrites in full: an applied step then skips the clear, and a vetoed step still leaves it zero).
+        background_ctas > 0: run as a background kernel with that many resident CTAs per SM -- for an update queued on a
+        second stream beside latency-bound kernels."""
         end = self.flat.numel() if end is None else end
         if not (0 <= begin <= end <= self.flat.numel()) or begin % 4:
             raise ValueError(f"FlatAdam.update_state: bad slice [{begin}, {end}) (must start on a 16-byte boundary)")
+        if zero_grad not in (True, False, "veto"):
+            raise ValueError(f"FlatAdam.update_state: zero_grad must be True, False or 'veto', got {zero_grad!r}")
+        clear = CLEAR_ON_VETO if zero_grad == "veto" else int(bool(zero_grad))
         segs = self._segments
         if self.groups is not None and not segs.shape[0]:
             raise ValueError("FlatAdam.update_state: a grouped update needs set_groups(segments) with at least one segment")
@@ -277,7 +283,7 @@ class FlatAdam:
         with _lib.on_device(self.flat.device):
             check(self._lib.b200_adam_update(end - begin, begin, p + off, g + off, m + off, v + off, segs.shape[0],
                                              segs.data_ptr(), self.state.data_ptr(), self._table.data_ptr(), self.betas[0],
-                                             self.betas[1], self.eps, float(grad_scale), 1 if zero_grad else 0,
+                                             self.betas[1], self.eps, float(grad_scale), clear,
                                              max(int(background_ctas), 0), stream()))
 
     def rebind(self, flat: torch.Tensor, flat_grad: torch.Tensor):

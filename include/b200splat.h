@@ -720,13 +720,16 @@ B200_API int b200_adam_step(long long numel, float *param, float *grad, float *e
  *       detached_groups step, and group cond_group as well when s is a multiple of cond_every (cond_group < 0: none).  A
  *       group that steps advances t_g and gets new constants; the others keep both.
  *   b200_adam_update: the update of numel floats whose first one is GLOBAL flat index `offset`; the slice must start
- *       16-byte aligned.  A vetoed step moves nothing and clears the gradient slice.  n_segments == 0: every element uses
+ *       16-byte aligned.  A vetoed step moves nothing and clears the gradient slice.  zero_grad: 1 clears the gradient
+ *       slice, 0 leaves it, B200_ADAM_CLEAR_ON_VETO clears it on a vetoed step only -- for a caller whose backward
+ *       overwrites every gradient of the slice, which then needs no clear behind an applied step (and no masked group's
+ *       clear: a detached image's rows are already zero).  n_segments == 0: every element uses
  *       the state's constants.  n_segments > 0: every element uses its own group's constants from group_table.
  *       segments: HOST long long[n_segments][B200_ADAM_SEGMENT_WORDS], sorted and disjoint, by value like `groups`:
  *       {begin, end, period, split, group_a, group_b}.  Global index i in [begin, end) belongs to group_a when
  *       period == 0 or (i - begin) % period < split, else to group_b.  An element in no segment, or in a group outside the
- *       step's mask, keeps its parameter and moments bit-unchanged; its gradient is still cleared.  The slice need not
- *       start or end on a segment boundary.  After a prepare with a `detached` word, pass the segment table: without one
+ *       step's mask, keeps its parameter and moments bit-unchanged; its gradient is cleared as zero_grad says.  The
+ *       slice need not start or end on a segment boundary.  After a prepare with a `detached` word, pass the segment table: without one
  *       the update reads word [3] = 2 as a veto.  ctas_per_sm: 0 = many short CTAs; 1..32 = a background kernel for a
  *       caller that runs it on a second stream beside latency-bound work: at most ctas_per_sm resident CTAs of 256 threads
  *       per SM loop over the slice, so kernels launched beside it always find free thread slots instead of queueing
@@ -740,6 +743,7 @@ B200_API int b200_adam_step(long long numel, float *param, float *grad, float *e
 #define B200_ADAM_SEGMENT_WORDS 6
 #define B200_ADAM_GROUP_TABLE_FLOATS 64
 #define B200_DETACHED_MAX_RANGES 4
+#define B200_ADAM_CLEAR_ON_VETO 2
 B200_API size_t b200_adam_state_bytes(void);
 B200_API int b200_adam_prepare_step(void *state, int32_t *veto_flag, const int32_t *detached, unsigned detached_groups,
                                     int cond_group, int cond_every, int n_groups, const double *groups, double beta1,
