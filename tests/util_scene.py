@@ -39,12 +39,15 @@ def oracle_colors(d, deg=3):
     return np.maximum(col + 0.5, 0.0).astype(np.float32)
 
 
-def oracle_render(d, proj=None, colors=None):
-    """Full oracle forward: projection -> binning -> blend.  Returns dict with everything."""
+def oracle_render(d, proj=None, colors=None, blend=True):
+    """Full oracle forward: projection -> binning -> blend.  Returns dict with everything (blend=False: without the
+    blend's img / final_Ts / final_idx)."""
     proj = oracle_project(d) if proj is None else proj
     colors = oracle_colors(d) if colors is None else colors
     opac = (d["opacity"][:, 0] * proj["compensation"]).astype(np.float32)[:, None]
     b = O.bin_and_sort(proj["xys"], proj["depths"], proj["radii"], proj["num_tiles_hit"], d["H"], d["W"], d["bw"])
+    if not blend:
+        return dict(proj=proj, colors=colors, opac=opac, bins=b)
     img, Ts, fi = O.rasterize_forward(d["H"], d["W"], d["bw"], d["S"], b["gaussian_ids_sorted"], b["tile_bins"],
                                       proj["xys"], proj["pix_vels"], d["rs"], d["exposure"], proj["conics"], colors,
                                       opac, d["background"])
