@@ -3,6 +3,7 @@
 // blend backward consumes, instead of sub / abs / mean forward plus sign / mul / div / expand in autograd
 // (7 image-sized passes).  Deterministic: per-block partial sums, the last block to finish adds them in block order.
 #include "common.cuh"
+#include "target_prep.cuh"
 
 namespace b200 {
 
@@ -107,12 +108,7 @@ __device__ __forceinline__ float l1_target_pixel(const float *x, float t0, float
                                                  bool has_mask, const L1U8Args &a, const float (&bg)[3], float *g,
                                                  float *t_out) {
     float t[3] = {t0, t1, t2};
-    if (CH == 4) {
-        const float om = __fsub_rn(1.0f, al);
-        t[0] = __fadd_rn(__fmul_rn(al, t[0]), __fmul_rn(om, bg[0]));
-        t[1] = __fadd_rn(__fmul_rn(al, t[1]), __fmul_rn(om, bg[1]));
-        t[2] = __fadd_rn(__fmul_rn(al, t[2]), __fmul_rn(om, bg[2]));
-    }
+    if (CH == 4) composite_over_bg(t, al, bg);
     float sum = 0.f;
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
@@ -137,8 +133,8 @@ __device__ __forceinline__ float l1_target_pixel(const float *x, float t0, float
 template <int CH, bool GAMMA>
 __device__ __forceinline__ float l1_u8_pixel(const float *x, const uint8_t *t8, float m, bool has_mask, const L1U8Args &a,
                                              const float (&bg)[3], float *g, float *t_out) {
-    return l1_target_pixel<CH, GAMMA>(x, (float)t8[0] / 255.0f, (float)t8[1] / 255.0f, (float)t8[2] / 255.0f,
-                                      CH == 4 ? (float)t8[3] / 255.0f : 1.0f, m, has_mask, a, bg, g, t_out);
+    return l1_target_pixel<CH, GAMMA>(x, unit_u8(t8[0]), unit_u8(t8[1]), unit_u8(t8[2]), CH == 4 ? unit_u8(t8[3]) : 1.0f,
+                                      m, has_mask, a, bg, g, t_out);
 }
 
 template <int CH, bool GAMMA>

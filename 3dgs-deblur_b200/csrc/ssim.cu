@@ -13,6 +13,7 @@
 //                         to a scaled L1 cotangent so the combined photometric cotangent is written once.
 // Images are (H, W, C) fp32 as the rasterizer produces them; maps are planar [3][C][H-10][W-10].
 #include "common.cuh"
+#include "target_prep.cuh"
 
 namespace b200 {
 
@@ -46,21 +47,15 @@ struct SsimFwdParams {
 // Both kernels filter separably through shared memory, and both passes are register-tiled: a thread produces 4 (2)
 // neighbouring outputs from one sliding run of 14 (12) shared loads instead of 11 loads per output -- the first version
 // was bound by the shared-memory pipe (ncu: mio_throttle, LSU 46 %).
-__global__ void __launch_bounds__(SSIM_THREADS) ssim_forward_kernel(const SsimFwdParams p) {
-    __shared__ float s_p[SSIM_PH][SSIM_PW + 1], s_t[SSIM_PH][SSIM_PW + 1];
-    __shared__ float s_v[5][SSIM_TH][SSIM_PW + 1];  // after the pass along H
-    __shared__ float s_red[SSIM_THREADS / 32];
-    __shared__ bool s_last;
-    const int c = blockIdx.z, i0 = blockIdx.y * SSIM_TH, j0 = blockIdx.x * SSIM_TW;
+//
+// The forward filter of one staged tile, shared by ssim_forward_kernel and eval_metrics_kernel: the five moments
+// {p, t, p^2, t^2, pt} of the 42x26 patches s_p, s_t filtered along H into s_v (threads < 208), then along W into
+// out[o][m] for this thread's outputs (row tid / 8, columns 2 (tid % 8) + o).  Starts after the patches are staged and
+// synchronised; s_v is free again when it returns.
+__device__ __forceinline__ void ssim_filter_tile(const float (&s_p)[SSIM_PH][SSIM_PW + 1], const float (&s_t)[SSIM_PH][SSIM_PW + 1],
+                                                 float (&s_v)[5][SSIM_TH][SSIM_PW + 1], const SsimWindow &win,
+                                                 float (&out)[SSIM_RH][5]) {
     const int tid = threadIdx.x;
-    for (int e = tid; e < SSIM_PH * SSIM_PW; e += SSIM_THREADS) {
-        const int r = e / SSIM_PW, q = e % SSIM_PW;
-        const int i = min(i0 + r, p.H - 1), j = min(j0 + q, p.W - 1);  // clamped reads only feed masked outputs
-        const size_t idx = ((size_t)i * p.W + j) * p.C + c;
-        s_p[r][q] = p.pred[idx];
-        s_t[r][q] = __ldg(p.target + idx);
-    }
-    __syncthreads();
     if (tid < (SSIM_TH / SSIM_RV) * SSIM_PW) {  // along H: column q, output rows r0 .. r0 + 3
         const int q = tid % SSIM_PW, r0 = (tid / SSIM_PW) * SSIM_RV;
         float acc[SSIM_RV][5];
@@ -76,7 +71,7 @@ __global__ void __launch_bounds__(SSIM_THREADS) ssim_forward_kernel(const SsimFw
             for (int o = 0; o < SSIM_RV; ++o) {
                 const int k = j - o;  // tap index of this input row for output row r0 + o (compile-time after unrolling)
                 if (k >= 0 && k < SSIM_WIN) {
-                    const float w = p.win.w[k];
+                    const float w = win.w[k];
                     acc[o][0] += w * x; acc[o][1] += w * y; acc[o][2] += w * xx; acc[o][3] += w * yy; acc[o][4] += w * xy;
                 }
             }
@@ -89,7 +84,6 @@ __global__ void __launch_bounds__(SSIM_THREADS) ssim_forward_kernel(const SsimFw
     __syncthreads();
     // along W: row r, output columns q0, q0 + 1
     const int r = tid / (SSIM_TW / SSIM_RH), q0 = (tid % (SSIM_TW / SSIM_RH)) * SSIM_RH;
-    float out[SSIM_RH][5];
 #pragma unroll
     for (int o = 0; o < SSIM_RH; ++o)
 #pragma unroll
@@ -103,12 +97,32 @@ __global__ void __launch_bounds__(SSIM_THREADS) ssim_forward_kernel(const SsimFw
         for (int o = 0; o < SSIM_RH; ++o) {
             const int k = j - o;
             if (k >= 0 && k < SSIM_WIN) {
-                const float w = p.win.w[k];
+                const float w = win.w[k];
 #pragma unroll
                 for (int m = 0; m < 5; ++m) out[o][m] += w * v[m];
             }
         }
     }
+}
+
+__global__ void __launch_bounds__(SSIM_THREADS) ssim_forward_kernel(const SsimFwdParams p) {
+    __shared__ float s_p[SSIM_PH][SSIM_PW + 1], s_t[SSIM_PH][SSIM_PW + 1];
+    __shared__ float s_v[5][SSIM_TH][SSIM_PW + 1];  // after the pass along H
+    __shared__ float s_red[SSIM_THREADS / 32];
+    __shared__ bool s_last;
+    const int c = blockIdx.z, i0 = blockIdx.y * SSIM_TH, j0 = blockIdx.x * SSIM_TW;
+    const int tid = threadIdx.x;
+    for (int e = tid; e < SSIM_PH * SSIM_PW; e += SSIM_THREADS) {
+        const int r = e / SSIM_PW, q = e % SSIM_PW;
+        const int i = min(i0 + r, p.H - 1), j = min(j0 + q, p.W - 1);  // clamped reads only feed masked outputs
+        const size_t idx = ((size_t)i * p.W + j) * p.C + c;
+        s_p[r][q] = p.pred[idx];
+        s_t[r][q] = __ldg(p.target + idx);
+    }
+    __syncthreads();
+    float out[SSIM_RH][5];
+    ssim_filter_tile(s_p, s_t, s_v, p.win, out);
+    const int r = tid / (SSIM_TW / SSIM_RH), q0 = (tid % (SSIM_TW / SSIM_RH)) * SSIM_RH;
     float S_sum = 0.f;
     const int i = i0 + r;
 #pragma unroll
@@ -246,6 +260,118 @@ __global__ void __launch_bounds__(SSIM_THREADS) ssim_backward_kernel(const SsimB
     }
 }
 
+// ---- Evaluation metrics of B views in one launch (nerfstudio's get_image_metrics_and_images, splatfacto.py:1006-1042) ---
+// Per view v: y = min(pred, 1)^(1/gamma) (splatfacto.py:880; gamma == 1: min(pred, 1) with no powf), t = the target as
+// b200_l1_loss_u8 prepares it with no minimum level and no mask (uint8 / 255 or float, RGBA composited over bg), then
+// mse = mean (y - t)^2 over 3 H W, psnr = 10 log10(1 / mse) (torchmetrics' PeakSignalNoiseRatio(data_range=1)) and ssim
+// = ssim_forward_kernel's value of (y, t).  Grid (SSIM tiles along W, along H, 3 B): CTA (bx, by, 3 v + c) stages
+// channel c of view v's 42x26 patches with both steps applied on the load, so no intermediate image or map is written.
+// Its squared errors are taken on the same load from the pixels the CTA owns: the tile's 32x16 pixels, and for the last
+// tile row / column the 10 rows / columns past it that no output tile starts at -- every pixel exactly once.
+// Reduction per view, in a fixed order: thread sums (squared errors in patch order), warp butterflies, the 8 warps in
+// order into partial[v][bid], bid = (c * gy + by) * gx + bx as in ssim_forward_kernel; the last CTA of the view to take
+// the view's ticket adds the view's partials lane-strided and by butterfly and re-arms the ticket.
+struct EvalParams {
+    int H, W, Ho, Wo;
+    const float *pred;
+    const void *target;
+    const float *background;
+    float inv_gamma, inv_count, inv_n, C1, C2;
+    float *part_s, *part_e;  // [B][3 gy gx] SSIM and squared-error partials
+    unsigned int *tickets;   // [B]
+    float *mse, *psnr, *ssim;
+    SsimWindow win;
+};
+
+template <int CH, bool U8, bool GAMMA>
+__global__ void __launch_bounds__(SSIM_THREADS) eval_metrics_kernel(const EvalParams p) {
+    __shared__ float s_p[SSIM_PH][SSIM_PW + 1], s_t[SSIM_PH][SSIM_PW + 1];
+    __shared__ float s_v[5][SSIM_TH][SSIM_PW + 1];
+    __shared__ float s_red[2][SSIM_THREADS / 32];
+    __shared__ bool s_last;
+    const int v = blockIdx.z / 3, c = blockIdx.z - 3 * v;
+    const int i0 = blockIdx.y * SSIM_TH, j0 = blockIdx.x * SSIM_TW;
+    const bool last_y = blockIdx.y == gridDim.y - 1, last_x = blockIdx.x == gridDim.x - 1;
+    const int tid = threadIdx.x;
+    float bg[3] = {0.f, 0.f, 0.f};
+    if (CH == 4) { bg[0] = __ldg(p.background); bg[1] = __ldg(p.background + 1); bg[2] = __ldg(p.background + 2); }
+    const size_t view = (size_t)v * p.H * p.W;
+    float se = 0.f;
+    for (int e = tid; e < SSIM_PH * SSIM_PW; e += SSIM_THREADS) {
+        const int r = e / SSIM_PW, q = e % SSIM_PW;
+        const int i = min(i0 + r, p.H - 1), j = min(j0 + q, p.W - 1);  // clamped reads only feed masked outputs
+        const size_t px = view + (size_t)i * p.W + j;
+        const float x = fminf(p.pred[3 * px + c], 1.0f);
+        const float y = GAMMA ? powf(x, p.inv_gamma) : x;
+        float t[3], al = 1.0f;
+        if (U8) {
+            const uint8_t *t8 = static_cast<const uint8_t *>(p.target) + CH * px;
+#pragma unroll
+            for (int k = 0; k < 3; ++k) t[k] = unit_u8(__ldg(t8 + k));
+            if (CH == 4) al = unit_u8(__ldg(t8 + 3));
+        } else {
+            const float *tf = static_cast<const float *>(p.target) + CH * px;
+#pragma unroll
+            for (int k = 0; k < 3; ++k) t[k] = __ldg(tf + k);
+            if (CH == 4) al = __ldg(tf + 3);
+        }
+        if (CH == 4) composite_over_bg(t, al, bg);
+        const float tc = c == 0 ? t[0] : (c == 1 ? t[1] : t[2]);
+        s_p[r][q] = y;
+        s_t[r][q] = tc;
+        if ((r < SSIM_TH || last_y) && (q < SSIM_TW || last_x) && i0 + r < p.H && j0 + q < p.W) {
+            const float d = y - tc;
+            se += d * d;
+        }
+    }
+    __syncthreads();
+    float out[SSIM_RH][5];
+    ssim_filter_tile(s_p, s_t, s_v, p.win, out);
+    const int r = tid / (SSIM_TW / SSIM_RH), q0 = (tid % (SSIM_TW / SSIM_RH)) * SSIM_RH;
+    float S_sum = 0.f;
+#pragma unroll
+    for (int o = 0; o < SSIM_RH; ++o) {
+        if (i0 + r < p.Ho && j0 + q0 + o < p.Wo) {  // ssim_forward_kernel's expression of S
+            const float mu_p = out[o][0], mu_t = out[o][1], e_pp = out[o][2], e_tt = out[o][3], e_pt = out[o][4];
+            const float mpp = mu_p * mu_p, mtt = mu_t * mu_t, mpt = mu_p * mu_t;
+            const float var_p = e_pp - mpp, var_t = e_tt - mtt, cov = e_pt - mpt;
+            const float A1 = 2.f * mpt + p.C1, A2 = 2.f * cov + p.C2;
+            const float B1 = mpp + mtt + p.C1, B2 = var_p + var_t + p.C2;
+            S_sum += (A1 * (1.f / B1)) * (A2 * (1.f / B2));
+        }
+    }
+    const float ws = warp_sum(S_sum), we = warp_sum(se);
+    if ((tid & 31) == 0) { s_red[0][tid >> 5] = ws; s_red[1][tid >> 5] = we; }
+    __syncthreads();
+    const unsigned int per_view = 3u * gridDim.x * gridDim.y;
+    const unsigned int bid = (c * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
+    float *ps = p.part_s + (size_t)v * per_view, *pe = p.part_e + (size_t)v * per_view;
+    if (tid == 0) {
+        float bs = 0.f, be = 0.f;
+#pragma unroll
+        for (int w = 0; w < SSIM_THREADS / 32; ++w) { bs += s_red[0][w]; be += s_red[1][w]; }
+        ps[bid] = bs;
+        pe[bid] = be;
+        __threadfence();
+        s_last = atomicAdd(p.tickets + v, 1u) == per_view - 1;
+    }
+    __syncthreads();
+    if (s_last && tid < 32) {
+        __threadfence();
+        float ts = 0.f, te = 0.f;
+        for (unsigned int k = tid; k < per_view; k += 32) { ts += __ldcg(ps + k); te += __ldcg(pe + k); }
+        ts = warp_sum(ts);
+        te = warp_sum(te);
+        if (tid == 0) {
+            const float mse = te * p.inv_n;
+            p.mse[v] = mse;
+            p.psnr[v] = -10.f * log10f(mse);  // 10 log10(1 / mse); +inf at mse == 0
+            p.ssim[v] = ts * p.inv_count;
+            p.tickets[v] = 0u;
+        }
+    }
+}
+
 // SSIM of smooth images is ill-conditioned in the window's normalisation (var = E[x^2] - mu^2 with E[x^2] >> var: a
 // relative error d in sum(w) moves var by ~25 d), so a caller that wants the library's numbers passes the library's own
 // float32 taps (gsplat/losses.py builds them with the same torch ops as pytorch_msssim._fspecial_gauss_1d); the
@@ -322,6 +448,68 @@ extern "C" int b200_ssim_backward(unsigned img_height, unsigned img_width, unsig
     p.win = make_window(window11);
     dim3 grid((p.W + SSIM_TW - 1) / SSIM_TW, (p.H + SSIM_TH - 1) / SSIM_TH, p.C);
     ssim_backward_kernel<<<grid, SSIM_THREADS, 0, as_stream(stream)>>>(p);
+    B200_LAUNCH_CHECK();
+    return B200_OK;
+}
+
+// workspace of b200_eval_metrics_views: B tickets, then B x (3 gy gx) SSIM partials and as many squared-error partials
+static size_t eval_ws_layout(unsigned views, unsigned H, unsigned W, size_t *off_s, size_t *off_e) {
+    const size_t per_view = 3 * (size_t)((W - SSIM_WIN + 1 + SSIM_TW - 1) / SSIM_TW) * ((H - SSIM_WIN + 1 + SSIM_TH - 1) / SSIM_TH);
+    WsCarver ws;
+    ws.take(sizeof(unsigned int) * views);
+    *off_s = ws.take(sizeof(float) * per_view * views);
+    *off_e = ws.take(sizeof(float) * per_view * views);
+    return ws.off;
+}
+
+extern "C" size_t b200_eval_metrics_ws_bytes(unsigned views, unsigned img_height, unsigned img_width) {
+    if (views == 0 || img_height < SSIM_WIN || img_width < SSIM_WIN) return 256;
+    size_t a, b;
+    return eval_ws_layout(views, img_height, img_width, &a, &b);
+}
+
+extern "C" int b200_eval_metrics_views(unsigned views, unsigned img_height, unsigned img_width, unsigned channels,
+                                       const float *pred_linear, const void *target, int target_is_u8,
+                                       const float *background, float gamma, const float *window11, float *mse_out,
+                                       float *psnr_out, float *ssim_out, void *ws, int ws_is_zeroed, void *stream) {
+    B200_REQUIRE(views >= 1 && views <= 65535 / 3, "views must be 1 .. 21845");
+    B200_REQUIRE(img_height >= SSIM_WIN && img_width >= SSIM_WIN, "SSIM needs an image of at least 11 x 11 pixels");
+    B200_REQUIRE(channels == 3 || channels == 4, "target must have 3 or 4 channels");
+    B200_REQUIRE(target_is_u8 == 0 || target_is_u8 == 1, "target_is_u8 must be 0 or 1");
+    B200_REQUIRE(gamma > 0.f && gamma < INFINITY, "gamma must be positive and finite");
+    B200_REQUIRE(pred_linear && target && mse_out && psnr_out && ssim_out && ws, "null pointer");
+    B200_REQUIRE(channels == 3 || background, "an RGBA target needs a background colour");
+    B200_REQUIRE(aligned16(ws), "ws must be 16-byte aligned");
+    EvalParams p;
+    p.H = (int)img_height; p.W = (int)img_width;
+    p.Ho = p.H - SSIM_WIN + 1; p.Wo = p.W - SSIM_WIN + 1;
+    p.pred = pred_linear; p.target = target; p.background = background;
+    p.inv_gamma = (float)(1.0 / (double)gamma);
+    p.inv_count = (float)(1.0 / ((double)p.Ho * (double)p.Wo * 3.0));
+    p.inv_n = (float)(1.0 / ((double)p.H * (double)p.W * 3.0));
+    p.C1 = 0.01f * 0.01f; p.C2 = 0.03f * 0.03f;
+    size_t off_s, off_e;
+    eval_ws_layout(views, img_height, img_width, &off_s, &off_e);
+    p.tickets = static_cast<unsigned int *>(ws);
+    p.part_s = reinterpret_cast<float *>(static_cast<char *>(ws) + off_s);
+    p.part_e = reinterpret_cast<float *>(static_cast<char *>(ws) + off_e);
+    p.mse = mse_out; p.psnr = psnr_out; p.ssim = ssim_out;
+    p.win = make_window(window11);
+    cudaStream_t st = as_stream(stream);
+    if (!ws_is_zeroed) B200_CUDA(cudaMemsetAsync(p.tickets, 0, sizeof(unsigned int) * views, st));
+    dim3 grid((p.Wo + SSIM_TW - 1) / SSIM_TW, (p.Ho + SSIM_TH - 1) / SSIM_TH, 3 * views);
+    const bool pw = gamma != 1.0f;
+#define B200_EVAL(CH, U8)                                                                         \
+    (pw ? eval_metrics_kernel<CH, U8, true><<<grid, SSIM_THREADS, 0, st>>>(p)                  \
+        : eval_metrics_kernel<CH, U8, false><<<grid, SSIM_THREADS, 0, st>>>(p))
+    if (channels == 4) {
+        if (target_is_u8) B200_EVAL(4, true);
+        else B200_EVAL(4, false);
+    } else {
+        if (target_is_u8) B200_EVAL(3, true);
+        else B200_EVAL(3, false);
+    }
+#undef B200_EVAL
     B200_LAUNCH_CHECK();
     return B200_OK;
 }

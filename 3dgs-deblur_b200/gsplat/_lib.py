@@ -72,6 +72,8 @@ SIGNATURES = {
     "b200_ssim_maps_bytes": (_sz, [_u, _u, _u]),
     "b200_ssim_forward": (_i, [_u, _u, _u, _p, _p, _p, _p, _p, _p, _f, _p, _p, _i, _p]),
     "b200_ssim_backward": (_i, [_u, _u, _u, _p, _p, _p, _f, _p, _f, _p, _p, _p, _p]),
+    "b200_eval_metrics_ws_bytes": (_sz, [_u, _u, _u]),
+    "b200_eval_metrics_views": (_i, [_u, _u, _u, _u, _p, _p, _i, _p, _f, _p, _p, _p, _p, _p, _i, _p]),
     "b200_l1_loss_ws_bytes": (_sz, []),
     "b200_l1_loss": (_i, [C.c_longlong, _p, _p, _p, _p, _p, _i, _p]),
     "b200_l1_loss_gamma": (_i, [C.c_longlong, _p, _p, _f, _p, _p, _p, _i, _p]),

@@ -222,6 +222,130 @@ def render_fused(model: FlatGaussians, cam: Dict, scene: Dict, cam_index: int = 
     return rgb, alpha, info
 
 
+def _camera_row(cam) -> torch.Tensor:
+    """The 21 camera floats (viewmat 12 | lin_vel 3 | ang_vel 3 | cam_pos 3) of a camera dict or row."""
+    if torch.is_tensor(cam):
+        return cam.detach().reshape(-1)[:21].float()
+    d0 = cam["viewmat"].device
+    return torch.cat([cam["viewmat"].reshape(-1)[:12], cam["lin_vel"].reshape(-1)[:3].to(d0),
+                      cam["ang_vel"].reshape(-1)[:3].to(d0), cam["cam_pos"].reshape(-1)[:3].to(d0)]).float()
+
+
+def evaluate(model: FlatGaussians, scene: Dict, cams, images, cam_indices=None, *, gamma: float = 2.2,
+             sh_degree_to_use: int = 3, rasterize_mode: str = "antialiased", color_mode: str = "sh", background=None,
+             batch_size: int = 8, get_std: bool = False, return_renders: bool = False) -> Dict:
+    """PSNR and SSIM of the model's renders of held-out images, as nerfstudio's ns-eval reports them for Splatfacto
+    (VanillaPipeline.get_average_eval_image_metrics, pipelines/base_pipeline.py:348-414, with
+    get_image_metrics_and_images, splatfacto.py:1006-1042), LPIPS aside: it needs AlexNet weights, and the key is absent.
+
+    cams: one camera per image, a dict (viewmat (3,4) or (4,4), lin_vel, ang_vel, cam_pos; optional fx, fy, cx, cy, which
+    default to the scene's) or 21 floats in that order.  images: the ground truth, (H, W, 3) or (H, W, 4) uint8 (or
+    float32) tensors on the host or the device, each copied to the device with its batch.  Views are rendered at their
+    image's full size through gsplat.fused.render_gaussians_batch under no_grad, `batch_size` at a time (consecutive
+    views of equal size and kind share a batch), with the scene's blur and rolling-shutter settings, and scored by
+    gsplat.losses.image_metrics: clamp(rgb, max=1) ** (1 / gamma) against the image / 255, RGBA composited over the
+    render's background.
+
+    cam_indices: view k is camera row cam_indices[k] of the model -- required when the model has pose or velocity rows,
+    range-checked on the host.  With pose rows the view matrix and position are gsplat.camera_opt.apply_pose's; with
+    velocity rows the velocities are cam_vel[cam_indices[k]] + the camera's own (render_fused's rule); otherwise the
+    camera is used as it is.  With gsplat.data.load_transforms(..., optimize_eval_cameras=True) the eval images are the
+    first len(val) training cameras, in eval-split order (3dgs-deblur's detached eval cameras, whose rows ns-eval
+    renders the eval images with: base_pipeline.py:381-382 and nerfstudio_dataparser.py:241-252).
+
+    Background: sigmoid(learnable_bg) for a model that learns it (Splatfacto's background_color "auto"); otherwise
+    `background`, by default scene["background"].  Splatfacto's default background_color "random" evaluates over
+    torch.tensor([0.1490, 0.1647, 0.2157]) ** gamma (splatfacto.py:267-270): pass that to match it.
+
+    Returns a dict: psnr, ssim (n,) float32 device tensors; psnr_mean, ssim_mean floats, the mean of the per-image float32
+    values as get_average_eval_image_metrics computes it (torch.mean of a float32 tensor), and with get_std psnr_std,
+    ssim_std from torch.std_mean -- the one host read; with return_renders, renders: the linear renders (n, H, W, 3)
+    (a list of (H, W, 3) tensors when the images differ in size)."""
+    from gsplat.fused import render_gaussians_batch
+    from gsplat.losses import image_metrics
+
+    cams, images = list(cams), list(images)
+    n = len(cams)
+    if n < 1 or len(images) != n:
+        raise ValueError(f"evaluate: need one camera per image and at least one image, got {n} cameras and "
+                         f"{len(images)} images")
+    if int(batch_size) < 1:
+        raise ValueError("evaluate: batch_size must be >= 1")
+    has_rows = model.cam_pose is not None or model.cam_vel is not None
+    if cam_indices is None:
+        if has_rows:
+            raise ValueError("evaluate: the model has camera rows, so cam_indices (the camera row of each view) is needed")
+    else:
+        idx = [int(i) for i in (cam_indices.tolist() if torch.is_tensor(cam_indices) else cam_indices)]
+        if len(idx) != n:
+            raise ValueError(f"evaluate: {n} views need {n} cam_indices, got {len(idx)}")
+        rows_n = (model.cam_pose if model.cam_pose is not None else model.cam_vel).shape[0] if has_rows else None
+        if rows_n is not None and any(i < 0 or i >= rows_n for i in idx):
+            raise IndexError(f"evaluate: cam_indices out of range for {rows_n} camera rows")
+        cam_indices = idx
+    for k, im in enumerate(images):
+        if im.dim() != 3 or im.shape[2] not in (3, 4) or im.dtype not in (torch.uint8, torch.float32):
+            raise ValueError(f"evaluate: image {k} must be an (H, W, 3) or (H, W, 4) uint8 or float32 tensor, got "
+                             f"{tuple(im.shape)} {im.dtype}")
+    dev = model.flat.device
+    p = {k: v.detach() for k, v in model.params.items()}
+    if "sh" in p:
+        p.update(model.views)
+    if model.learnable_bg is not None:
+        bg = torch.sigmoid(model.learnable_bg.detach())
+    else:
+        bg = scene["background"] if background is None else background
+        bg = torch.as_tensor(bg, dtype=torch.float32).to(dev).reshape(3)
+    bw, rs, ex = scene["block_width"], scene["rolling_shutter_time"], scene["exposure_time"]
+    blur = scene["blur_samples"] if ex > 0 else 1
+    intr = [[float(c[k]) if not torch.is_tensor(c) and k in c else float(scene[k]) for k in ("fx", "fy", "cx", "cy")]
+            for c in cams]
+    kind = lambda k: tuple(images[k].shape) + (images[k].dtype,)  # noqa: E731
+    psnr, ssim, renders = [], [], []
+    with torch.no_grad():
+        a = 0
+        while a < n:
+            b = a + 1
+            while b < n and b - a < batch_size and kind(b) == kind(a):
+                b += 1
+            B = b - a
+            H, W = int(images[a].shape[0]), int(images[a].shape[1])
+            rows = torch.stack([_camera_row(c).to(dev) for c in cams[a:b]])
+            if model.cam_pose is not None:
+                from gsplat.camera_opt import apply_pose
+                viewmats, cam_pos = apply_pose(rows, model.cam_pose.detach(), torch.tensor(cam_indices[a:b]))
+            else:
+                viewmats, cam_pos = rows[:, :12].reshape(B, 3, 4), rows[:, 18:21]
+            vel = rows[:, 12:18]
+            if model.cam_vel is not None:
+                vel = model.cam_vel.detach()[torch.tensor(cam_indices[a:b], device=dev)] + vel
+            ks = torch.tensor(intr[a:b], dtype=torch.float32).to(dev).unbind(1)
+            rgb, _, _ = render_gaussians_batch(
+                p["means"], p["log_scales"], p["quats"], p["opacity_logit"], p["sh_dc"], p["sh_rest"], viewmats,
+                cam_pos.contiguous(), vel[:, :3].contiguous(), vel[:, 3:].contiguous(), *ks, H, W, bw, bg,
+                rolling_shutter_time=rs, exposure_time=ex, blur_samples=blur, sh_degree_to_use=sh_degree_to_use,
+                rasterize_mode=rasterize_mode, color_mode=color_mode)
+            target = torch.stack([im.to(dev, non_blocking=True) for im in images[a:b]])
+            ps, ss = image_metrics(rgb, target, gamma=gamma, background=bg)
+            psnr.append(ps)
+            ssim.append(ss)
+            if return_renders:
+                renders.append(rgb)
+            a = b
+    out = dict(psnr=torch.cat(psnr), ssim=torch.cat(ssim))
+    host = torch.stack([out["psnr"], out["ssim"]]).cpu()  # float32, as the per-image floats ns-eval collects
+    for key, vals in zip(("psnr", "ssim"), host):
+        if get_std:
+            std, mean = torch.std_mean(vals)
+            out[f"{key}_mean"], out[f"{key}_std"] = float(mean), float(std)
+        else:
+            out[f"{key}_mean"] = float(torch.mean(vals))
+    if return_renders:
+        same = all(r.shape[1:] == renders[0].shape[1:] for r in renders)
+        out["renders"] = torch.cat(renders) if same else [v for r in renders for v in r.unbind(0)]
+    return out
+
+
 class ImageShardedTrainer:
     """One process per GPU; rank r renders image (step * world + r) % n_images; one gradient exchange per step."""
 
@@ -1291,6 +1415,27 @@ class PipelinedTrainer:
             return True
         e = self._graphs.get(self._key() + (target_shape_dtype,))
         return e is not None and e["gA"] is not None and e["gB"] is not None
+
+    def evaluate(self, cams, images, cam_indices=None, **kw) -> Dict:
+        """`evaluate` of the model as it stands after the steps queued so far, with this trainer's render modes, the SH
+        degree of the next step (sh_degree_at(steps)) and the full-resolution scene; cam_indices defaults to the detached
+        cameras in ascending order (the eval images in eval-split order, as load_transforms(..., optimize_eval_cameras=
+        True) lays them out).  Other keywords go to `evaluate`.  The evaluation runs on the trainer's stream behind
+        everything queued, the SH update on the side stream included, and the next step runs behind it; it reads the
+        parameters and writes none of the trainer's state, so training goes on bit for bit as without the call.  On a
+        data-parallel trainer it evaluates this rank's images alone (no collective call)."""
+        if cam_indices is None and self._detached:
+            cam_indices = sorted(self._detached)
+        scene = dict(self.scene)
+        if self._full is not None:
+            scene.update(self._full)
+        kw.setdefault("sh_degree_to_use", self.sh_degree_at(self.steps))
+        kw.setdefault("rasterize_mode", self.rasterize_mode)
+        kw.setdefault("color_mode", self.color_mode)
+        with self._OnMain(self):
+            if self.cuda and self._pending_sh is not None:
+                torch.cuda.current_stream().wait_event(self.ev_sh_done)  # (the next step waits for it as well)
+            return evaluate(self.model, scene, cams, images, cam_indices, **kw)
 
     def finish(self):
         """Order the caller's stream after everything queued so far, the SH update on the side stream included (call

@@ -294,3 +294,78 @@ def photometric_loss(pred: torch.Tensor, target: torch.Tensor, ssim_lambda: floa
 photometric_loss.accepts_uint8 = True
 photometric_loss.accepts_downscale = True
 ssim.accepts_downscale = True
+
+
+# ---- evaluation metrics (what ns-eval reports per image, splatfacto.py:1006-1042) ----------------------------------
+
+_eval_ws = {}
+_EVAL_MAX_VIEWS = 21845  # views of one b200_eval_metrics_views launch
+
+
+def _eval_workspace(dev, B, H, W):
+    key = (dev.index, stream(), B, H, W)
+    ws = _eval_ws.get(key)
+    if ws is None:
+        ws = torch.zeros(_lib.load().b200_eval_metrics_ws_bytes(B, H, W), dtype=torch.uint8, device=dev)
+        _eval_ws[key] = ws
+    return ws
+
+
+def eval_metrics(pred: torch.Tensor, target: torch.Tensor, *, gamma: float = 2.2, background: torch.Tensor = None):
+    """(mse, psnr, ssim) of `image_metrics`, each a (B,) (or 0-d) float32 device tensor; same arguments and checks."""
+    name = "image_metrics"
+    single = pred.dim() == 3
+    if pred.dim() not in (3, 4) or pred.shape[-1] != 3:
+        raise ValueError(f"{name}: expected an (H, W, 3) or (B, H, W, 3) render, got {tuple(pred.shape)}")
+    if pred.dtype != torch.float32:
+        raise RuntimeError(f"{name}: expected a float32 render")
+    if target.dim() != pred.dim() or target.shape[:-1] != pred.shape[:-1] or target.shape[-1] not in (3, 4):
+        raise ValueError(f"{name}: the target must be the render's shape with 3 or 4 channels, got {tuple(target.shape)} "
+                         f"for {tuple(pred.shape)}")
+    if target.dtype not in (torch.uint8, torch.float32):
+        raise RuntimeError(f"{name}: expected a uint8 or float32 target")
+    H, W = int(pred.shape[-3]), int(pred.shape[-2])
+    if H < 11 or W < 11:
+        raise ValueError(f"{name}: SSIM needs an image of at least 11 x 11 pixels")
+    if not float(gamma) > 0.0 or float(gamma) == float("inf"):
+        raise ValueError(f"{name}: gamma must be positive and finite")
+    ch = int(target.shape[-1])
+    bg = None
+    if ch == 4:
+        if background is None:
+            raise ValueError(f"{name}: an RGBA target is composited over `background` (3 floats on the device)")
+        bg = background.detach().to(dtype=torch.float32).reshape(-1).contiguous()
+        if bg.numel() != 3:
+            raise ValueError(f"{name}: background must have 3 components")
+    B = 1 if single else int(pred.shape[0])
+    if B < 1:
+        raise ValueError(f"{name}: at least one image is needed")
+    _lib.require_cuda(pred, target, bg)
+    pred_c, target_c = pred.detach().contiguous().view(B, H, W, 3), target.contiguous().view(B, H, W, ch)
+    u8 = int(target_c.dtype == torch.uint8)
+    dev, lib = pred.device, _lib.load()
+    with _lib.on_device(dev):
+        out = torch.empty(3, B, dtype=torch.float32, device=dev)
+        for a in range(0, B, _EVAL_MAX_VIEWS):
+            n = min(B - a, _EVAL_MAX_VIEWS)
+            check(lib.b200_eval_metrics_views(n, H, W, ch, ptr(pred_c[a:]), ptr(target_c[a:]), u8, ptr(bg), float(gamma),
+                                              _window_taps(), ptr(out[0, a:]), ptr(out[1, a:]), ptr(out[2, a:]),
+                                              ptr(_eval_workspace(dev, n, H, W)), 1, stream()))
+    if single:
+        return out[0, 0], out[1, 0], out[2, 0]
+    return out[0], out[1], out[2]
+
+
+def image_metrics(pred: torch.Tensor, target: torch.Tensor, *, gamma: float = 2.2, background: torch.Tensor = None):
+    """(psnr, ssim) of rendered images against their ground truth, as nerfstudio's ns-eval scores a Splatfacto render
+    (get_image_metrics_and_images, splatfacto.py:1006-1042), LPIPS aside.  One kernel for the whole batch; no host sync,
+    no autograd.
+
+    pred: (H, W, 3) or (B, H, W, 3) float32, the LINEAR render; it is scored as clamp(pred, max=1) ** (1 / gamma)
+    (splatfacto.py:880; gamma = 1 scores clamp(pred, max=1)).  target: the matching ground truth, uint8 (the dataset's
+    image, / 255) or float32, with 3 or 4 channels; a 4-channel image is composited over `background` (3 floats on the
+    device) exactly as the uint8 loss prepares it (:901-923).  Returns (psnr, ssim) float32 device tensors of shape (B,),
+    0-d for a single image: psnr = torchmetrics' PeakSignalNoiseRatio(data_range=1) of each image (+inf for a perfect
+    one), ssim = pytorch_msssim.SSIM(data_range=1, size_average=True, channel=3) (:259-261).  CUDA tensors only."""
+    _, psnr, ssim_v = eval_metrics(pred, target, gamma=gamma, background=background)
+    return psnr, ssim_v

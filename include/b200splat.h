@@ -679,6 +679,27 @@ B200_API int b200_ssim_backward(unsigned img_height, unsigned img_width, unsigne
                                 float add_scale, const float *v_scale, const float *window11, float *grad,
                                 void *stream);
 
+/* ---- evaluation metrics of B views in one launch --------------------------------------------------------------------
+ * What nerfstudio's ns-eval computes per image (Splatfacto's get_image_metrics_and_images, splatfacto.py:1006-1042),
+ * LPIPS aside, for `views` images of one size:
+ *   pred_linear (views, H, W, 3) float, the LINEAR render; y = min(pred, 1)^(1/gamma) (splatfacto.py:880), with the
+ *       exponent (float)(1.0 / gamma); gamma == 1: y = min(pred, 1) exactly (no powf);
+ *   target (views, H, W, channels), uint8 (target_is_u8 = 1) or float (0; the reference's float-image branch), channels
+ *       3 or 4; prepared as b200_l1_loss_u8 prepares it with min_level 0 and no mask (its target_out, bit for bit):
+ *       uint8 / 255, RGBA composited over `background` (3 DEVICE floats, needed for channels = 4);
+ *   mse_out[v] = mean (y - t)^2 over 3 H W;  psnr_out[v] = 10 log10(1 / mse) (torchmetrics' PeakSignalNoiseRatio with
+ *       data_range 1; +inf when mse == 0);  ssim_out[v] = the b200_ssim_forward value of (y, t) with the same window11.
+ * One pass over each view's SSIM tiles; neither the prepared images nor the SSIM maps are written.  Every squared error
+ * is summed once.  ws: b200_eval_metrics_ws_bytes(views, H, W) bytes, 16-byte aligned, one ticket per view in its first
+ * 4 * views bytes (ws_is_zeroed as for b200_l1_loss: they are left zero on return).  Deterministic: each view's sums
+ * run in one fixed order, so a view's metrics do not depend on the batch it is evaluated in and repeated calls agree bit
+ * for bit.  views <= 21845 (three grid layers per view). */
+B200_API size_t b200_eval_metrics_ws_bytes(unsigned views, unsigned img_height, unsigned img_width);
+B200_API int b200_eval_metrics_views(unsigned views, unsigned img_height, unsigned img_width, unsigned channels,
+                                     const float *pred_linear, const void *target, int target_is_u8,
+                                     const float *background, float gamma, const float *window11, float *mse_out,
+                                     float *psnr_out, float *ssim_out, void *ws, int ws_is_zeroed, void *stream);
+
 /* ---- optimizer ("next" row f-2 of SURVEY section 8) ---------------------------------------------
  * One Adam update (no weight decay, no amsgrad: what nerfstudio/engine/optimizers.py:158-171 builds for every Splatfacto
  * group, eps = 1e-15) of `numel` consecutive floats of the flat {param, grad, exp_avg, exp_avg_sq} buffers:
